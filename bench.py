@@ -1,10 +1,11 @@
 #!/usr/bin/env python
 """
-bench.py  --  512^3 smoke-plume steps/s on N B200s (BASELINE.json metric), laplace / CG / stencil HBM rooflines, CPU baseline.
+bench.py  --  512^3 smoke-plume steps/s on N H100s (BASELINE.json metric), laplace / CG / stencil HBM rooflines, CPU baseline.
 
     python bench.py --gpus N --steps K --warmup W            # our arm   (N>1: launched under torch.distributed.run)
     python bench.py --impl reference --steps K --warmup W    # reference arm: the oracle port on the host cores
     python bench.py --config c2|c3|c5 ...                    # the other BASELINE configs (extra modes, same JSON contract)
+    python bench.py ... --dump-outputs DIR                   # also write the state after the last timed step as DIR/<name>.npy
 
 One "step" = incompressible_step on the whole grid (SURVEY.md section 3.3 / 8d), ONE call of the product API
 (phicuda_plume_step_f32 through phiflow_b200._ops.plume_step):
@@ -14,7 +15,6 @@ Default workload = BASELINE.json configs[3] at N GPUs ("3-D smoke plume 512^3 fp
 scaling.  Inputs are larger than L2 (every array is 512 MiB), so no L2 flush is needed between timed iterations.
 """
 import argparse
-import glob
 import json
 import os
 import sys
@@ -36,17 +36,7 @@ def load_peaks():
     path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(path):
         return float(json.load(open(path))['hbm_gbs']), 'measured'
-    return 6650.0, 'fallback'
-
-
-def load_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE launch of the CG kernel in this bench (ncu --set full capture of the
-    same command, newest profiles/r*_cg_traffic.json); None when no capture is committed."""
-    files = sorted(glob.glob(os.path.join(ROOT, 'profiles', 'r*_cg_traffic.json')))
-    try:
-        return float(json.load(open(files[-1]))['dram_bytes_per_launch'])
-    except Exception:
-        return None
+    return 3350.0, 'datasheet'           # H100 SXM HBM3
 
 
 from phiflow_b200._clocks import ClockSampler  # noqa: E402
@@ -84,12 +74,12 @@ def cpu_plume(n: int, steps: int, warmup: int):
 
 
 def reference_library_check(n: int = 64):
-    """How the port compares with the reference LIBRARY itself, run live: where baseline/_ref holds the unmodified PhiML that
+    """How the port compares with the reference LIBRARY itself, run live: where oracle/_ref holds the unmodified PhiML that
     `__graft_entry__.build()` installs, one pressure system of the plume at n^3 is solved by the oracle port's CG and by
     `phiml.backend.NUMPY.linear_solve('CG', ...)` (= PhiML/phiml/backend/_linalg.py:23-89, what the reference's NumPy path runs), and
     n^3 points are gathered by the port's grid_sample and by `phiml.math.grid_sample`.  Reports both times, the iteration counts and
     whether the results are identical - the evidence that timing the port does not flatter the GPU arm.  None when PhiML is absent."""
-    ref_dir = os.path.join(ROOT, 'baseline', '_ref')
+    ref_dir = os.path.join(ROOT, 'oracle', '_ref')
     if not os.path.isdir(os.path.join(ref_dir, 'phiml')):
         return None
     if ref_dir not in sys.path:
@@ -130,18 +120,11 @@ def reference_library_check(n: int = 64):
         t0 = time.perf_counter()
         b = math.grid_sample(gt, ct, E.ZERO_GRADIENT).numpy('points')
         t_gs_ref = time.perf_counter() - t0
-    return {"library": "PhiML 1.7.2 (unmodified, baseline/_ref), NumPy backend", "grid": n,
+    return {"library": "PhiML 1.7.2 (unmodified, oracle/_ref), NumPy backend", "grid": n,
             "cg": {"port_s": t_port, "phiml_s": t_ref, "iterations_port": int(port['iterations']),
                    "iterations_phiml": int(np.asarray(ref.iterations)[0]),
                    "bitwise_equal": bool(np.array_equal(np.asarray(ref.x)[0], port['x'].reshape(-1)))},
             "grid_sample": {"points": n ** 3, "port_s": t_gs_port, "phiml_s": t_gs_ref, "max_abs_diff": float(np.abs(a - b).max())}}
-
-
-# CG iterations per step of the SAME algorithm on the full grid, measured on the GPU by the driver (BENCH_r01.json: 512^3,
-# --steps 20 --warmup 5 -> 641.45; this round's builder runs agree to a few iterations).  The iteration count is a property
-# of the algorithm and the data (both arms run unpreconditioned CG to the same tolerance), so the CPU extrapolation uses it when
-# the step window matches instead of guessing a growth law.
-GPU_MEASURED_ITERATIONS = {(512, 5, 20): 641.45}
 
 
 def extrapolate(samples, full: int, it_full=None):
@@ -188,7 +171,7 @@ def run_reference(args):
     if int(os.environ.get('RANK', '0')) != 0:
         return
     sizes = [int(v) for v in str(args.cpu_sizes or args.cpu_size).split(',')]
-    base = cpu_report(sizes, args.steps, args.warmup, args.size, GPU_MEASURED_ITERATIONS.get((args.size, args.warmup, args.steps)))
+    base = cpu_report(sizes, args.steps, args.warmup, args.size)
     line = {"impl": "reference", "metric": METRIC, "value": base["value"], "unit": "steps/s", "n_gpus": args.gpus,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 / base["value"], "higher_is_better": True,
             "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic", "extrapolated": True,
@@ -310,6 +293,9 @@ def run_ours(args):
     torch.cuda.synchronize()
     clocks = sampler.summary()
     ms = start.elapsed_time(end) / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {'velocity_x': sim.v[0], 'velocity_y': sim.v[1], 'velocity_z': sim.v[2], 'smoke': sim.s,
+                                         'pressure': sim.p}, {'cg_iterations': res_host[-1:, 0]}, torch)
     iters = res_host[args.warmup:, 0].numpy().astype(np.int64)
     cg_ms = np.array([a.elapsed_time(b) for a, b in sim.cg_events])
     # algorithmic bytes of one solve: 30 B/cell/iteration (pass A 12 + pass B 12 / 24 alternating: the x update is applied
@@ -339,13 +325,31 @@ def run_ours(args):
                        "l2": f"inputs ({4 * n ** 3 / 2 ** 20:.0f} MiB per array) exceed L2, no flush"},
             "clocks": clocks, "gpu_launches": sim.launches_per_step * args.steps,
             "roofline": {"bound": "hbm", "kernel": "k_cg_ring<3,GENERIC=false,DIST=false> (persistent CG solve)", "achieved": cg_gbs, "peak": peak, "unit": "GB/s",
-                         "frac": cg_gbs / peak, "traffic": load_traffic(), "peak_kind": peak_kind,
+                         "frac": cg_gbs / peak, "traffic": None, "peak_kind": peak_kind,
                          "algorithmic_bytes": "cells*(30*iterations+32) per solve"},
             "laplace": lap, "kernels": kernels,
             "e2e": e2e}
     if base:
         line["cpu_baseline"] = base
     print(json.dumps(line))
+
+
+# at most 2^21 values per array (8 MiB in float32): five arrays of the 512^3 plume stay far below 64 MB
+DUMP_SAMPLE = 1 << 21
+
+
+def dump_outputs(out_dir, device_arrays, host_arrays, torch):
+    """Writes what the timed path left behind as out_dir/<name>.npy: arrays of at most DUMP_SAMPLE values whole (device layout,
+    batch first), larger ones as the flattened device array at DUMP_SAMPLE positions drawn from a fixed seed, so that two builds
+    run with the same arguments can be compared value by value."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in device_arrays.items():
+        if t.numel() > DUMP_SAMPLE:
+            idx = torch.randint(t.numel(), (DUMP_SAMPLE,), generator=torch.Generator().manual_seed(t.numel()))
+            t = t.reshape(-1)[idx.sort().values.to(t.device)]
+        np.save(os.path.join(out_dir, f'{name}.npy'), t.float().cpu().numpy())
+    for name, a in host_arrays.items():
+        np.save(os.path.join(out_dir, f'{name}.npy'), np.asarray(a, np.float64))
 
 
 def run_e2e(sim, host, args, torch):
@@ -530,9 +534,9 @@ def run_c5(args):
                                        f"dt 0.05, CG rtol=1e-3 warm start (BASELINE configs[4])",
                            "entry_steps_per_sec": per_gpu * world * 1e3 / ms, "cg_iterations_per_entry_step": float(it_mean.item()),
                            "cg_ms_per_step": float(cg_t.item()) / args.steps, "collectives_in_loop": 0,
-                           "l2": f"working set {7 * cells * 4 / 2 ** 20:.0f} MiB per GPU is L2-resident (126 MB): the HBM roofline fraction below is "
-                                 f"reported against HBM peak although most traffic is served by L2; no flush between steps by design (the "
-                                 f"workload IS a resident batch)"},
+                           "l2": f"working set {7 * cells * 4 / 2 ** 20:.0f} MiB per GPU against 50 MB of L2: the HBM roofline fraction below "
+                                 f"is reported against HBM peak although part of the traffic is served by L2; no flush between steps by design "
+                                 f"(the workload IS a resident batch)"},
                 "clocks": clocks, "gpu_launches": 4 * args.steps * world,
                 "roofline": {"bound": "hbm", "kernel": "k_cg_ring<2> (persistent CG, 64 systems per launch)", "achieved": cg_gbs, "peak": peak,
                              "unit": "GB/s", "frac": cg_gbs / peak, "traffic": None, "peak_kind": peak_kind,
@@ -556,12 +560,17 @@ def main():
     ap.add_argument('--cpu-sizes', default=None, dest='cpu_sizes', help='comma-separated sample grids of the CPU baseline (default: 96,128; add 256 for a ~6-minute third sample)')
     ap.add_argument('--no-cpu', action='store_true', dest='no_cpu')
     ap.add_argument('--halo', type=int, default=16, help='z-slab halo planes allocated per side (N>1); grows on demand')
+    ap.add_argument('--dump-outputs', default=None, dest='dump_outputs', metavar='DIR',
+                    help='plume on one GPU: write velocity, smoke, pressure (a seeded sample of large arrays) and the CG iteration count '
+                         'of the last timed step as DIR/<name>.npy')
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != 'ours' or args.config not in ('plume', 'c2', 'c4') or args.gpus > 1):
+        ap.error('--dump-outputs applies to the plume on one GPU')
     if args.config == 'c2':
         args.size = 256
     if args.impl == 'reference':
         if args.cpu_sizes is None and args.cpu_size == 96:
-            args.cpu_sizes = '96,128'          # 256^3 takes ~5 min per step: opt in with --cpu-sizes 96,128,256 (recorded: profiles/r2_cpu_samples.json)
+            args.cpu_sizes = '96,128'          # 256^3 takes ~5 min per step: opt in with --cpu-sizes 96,128,256
         return run_reference(args)
     args.warmup = max(args.warmup, 3)
     if args.cpu_sizes is None and args.cpu_size == 96:

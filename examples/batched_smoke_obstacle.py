@@ -1,4 +1,4 @@
-"""examples/grids/Batched_Smoke.ipynb on the B200 path: three inflow settings as one batch, an obstacle in the flow.
+"""examples/grids/Batched_Smoke.ipynb on the H100 path: three inflow settings as one batch, an obstacle in the flow.
 python examples/batched_smoke_obstacle.py [--res 64] [--steps 100]"""
 import argparse
 import os

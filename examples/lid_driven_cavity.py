@@ -1,4 +1,4 @@
-"""examples/grids/Lid_Driven_Cavity.ipynb on the B200 path.  python examples/lid_driven_cavity.py [--steps 300]"""
+"""examples/grids/Lid_Driven_Cavity.ipynb on the H100 path.  python examples/lid_driven_cavity.py [--steps 300]"""
 import argparse
 import os
 import sys

@@ -1,4 +1,4 @@
-"""examples/grids/Smoke_Plume.ipynb on the B200 path (cells :39-68).  python examples/smoke_plume.py [--res 128] [--steps 50] [--scene DIR]"""
+"""examples/grids/Smoke_Plume.ipynb on the H100 path (cells :39-68).  python examples/smoke_plume.py [--res 128] [--steps 50] [--scene DIR]"""
 import argparse
 import os
 import sys

@@ -1,5 +1,5 @@
 /*
- * phicuda.h  --  C ABI of libphicuda.so: the B200 (sm_100a) incompressible-fluid hot path of PhiFlow.
+ * phicuda.h  --  C ABI of libphicuda.so: the H100 (sm_90a) incompressible-fluid hot path of PhiFlow.
  *
  * Every entry point replaces one piece of the reference's Python hot path (file:line relative to the PhiFlow tree,
  * PhiML = its vendored arithmetic layer); see DESIGN.md for the data layout and INTEGRATION.md for the ctypes binding.

@@ -12,11 +12,11 @@ its CUDA library is missing instead of falling back to this file.
 Parity pinning: every function here is checked (tests/test_oracle_golden.py) against
   * the reference's own known-answer tests (SURVEY.md §4), re-expressed on raw arrays, and
   * golden fixtures tests/golden/*.npz produced by tests/golden/make_golden.py, which imports the vendored
-    `phiml.math` from /root/reference/PhiML and runs the reference's own pad / laplace / spatial_gradient /
+    `phiml.math` and runs the reference's own pad / laplace / spatial_gradient /
     grid_sample / sample_subgrid / jit_compile_linear(...).sparse_matrix / solve_linear on seeded inputs.
-  * the reference library run LIVE where it is importable (tests/test_oracle_live_phiml.py, tests/test_vector_boundaries.py: PhiML 1.7.2
-    from baseline/_ref or /root/reference/PhiML): pad / laplace / grid_sample / closest_grid_values / the staggered laplace on fresh
-    inputs, and cg() against phiml.backend.NUMPY.linear_solve - bitwise-equal iterates.
+  * more shapes and boundary mixes recorded from PhiML 1.7.2 by tests/golden/make_live_golden.py (tests/test_oracle_live_phiml.py,
+    tests/test_vector_boundaries.py): pad / laplace / grid_sample / closest_grid_values / the staggered laplace, and cg() against
+    phiml.backend.NUMPY.linear_solve - bitwise-equal iterates.
 `phi` itself (the Field layer) cannot be imported in the build container (it needs phiml>=1.14, only 1.7.2 is
 vendored), so the thin phi.field glue is restated here from the cited lines and pinned by the known-answer tests.
 

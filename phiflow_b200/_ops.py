@@ -56,7 +56,7 @@ def stored_faces(vspec, axis):
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise RuntimeError("phiflow_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback.")
+        raise RuntimeError("phiflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback.")
 
 
 def _ptr(t: Optional[torch.Tensor], off: int = 0):

@@ -31,6 +31,14 @@ bool phi_scalar_kernels()
     return v && v[0] == '1';
 }
 
+int phi_sm_count()
+{
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms > 0 ? sms : 1;
+}
+
 static int cuda_fail(int err, const char* what)
 {
     if (err > 0) phi_set_error("%s: %s", what, cudaGetErrorString((cudaError_t)err));

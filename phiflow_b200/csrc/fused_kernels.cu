@@ -664,7 +664,8 @@ int phi_launch_grid_sample(const DGrid& g, const DField& f, const float* grid, c
     const long long total = npoints * g.batch;
     if (total <= 0) return 0;
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    const long long max_blocks = (long long)phi_sm_count() * 32;
+    if (blocks > max_blocks) blocks = max_blocks;
     if (g.dim == 3) k_grid_sample<3><<<(int)blocks, 256, 0, s>>>(g, f, grid, coords, npoints, out);
     else            k_grid_sample<2><<<(int)blocks, 256, 0, s>>>(g, f, grid, coords, npoints, out);
     return (int)cudaGetLastError();

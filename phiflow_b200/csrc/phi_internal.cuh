@@ -1,4 +1,4 @@
-// Internal device-side definitions shared by all kernels of libphicuda.so (sm_100a only).
+// Internal device-side definitions shared by all kernels of libphicuda.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -333,5 +333,6 @@ int phi_make_centered(const PhiGrid* g, const PhiBC* bc, DField* out);
 int phi_make_component(const PhiGrid* g, const PhiBC* bc, int c, DField* out);
 int phi_pressure_bc(const PhiVBC* vbc, int dim, PhiBC* out);
 UnitMap phi_make_unit_map(const DGrid& g, int target_units);
+int phi_sm_count();                      // SMs of the current device
 void phi_set_error(const char* fmt, ...);
 void phi_note_launch(const PhiLaunchInfo& info);

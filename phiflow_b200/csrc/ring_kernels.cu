@@ -1,6 +1,6 @@
-// TMA-staged shared-memory ring for the 5/7-point stencil: the B200 fast path of laplace (A7) and of the CG solve (A12).
+// TMA-staged shared-memory ring for the 5/7-point stencil: the H100 fast path of laplace (A7) and of the CG solve (A12).
 //
-// Why: the stencil kernels are pure HBM streams (8..20 B/cell).  Saturating 6.5 TB/s needs ~50 KB in flight per SM; with
+// Why: the stencil kernels are pure HBM streams (8..20 B/cell).  Saturating 3.35 TB/s needs ~25 KB in flight per SM; with
 // register-staged loads that costs occupancy the CG passes do not have.  Here ONE producer warp per CTA streams whole
 // grid lines into a ring of shared-memory stages with cp.async.bulk (the TMA engine; SASS: UBLKCP) completing on
 // mbarriers, and eight consumer warps compute out of shared memory.  Loads never occupy registers, the pipeline depth
@@ -42,7 +42,7 @@ struct RingCfg {
     int dbg;                   // profiling only (PHICUDA_RING_DEBUG): 1 skip CG pass A, 2 skip pass B, 4 consumers skip the arithmetic
     // "tail split" decomposition of the CG kernel (3-D, batch 1, fewer y tiles than persistent CTAs): CTA c < nyt marches tile c
     // over planes [0, Zm); the remaining CTAs share the tails [Zm, nz) of all tiles, split_t tiles each.  Keeps every SM busy
-    // when the tile count does not divide the CTA count (128 tiles on 148 SMs for 512-wide slabs).
+    // when the tile count does not divide the CTA count (128 tiles on 132 SMs for 512-wide slabs).
     int split, Zm, split_t;
 };
 
@@ -1121,8 +1121,8 @@ k_cg_ring(CgRingArgs A)
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------------
-static const int kSmemBudget = 227 * 1024;
-// cost of starting a unit, in plane loads (512 x 512 x 64, tails of 6 planes x 7 units against one unit of 64: +5 % instead of -9 %)
+static const int kSmemBudget = 227 * 1024;           // opt-in shared memory per block on H100
+// cost of starting a unit, in plane loads (two halo planes are counted separately)
 #define RING_UNIT_OVERHEAD 2.5
 
 // lines staged per stage = lines_a * TY + lines_b; returns false when the grid lines are too long for a useful ring
@@ -1134,12 +1134,11 @@ static bool ring_config(const DGrid& g, int lines_a, int lines_b, int reserve_by
     c.consumers = consumers;
     c.pitch = g.cext[0]; c.nx4 = g.cext[0] / 4;
     const int row_bytes = c.pitch * 4;
-    // measured on B200 (512^3): TY=4 beats TY=8 for both laplace (6.12 vs 5.85 TB/s) and CG (5.18 vs 5.10 TB/s): smaller
-    // stages -> deeper ring; the extra y-halo lines are served by L2
+    // smaller stages -> deeper ring; the extra y-halo lines are served by L2 (tools/sweep_ring.py sweeps TY and the ring depth)
     int ty = g.dim == 3 ? 4 : 16;
     if (g.dim == 3) {
-        // measured (tools/sweep_ring.py, 256^3): a CTA wants >= 2048 cells per staged plane - TY=4 146 us, TY=8 114 us, TY=16 114 us
-        // per CG iteration, TY=2 538 us; the per-plane mbarrier bookkeeping is amortised over TY * nx cells.  512 -> 4, 256 -> 8, ...
+        // a CTA wants >= 2048 cells per staged plane: the per-plane mbarrier bookkeeping is amortised over TY * nx cells.
+        // 512 -> 4, 256 -> 8, ...
         const int want = 2048 / (g.cext[0] > 0 ? g.cext[0] : 1);
         ty = 1;
         while (ty * 2 <= want && ty < 16) ty *= 2;
@@ -1163,7 +1162,7 @@ static bool ring_config(const DGrid& g, int lines_a, int lines_b, int reserve_by
     { const char* e = getenv("PHICUDA_RING_DEBUG"); c.dbg = e ? atoi(e) : 0; }
     if (g.dim == 3) {
         c.nyt = (g.n[1] + c.TY - 1) / c.TY;
-        // z chunking: every unit pays two halo planes plus a pipeline start (measured: ~2.5 plane loads, RING_UNIT_OVERHEAD), and
+        // z chunking: every unit pays two halo planes plus a pipeline start (~2.5 plane loads, RING_UNIT_OVERHEAD), and
         // the persistent grid of `ctas` CTAs is only fully busy when the unit count is close to a multiple of it -> maximise
         //   utilisation(units, ctas) / (1 + (2 + overhead)/ZC)
         const int ctas = target_units;
@@ -1209,19 +1208,11 @@ static void note_ring_launch(int kernel, const RingCfg& c, bool generic, bool di
     phi_note_launch(li);
 }
 
-static int sm_count()
-{
-    int dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    return sms;
-}
-
 // returns -100 when the ring does not apply (caller falls back to the register-marching kernel)
 int phi_launch_laplace_ring(const DGrid& g, const DField& f, const float* x, float* y, float coeff, bool axpy, cudaStream_t s)
 {
     RingCfg cfg;
-    const int sms = sm_count();
+    const int sms = phi_sm_count();
     // two CTAs per SM: each gets half of the shared memory
     if (!ring_config(g, 1, 2, kSmemBudget / 2 + 1024, g.dim == 3 ? 4 : 2, 6, sms * 2, &cfg)) return -100;
     const size_t smem = 128 + (size_t)cfg.R * cfg.stage_floats * 4;
@@ -1250,7 +1241,7 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     if (mask && (l.prm.method == PHI_SOLVER_CG_ADAPTIVE || l.prm.matrix_offset != 0.f)) return -100;
     CgRingArgs A;
     const int cgs = (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128);
-    const int sms = sm_count();
+    const int sms = phi_sm_count();
     // lines staged per stage: pass B (even) = 1 haloed + 3 element-wise arrays = 4 TY + 2; with the obstacle mask as an extra
     // haloed array 5 TY + 4 (pass A: 3 haloed = 3 TY + 6)
     if (!ring_config(g, mask ? 5 : 4, mask ? 6 : 2, cgs, g.dim == 3 ? (mask ? 3 : 4) : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
@@ -1309,8 +1300,7 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     a.partials = (double*)(ws + 3 * arr);
     a.result = l.result; a.prm = l.prm;
     if (cm) A.cm = *cm; else { memset(&A.cm, 0, sizeof(A.cm)); A.cm.n = 1; A.cm.lower = A.cm.upper = -1; }
-    // measured on 2 GPUs (512 x 512 x 64 slabs): merged 138.0 us / iteration, grid.sync + block-0 send 137.3 us - no gain, so the
-    // path that was also verified on 8 GPUs stays the default; PHICUDA_COMM_MERGE=1 selects the merged barrier
+    // grid.sync + block-0 send is the default multi-GPU barrier; PHICUDA_COMM_MERGE=1 selects the merged barrier
     { const char* e = getenv("PHICUDA_COMM_MERGE"); A.comm_merge = (e && e[0] == '1') ? 1 : 0; }
     void* args[] = {&A};
     e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(threads), args, smem, s);

@@ -38,7 +38,7 @@ int phi_launch_laplace(const DGrid& g, const DField& f, const float* x, float* y
         const int e = phi_launch_laplace_ring(g, f, x, y, coeff, axpy, s);
         if (e != -100) return e;
     }
-    UnitMap um = phi_make_unit_map(g, 148 * 16);
+    UnitMap um = phi_make_unit_map(g, phi_sm_count() * 16);
     const int blocks = um.total_units;
     dim3 block(PHI_WARPS_PER_CTA * 32);
     if (g.dim == 3) {
@@ -259,9 +259,7 @@ int phi_launch_absmax(const DGrid& g, const DVec& v, float* out, cudaStream_t s)
 {
     cudaError_t e = cudaMemsetAsync(out, 0, 3 * sizeof(float), s);
     if (e != cudaSuccess) return (int)e;
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = phi_sm_count();
     if (g.dim == 3) k_absmax<3><<<sms * 8, 256, 0, s>>>(g, v, reinterpret_cast<unsigned*>(out));
     else            k_absmax<2><<<sms * 8, 256, 0, s>>>(g, v, reinterpret_cast<unsigned*>(out));
     return (int)cudaGetLastError();

@@ -1,6 +1,6 @@
 # pylint: disable-msg = wildcard-import, unused-wildcard-import, unused-import
 """
-Standard import for the B200 fast path:   from phiflow_b200.phi_cuda.flow import *      (installed into the phi tree: phi.cuda.flow)
+Standard import for the H100 fast path:   from phiflow_b200.phi_cuda.flow import *      (installed into the phi tree: phi.cuda.flow)
 
 Extends `from phi.flow import *` exactly like phi/torch/flow.py:14-35 does for PyTorch: same names, the `phicuda` backend becomes
 the default backend (unless imported inside a backend context), and the module objects `fluid`, `advect`, `field`, `diffuse` are

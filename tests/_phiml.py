@@ -1,36 +1,23 @@
 """
-Where the tests find the reference's tensor library (PhiML 1.7.2, vendored by the reference as /root/reference/PhiML).
-
-`__graft_entry__.build()` installs an unmodified copy into baseline/_ref (git-ignored, travels to the GPU box with the snapshot like
-the built .so files), so that the reference-side plugin `phiflow_b200/phi_cuda` is tested on REAL phiml objects on the GPU box too,
-where /root/reference does not exist.  The -m gpu tests only ever use baseline/_ref.
+Where the tests find the reference's tensor library (PhiML 1.7.2) for the plugin tests on real phiml objects: an installed `phiml`, or
+the unmodified copy that `__graft_entry__.build()` installs into oracle/_ref from the reference's PhiML tree
+(oracle/ref_build.py).  Without either, those tests skip.
 """
 import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-INSTALLED = os.path.join(ROOT, 'baseline', '_ref')
-VENDORED = '/root/reference/PhiML'
+INSTALLED = os.path.join(ROOT, 'oracle', '_ref')
 
 
-def phiml_path(allow_reference_tree: bool):
-    """Directory to put on sys.path, or None."""
-    if os.path.isdir(os.path.join(INSTALLED, 'phiml')):
-        return INSTALLED
-    if allow_reference_tree and os.path.isdir(os.path.join(VENDORED, 'phiml')):
-        return VENDORED
-    return None
-
-
-def ensure_phiml(allow_reference_tree: bool) -> bool:
+def ensure_phiml() -> bool:
     try:
         import phiml  # noqa: F401
         return True
     except ImportError:
         pass
-    path = phiml_path(allow_reference_tree)
-    if path is None:
+    if not os.path.isdir(os.path.join(INSTALLED, 'phiml')):
         return False
-    if path not in sys.path:
-        sys.path.insert(0, path)
+    if INSTALLED not in sys.path:
+        sys.path.insert(0, INSTALLED)
     return True

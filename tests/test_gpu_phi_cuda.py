@@ -1,6 +1,6 @@
 """
 Row B1 on the GPU: the reference-side plugin `phiflow_b200/phi_cuda` with REAL phiml objects (the unmodified PhiML 1.7.2 that
-`__graft_entry__.build()` installs into baseline/_ref - /root/reference does not exist on the GPU box) and the REAL engine
+`__graft_entry__.build()` installs into oracle/_ref, see tests/_phiml.py) and the REAL engine
 (libphicuda.so through phiflow_b200._ops).  The comparison side is the reference library itself, run live on the box's CPU:
 
   * `phiml.math.grid_sample` with the NumPy backend   vs  the same call under `with get_backend():` -> phicuda_grid_sample_f32
@@ -22,8 +22,8 @@ pytestmark = pytest.mark.gpu
 
 if not torch.cuda.is_available():
     pytest.skip('needs a CUDA device', allow_module_level=True)
-if not ensure_phiml(allow_reference_tree=False):
-    pytest.skip('PhiML not installed under baseline/_ref (run __graft_entry__.build() where /root/reference exists)',
+if not ensure_phiml():
+    pytest.skip('PhiML not available (neither installed nor in oracle/_ref)',
                 allow_module_level=True)
 
 from phiml import math  # noqa: E402

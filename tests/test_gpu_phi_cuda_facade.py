@@ -1,6 +1,6 @@
 """
 tests/test_phi_cuda_facade.py once more, with the REAL engine (libphicuda.so) behind the facade: Fields of the `phi` test double in,
-CUDA kernels in the middle, Fields out - on the GPU box, with the PhiML copy of baseline/_ref.  Same test functions, same
+CUDA kernels in the middle, Fields out - on the GPU, with PhiML installed or copied into oracle/_ref.  Same test functions, same
 assertions; only the `flow` fixture differs.
 """
 import pytest
@@ -12,8 +12,8 @@ pytestmark = pytest.mark.gpu
 
 if not torch.cuda.is_available():
     pytest.skip('needs a CUDA device', allow_module_level=True)
-if not ensure_phiml(allow_reference_tree=False):
-    pytest.skip('PhiML not installed under baseline/_ref', allow_module_level=True)
+if not ensure_phiml():
+    pytest.skip('PhiML not available (neither installed nor in oracle/_ref)', allow_module_level=True)
 
 import test_phi_cuda_facade as cpu_tests  # noqa: E402
 from test_phi_cuda_facade import (  # noqa: E402,F401

@@ -1,37 +1,22 @@
 """
-The oracle against the reference LIBRARY run live (PhiML 1.7.2 from baseline/_ref or /root/reference/PhiML) on fresh seeded inputs -
-beyond the committed fixtures of tests/golden/ (which were recorded from the same library by tests/golden/make_golden.py): every run
-of the CPU suite re-derives the comparison, for more shapes, boundary mixes and solver settings than the fixture file holds.
+The oracle against outputs of the reference LIBRARY (PhiML 1.7.2) on seeded inputs, for more shapes, boundary mixes and solver settings
+than tests/golden/phiml_golden.npz holds.  The reference side was recorded into tests/golden/phiml_live.npz by
+tests/golden/make_live_golden.py, which runs the functions below under PhiML; the inputs are regenerated here from the same seeds.
 
     O.pad / O.laplace / O.grid_sample / O.closest_grid_values     vs  phiml.math.pad / laplace / grid_sample / closest_grid_values
     O.cg / O.cg_adaptive on O.poisson_matrix                       vs  phiml.backend.NUMPY.linear_solve('CG' | 'CG-adaptive', ...)
                                                                        (= PhiML/phiml/backend/_linalg.py:23-128, unmodified)
 """
+import os
+import zlib
+
 import numpy as np
 import pytest
 
-from _phiml import ensure_phiml
-
-if not ensure_phiml(allow_reference_tree=True):
-    pytest.skip('PhiML not available (neither baseline/_ref nor the reference tree)', allow_module_level=True)
-
-from phiml import math  # noqa: E402
-from phiml.backend import NUMPY  # noqa: E402
-from phiml.math import extrapolation as E, spatial, instance, channel  # noqa: E402
-
-from oracle import oracle_np as O  # noqa: E402
+from oracle import oracle_np as O
 
 AX = 'xyz'
-
-
-def to_ext(bc):
-    """oracle boundary spec -> phiml Extrapolation"""
-    def side(s):
-        return E.PERIODIC if s == 'periodic' else E.ZERO_GRADIENT if s == 'zg' else E.ConstantExtrapolation(float(s))
-    if all(ax == bc[0] and ax[0] == ax[1] for ax in bc):
-        return side(bc[0][0])
-    return E.combine_sides(**{AX[i]: (side(lo), side(hi)) for i, (lo, hi) in enumerate(bc)})
-
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'phiml_live.npz')
 
 SCALAR_BCS = {
     'zero': lambda d: O.uniform_bc(d, 0.0), 'const': lambda d: O.uniform_bc(d, 1.5), 'open': lambda d: O.uniform_bc(d, 'zg'),
@@ -43,53 +28,57 @@ SCALAR_BCS = {
 }
 RES = {2: [(9, 7), (16, 5)], 3: [(6, 5, 7)]}
 DX = {2: (0.5, 1.25), 3: (0.5, 1.0, 2.0)}
+PAD_WIDTHS = [(1, 2), (2, 1), (1, 1)]
+NPTS = 300
 
 
-def tensor_of(a):
-    return math.tensor(a, spatial(**{AX[i]: n for i, n in enumerate(a.shape)}))
+@pytest.fixture(scope='module')
+def golden():
+    with np.load(GOLDEN) as f:
+        return dict(f)
+
+
+def pad_laplace_inputs(name, d):
+    rng = np.random.default_rng(zlib.crc32(name.encode()) % 1000 + d)
+    return [rng.standard_normal(res).astype(np.float32) for res in RES[d]]
+
+
+def grid_sample_inputs(name, d):
+    """points up to 2.5 cells outside on every side, plus the exact grid corners"""
+    rng = np.random.default_rng(7 * d + len(name))
+    res = RES[d][0]
+    g = rng.standard_normal(res).astype(np.float32)
+    pts = (rng.random((NPTS, d)) * (np.array(res) + 4.0) - 2.5).astype(np.float32)
+    pts[:d] = np.eye(d, dtype=np.float32) * (np.array(res, np.float32) - 1)
+    return g, pts
 
 
 @pytest.mark.parametrize('d', [2, 3])
 @pytest.mark.parametrize('name', sorted(SCALAR_BCS))
-def test_pad_and_laplace(name, d):
+def test_pad_and_laplace(name, d, golden):
     bc = SCALAR_BCS[name](d)
-    ext = to_ext(bc)
-    rng = np.random.default_rng(hash(name) % 1000 + d)
-    for res in RES[d]:
-        a = rng.standard_normal(res).astype(np.float32)
-        names = tuple(AX[:d])
-        widths = [(1, 2), (2, 1), (1, 1)][:d]
-        got = O.pad(a, widths, bc)
-        want = math.pad(tensor_of(a), {names[i]: w for i, w in enumerate(widths)}, ext).numpy(names)
-        np.testing.assert_array_equal(got, want)
-        lap = math.laplace(tensor_of(a), dx=math.vec(**dict(zip(names, DX[d]))), padding=ext).numpy(names)
-        np.testing.assert_array_equal(O.laplace(a, DX[d], bc), lap)
+    for i, a in enumerate(pad_laplace_inputs(name, d)):
+        np.testing.assert_array_equal(O.pad(a, PAD_WIDTHS[:d], bc), golden[f'pad/{name}/{d}/{i}'])
+        np.testing.assert_array_equal(O.laplace(a, DX[d], bc), golden[f'laplace/{name}/{d}/{i}'])
 
 
 @pytest.mark.parametrize('d', [2, 3])
 @pytest.mark.parametrize('name', sorted(SCALAR_BCS))
-def test_grid_sample_and_closest_values(name, d):
+def test_grid_sample_and_closest_values(name, d, golden):
     """PhiML/phiml/math/_ops.py:878-1015: native modes (zeros / boundary / periodic) and the pad-one-layer fallback for constants
     other than 0 and for mixed boundaries; points up to 2.5 cells outside on every side."""
     bc = SCALAR_BCS[name](d)
-    ext = to_ext(bc)
-    rng = np.random.default_rng(7 * d + len(name))
-    res = RES[d][0]
-    names = tuple(AX[:d])
-    g = rng.standard_normal(res).astype(np.float32)
-    pts = (rng.random((300, d)) * (np.array(res) + 4.0) - 2.5).astype(np.float32)
-    pts[:d] = np.eye(d, dtype=np.float32) * (np.array(res, np.float32) - 1)
-    coords = math.tensor(pts, instance(points=300) & channel(vector=','.join(names)))
-    want = math.grid_sample(tensor_of(g), coords, ext).numpy('points')
+    g, pts = grid_sample_inputs(name, d)
+    res = g.shape
+    want = golden[f'grid_sample/{name}/{d}']
     got = O.grid_sample(g, pts, bc)
     # the reference's fallback pads ONE layer, so for non-native modes it is only defined within one cell of the grid
     # (documented in math.grid_sample: "values lying further outside will not be sampled according to the extrapolation")
     native = name in ('zero', 'open', 'periodic')
     near = np.all((pts >= -1.0) & (pts <= np.array(res, np.float32)), axis=1)
-    sel = np.ones(300, bool) if native else near
+    sel = np.ones(NPTS, bool) if native else near
     np.testing.assert_allclose(got[sel], want[sel], rtol=0, atol=2e-6 * float(np.abs(g).max()))
-    close = math.closest_grid_values(tensor_of(g), coords, ext)
-    want_c = close.numpy(('points',) + tuple(f'closest_{n}' for n in names))
+    want_c = golden[f'closest/{name}/{d}']
     got_c = O.closest_grid_values(g, pts, bc)
     np.testing.assert_array_equal(got_c[sel].reshape(want_c[sel].shape), want_c[sel])
 
@@ -100,37 +89,42 @@ VEL_BCS = {
 }
 
 
-@pytest.mark.parametrize('method', ['CG', 'CG-adaptive'])
-@pytest.mark.parametrize('d', [2, 3])
-@pytest.mark.parametrize('name', sorted(VEL_BCS))
-def test_cg_iterates_equal_the_reference_solver(name, d, method):
-    """Same matrix, same right-hand side: the oracle's loop and the reference's `_linalg.cg` give the SAME iterates - bitwise-equal
-    solutions and iteration counts - for full solves, truncated solves (max_iter 1, 2, 3, 7), warm starts and the plume's loose
-    tolerance.  CG-adaptive: equal iteration counts and solutions to 2e-5 of scale, not bitwise - the reference forms the new
-    direction as r - ((r.Ad) * d) / (d.Ad), element by element (_linalg.py:122), the oracle (and the CUDA kernel, which would otherwise
-    divide per element) as r - ((r.Ad) / (d.Ad)) * d: one rounding apart per element and iteration."""
+def cg_inputs(name, d):
+    """(matrix, right-hand side, [(rtol, atol, max_iter, x0)]): full solves, truncated solves, warm starts, the plume's tolerance"""
     vbc = VEL_BCS[name](d)
     res = (12, 10) if d == 2 else (8, 6, 7)
-    dx = DX[d]
-    n = int(np.prod(res))
-    Amat = O.poisson_matrix(res, dx, O.pressure_bc(vbc))
+    Amat = O.poisson_matrix(res, DX[d], O.pressure_bc(vbc))
     rng = np.random.default_rng(11 + d)
     y = rng.standard_normal(res).astype(np.float32)
     if not O.is_flexible(vbc):
         y -= y.mean(dtype=np.float32)
     x_warm = (0.1 * rng.standard_normal(res)).astype(np.float32)
+    zero = np.zeros(res, np.float32)
+    settings = [(1e-5, 1e-5, 1000, zero), (1e-3, 1e-5, 1000, x_warm), (1e-5, 1e-5, 1, zero), (1e-5, 1e-5, 2, zero),
+                (1e-5, 1e-5, 3, x_warm), (1e-5, 1e-5, 7, zero)]
+    return Amat, y, settings
+
+
+@pytest.mark.parametrize('method', ['CG', 'CG-adaptive'])
+@pytest.mark.parametrize('d', [2, 3])
+@pytest.mark.parametrize('name', sorted(VEL_BCS))
+def test_cg_iterates_equal_the_reference_solver(name, d, method, golden):
+    """Same matrix, same right-hand side: the oracle's loop and the reference's `_linalg.cg` give the SAME iterates - bitwise-equal
+    solutions and iteration counts - for full solves, truncated solves (max_iter 1, 2, 3, 7), warm starts and the plume's loose
+    tolerance.  CG-adaptive: equal iteration counts and solutions to 2e-5 of scale, not bitwise - the reference forms the new
+    direction as r - ((r.Ad) * d) / (d.Ad), element by element (_linalg.py:122), the oracle (and the CUDA kernel, which would otherwise
+    divide per element) as r - ((r.Ad) / (d.Ad)) * d: one rounding apart per element and iteration."""
+    Amat, y, settings = cg_inputs(name, d)
     solver = O.cg if method == 'CG' else O.cg_adaptive
-    for rtol, atol, max_iter, x0 in [(1e-5, 1e-5, 1000, None), (1e-3, 1e-5, 1000, x_warm), (1e-5, 1e-5, 1, None), (1e-5, 1e-5, 2, None),
-                                     (1e-5, 1e-5, 3, x_warm), (1e-5, 1e-5, 7, None)]:
-        x0 = np.zeros(res, np.float32) if x0 is None else x0
+    for j, (rtol, atol, max_iter, x0) in enumerate(settings):
         mine = solver(Amat, y, x0, rtol, atol, max_iter, None)
-        ref = NUMPY.linear_solve(method, Amat, y.reshape(1, n), x0.reshape(1, n).copy(), np.array([rtol], np.float32), np.array([atol], np.float32),
-                                 np.array([[max_iter]]), None, None)
+        ref_x = golden[f'cg/{method}/{name}/{d}/{j}/x']
+        ref_iterations, ref_converged, ref_diverged = (int(v) for v in golden[f'cg/{method}/{name}/{d}/{j}/info'])
         if method == 'CG':
-            assert int(np.asarray(ref.iterations)[0]) == mine['iterations'], (rtol, max_iter)
-            np.testing.assert_array_equal(np.asarray(ref.x)[0], mine['x'].reshape(-1))
+            assert ref_iterations == mine['iterations'], (rtol, max_iter)
+            np.testing.assert_array_equal(ref_x, mine['x'].reshape(-1))
         else:
-            assert abs(int(np.asarray(ref.iterations)[0]) - mine['iterations']) <= 1, (rtol, max_iter)
-            scale = max(float(np.abs(np.asarray(ref.x)).max()), 1e-3)
-            np.testing.assert_allclose(mine['x'].reshape(-1), np.asarray(ref.x)[0], rtol=0, atol=2e-5 * scale + (0 if max_iter < 1000 else 20 * rtol * scale))
-        assert bool(np.asarray(ref.converged)[0]) == bool(mine['converged']) and bool(np.asarray(ref.diverged)[0]) == bool(mine['diverged'])
+            assert abs(ref_iterations - mine['iterations']) <= 1, (rtol, max_iter)
+            scale = max(float(np.abs(ref_x).max()), 1e-3)
+            np.testing.assert_allclose(mine['x'].reshape(-1), ref_x, rtol=0, atol=2e-5 * scale + (0 if max_iter < 1000 else 20 * rtol * scale))
+        assert bool(ref_converged) == bool(mine['converged']) and bool(ref_diverged) == bool(mine['diverged'])

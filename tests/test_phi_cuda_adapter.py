@@ -1,6 +1,6 @@
 """
 Reference-side adapter (phiflow_b200/phi_cuda, row B1) against REAL phiml objects from the vendored PhiML 1.7.2
-(baseline/_ref as installed by __graft_entry__.build(), else /root/reference/PhiML): boundary translation, named-dim layouts incl. the
+(an installed phiml, or oracle/_ref as installed by __graft_entry__.build()): boundary translation, named-dim layouts incl. the
 non-uniform staggered TensorStack, the eligibility matrix of SURVEY.md section 3.4, and the hot-path functions with phiml Tensors
 in and out.  There is no GPU here, so the compute engine is replaced by an oracle-backed stand-in with the SAME interface as
 phiflow_b200._ops (device arrays in, device arrays updated in place) - this file tests the plumbing around the C ABI, the
@@ -16,8 +16,8 @@ import torch
 
 from _phiml import ensure_phiml  # noqa: E402
 
-if not ensure_phiml(allow_reference_tree=True):
-    pytest.skip('PhiML not available (neither baseline/_ref nor the reference tree)', allow_module_level=True)
+if not ensure_phiml():
+    pytest.skip('PhiML not available (neither installed nor in oracle/_ref)', allow_module_level=True)
 
 from phiml import math  # noqa: E402
 from phiml.math import extrapolation as E, spatial, batch, dual, channel  # noqa: E402

@@ -15,8 +15,8 @@ import pytest
 
 from _phiml import ensure_phiml
 
-if not ensure_phiml(allow_reference_tree=True):
-    pytest.skip('PhiML not available (neither baseline/_ref nor the reference tree)', allow_module_level=True)
+if not ensure_phiml():
+    pytest.skip('PhiML not available (neither installed nor in oracle/_ref)', allow_module_level=True)
 
 from phiml import math  # noqa: E402
 from phiml import backend as phiml_backend  # noqa: E402

@@ -1,8 +1,8 @@
 """
 The GPU path a PhiFlow user has today, timed beside ours (SURVEY.md section 8(d): "also report, labelled separately, the reference
-torch-CUDA backend on the same B200 for C2"): the pressure solve of the 256^3 periodic plume (98 % of a step) through
+torch-CUDA backend on the same GPU for C2"): the pressure solve of the 256^3 periodic plume (98 % of a step) through
 
-  (a) `phiml.backend.torch.TORCH.linear_solve('CG', csr, ...)`  - the UNMODIFIED PhiML 1.7.2 from baseline/_ref; with
+  (a) `phiml.backend.torch.TORCH.linear_solve('CG', csr, ...)`  - the UNMODIFIED PhiML 1.7.2 from oracle/_ref; with
       matrix_offset=None this is its best case, the fused `torch_sparse_cg` loop (cuSPARSE SpMM + torch reductions, one host sync
       per iteration for the `while` condition; PhiML/phiml/backend/torch/_torch_backend.py:857-872, 1264-1292);
   (b) the same call with the `matrix_offset` the reference sets on periodic / closed domains (phi/physics/fluid.py:145-148) ->
@@ -27,7 +27,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-REF = os.path.join(ROOT, 'baseline', '_ref')
+REF = os.path.join(ROOT, 'oracle', '_ref')
 
 
 def timed(fn, reps, cuda):
@@ -59,7 +59,7 @@ def main():
     ap.add_argument('--no-ours', action='store_true', help='reference side only (dry run on a CPU box)')
     args = ap.parse_args()
     if not os.path.isdir(os.path.join(REF, 'phiml')):
-        print(json.dumps({"unavailable": "PhiML not installed under baseline/_ref (run __graft_entry__.build() where /root/reference exists)"}))
+        print(json.dumps({"unavailable": "PhiML not installed under oracle/_ref (run __graft_entry__.build() where the reference's PhiML tree exists, oracle/ref_build.py)"}))
         return
     sys.path.insert(0, REF)
     from oracle import oracle_np as O
@@ -96,7 +96,7 @@ def main():
             return TORCH.linear_solve('CG', lin, yt, x0, tol[0], tol[1], tol[2], None, offset)
         r, t_ref, all_ref = timed(ref_solve, args.reps, cuda)
         it_ref = int(np.asarray(r.iterations.cpu())[0])
-        out["phiml_torch"] = {"library": f"PhiML {phiml.__version__} TorchBackend (unmodified, baseline/_ref), torch {torch.__version__}", "method": r.method,
+        out["phiml_torch"] = {"library": f"PhiML {phiml.__version__} TorchBackend (unmodified, oracle/_ref), torch {torch.__version__}", "method": r.method,
                               "s_per_solve": t_ref, "all_s": all_ref, "iterations": it_ref, "us_per_iteration": 1e6 * t_ref / max(it_ref, 1),
                               "converged": bool(np.asarray(r.converged.cpu())[0])}
         x_ref = r.x[0].float().cpu().numpy()

@@ -27,6 +27,6 @@ for line in sass.splitlines():
         if re.search(pat, line):
             counts[name][col] += 1
 demangled = subprocess.run(['cu++filt'] + list(counts), capture_output=True, text=True).stdout.splitlines()
-print('# ' + ' '.join(f'{c:>8s}' for c, _ in COLS) + '  kernel   (' + os.path.relpath(lib, ROOT) + ', sm_100a)')
+print('# ' + ' '.join(f'{c:>8s}' for c, _ in COLS) + '  kernel   (' + os.path.relpath(lib, ROOT) + ', sm_90a)')
 for (mangled, c), nice in zip(counts.items(), demangled):
     print('  ' + ' '.join(f'{c[col]:8d}' for col, _ in COLS) + '  ' + (nice[:nice.index('>(') + 1] if '>(' in nice else nice.split('(')[0]).replace('(int)', '').replace('(bool)', ''))
