@@ -127,6 +127,9 @@ typedef struct PhiLaunchInfo {
     int32_t split;         /* CG ring: 1 = tail-split decomposition (CTA c < tiles marches planes [0, ZC), the rest share the tails) */
 } PhiLaunchInfo;
 int phicuda_last_launch_info(PhiLaunchInfo* out);
+/* Sweeps over the grid per iteration of this thread's most recent CG launch: 1 = one-sweep ring CG (3-D, periodic y and z,
+ * one GPU, plain CG), 2 = two-sweep kernels (every other case, or PHICUDA_CG_PASSES=2); 0 before the first CG launch. */
+int phicuda_last_cg_passes(void);
 
 /* ---- A7  field.laplace order 2 (phi/field/_field_math.py:118-145 -> PhiML/phiml/math/_nd.py:825-861) ------------- */
 /* y = sum_d (x[i-1] + x[i+1] - 2 x[i]) / dx_d^2, ghost cells from `bc`.  8 B/cell. */

@@ -60,6 +60,7 @@ PROTOTYPES = {
     'phicuda_last_error': (C.c_size_t, [C.c_char_p, C.c_size_t]),
     'phicuda_device_info': (C.c_int, [C.c_char_p, C.c_size_t, _P(C.c_int), _P(C.c_int), _P(C.c_int)]),
     'phicuda_last_launch_info': (C.c_int, [_P(PhiLaunchInfo)]),
+    'phicuda_last_cg_passes': (C.c_int, []),
     'phicuda_max_abs_velocity_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), F3, C.c_void_p, C.c_void_p]),
     'phicuda_laplace_f32': (C.c_int, [_P(PhiGrid), _P(PhiBC), C.c_void_p, C.c_void_p, C.c_void_p]),
     'phicuda_laplace_axpy_f32': (C.c_int, [_P(PhiGrid), _P(PhiBC), C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]),

@@ -325,7 +325,9 @@ def last_launch_info() -> dict:
     """Which kernel variant this thread's most recent laplace / CG launch selected (include/phicuda.h PhiLaunchInfo)."""
     info = _lib.PhiLaunchInfo()
     _lib.check(_lib.load().phicuda_last_launch_info(C.byref(info)))
-    return {k: int(getattr(info, k)) for k, _ in _lib.PhiLaunchInfo._fields_}
+    out = {k: int(getattr(info, k)) for k, _ in _lib.PhiLaunchInfo._fields_}
+    out['passes'] = int(_lib.load().phicuda_last_cg_passes())      # sweeps per CG iteration of the last CG launch
+    return out
 
 
 def _is_flexible(vspec) -> bool:

@@ -18,6 +18,8 @@ void phi_set_error(const char* fmt, ...)
 
 static thread_local PhiLaunchInfo g_last_launch = {};
 void phi_note_launch(const PhiLaunchInfo& info) { g_last_launch = info; }
+static thread_local int g_last_cg_passes = 0;
+void phi_note_cg_passes(int passes) { g_last_cg_passes = passes; }
 
 bool phi_ring_enabled()
 {
@@ -195,6 +197,8 @@ int phicuda_last_launch_info(PhiLaunchInfo* out)
     *out = g_last_launch;
     return 0;
 }
+
+int phicuda_last_cg_passes(void) { return g_last_cg_passes; }
 
 int phicuda_device_info(char* name, size_t name_len, int* sm_count, int* cc_major, int* cc_minor)
 {

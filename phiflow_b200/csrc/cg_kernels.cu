@@ -299,13 +299,13 @@ static int cg_grid_size(int dim, int batch, bool mask, int* blocks_per_sm_out)
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-// workspace layout: r | d0 | d1 | partials[2][2][batch][max_grid]
+// workspace layout: r | d0 | d1 | partials[4][2][batch][max_grid] | d2 | r1  (d2, r1 and partial slots 4..7: one-sweep ring CG)
 
 size_t phi_cg_workspace_bytes(const DGrid& g)
 {
     const size_t pf_sb = (size_t)g.cext[0] * g.cext[1] * g.cext[2];
     const size_t arr = align_up((size_t)pf_sb * g.batch * sizeof(float), 256);
-    return 3 * arr + align_up((size_t)4 * g.batch * CG_MAX_GRID * sizeof(double), 256);
+    return 5 * arr + align_up((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double), 256);
 }
 
 int phi_launch_cg(const CgLaunch& l, cudaStream_t s)
@@ -344,6 +344,7 @@ int phi_launch_cg(const CgLaunch& l, cudaStream_t s)
     cudaError_t err;
     err = cudaLaunchCooperativeKernel(cg_kernel(g.dim, mask), dim3(grid), dim3(PHI_WARPS_PER_CTA * 32), args, smem, s);
     if (err != cudaSuccess) { phi_set_error("cg: cooperative launch failed: %s", cudaGetErrorString(err)); return (int)err; }
+    phi_note_cg_passes(2);
     PhiLaunchInfo li = {}; li.kernel = PHI_KERNEL_CG_MARCH; li.generic = 1; li.masked = mask; li.total_units = a.um.total_units; li.grid_ctas = grid;
     phi_note_launch(li);
     return 0;

@@ -336,3 +336,4 @@ UnitMap phi_make_unit_map(const DGrid& g, int target_units);
 int phi_sm_count();                      // SMs of the current device
 void phi_set_error(const char* fmt, ...);
 void phi_note_launch(const PhiLaunchInfo& info);
+void phi_note_cg_passes(int passes);       // sweeps per iteration of the last CG launch (phicuda_last_cg_passes)

@@ -755,6 +755,7 @@ struct CgRingArgs {
     int ring_smem_offset;        // byte offset of the ring inside dynamic shared memory (after the CgShared block)
     int comm_merge;              // multi-GPU: 1 = merged barrier + all-reduce (comm_barrier_allreduce), 0 = grid.sync + comm_allreduce
     CommDev cm;
+    float* d2; float* r1;        // one-sweep CG: third direction buffer, second residual buffer
 };
 
 __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p)
@@ -876,8 +877,280 @@ __device__ __forceinline__ void ring_unit_cells(const RingCfg& cfg, const DGrid&
         }
 }
 
+// ---- one-sweep CG (pass F) -----------------------------------------------------------------------------------------------
+// CG needs two sweeps per iteration only because beta = |r'|^2 / |r|^2 is a global sum that must be known before d' = r' + beta d
+// can be formed.  Pass F computes that beta one step ahead instead.  Iteration k starts with r_k, d_k in memory and alpha_k,
+// beta_{k+1} known, and in ONE sweep forms, per plane,
+//   q_k = A d_k, r_{k+1} = r_k - alpha_k q_k, d_{k+1} = r_{k+1} + beta_{k+1} d_k   on the tile plus one halo line / plane,
+//   q_{k+1} = A d_{k+1}                                                        on the tile,
+// and sums d_{k+1}.q_{k+1}, |r_{k+1}|^2, r_{k+1}.q_{k+1}, |q_{k+1}|^2.  After the one grid barrier alpha_{k+1} = |r_{k+1}|^2 / d.q and
+// beta_{k+2} = (|r_{k+1}|^2 - 2 alpha r.q + alpha^2 |q|^2) / |r_{k+1}|^2 (= |r_{k+2}|^2 / |r_{k+1}|^2 in exact arithmetic).  The
+// stopping rule still uses the true |r_{k+1}|^2, and the look-ahead is rebuilt from it every iteration, so its rounding does not
+// accumulate.  Bytes per iteration: d_k, r_k read, d_{k+1}, r_{k+1} written (16 B/cell) + x += alpha_{k-1} d_{k-1} + alpha_k d_k
+// every second iteration (12 B/cell) = 22 B/cell, against 30 for the two sweeps of k_cg_ring.
+// Stage layout: d_k (TY+4 lines: halo 2 in y, because d_{k+1} is needed on the halo lines), r_k (TY+2 lines), x and d_{k-1} (TY
+// lines each, fetched on x-update iterations only).  d_{k+1} of each plane goes to a triple-buffered shared tile (TY+2 lines) from
+// which the q_{k+1} stencil takes its y and warp-edge x neighbours; consumers sync on a named barrier once per plane.
+// Only for 3-D, the branch-free tiling, periodic y and z, one GPU, CG without matrix offset or obstacles (phi_launch_cg_ring).
+#define RING_GF 3                // consumer groups per thread on the haloed (TY+2)-line region: (TY + 2) * nx4 <= RING_GF * 256
+#define FUSED_TILE_BUFS 3
+
+struct FusedGroups {
+    int t[RING_GF];             // (jj * pitch + x0): offset in the d_{k+1} tile of line jj = j + 1 (j = -1 .. TY); in the d stage + pitch
+    int tl[RING_GF], tr[RING_GF];   // tile offsets of the x-1 / x+4 neighbours of the groups that cannot take them from a shuffle
+    int goff[RING_GF];          // (jj - 1) * sy + x0: element offset of an owned (inner) group relative to (y0, x = 0) of the plane
+    unsigned valid, inner, needl, needr;    // bit k; valid and inner are warp-uniform
+};
+
+__device__ __forceinline__ void fused_groups_init(FusedGroups& fg, const RingCfg& cfg, const DGrid& g, const DField& pf)
+{
+    const int lane = threadIdx.x & 31, nx = g.n[0], pitch = cfg.pitch;
+    fg.valid = fg.inner = fg.needl = fg.needr = 0;
+#pragma unroll
+    for (int k = 0; k < RING_GF; ++k) {
+        const int ge = threadIdx.x + k * cfg.consumers;
+        const int jj = ge / cfg.nx4, x0 = (ge - jj * cfg.nx4) * 4;
+        const int row = jj * pitch;
+        if (jj < cfg.TY + 2) fg.valid |= 1u << k;
+        if (jj >= 1 && jj <= cfg.TY) fg.inner |= 1u << k;
+        fg.t[k] = row + x0;
+        fg.goff[k] = (jj - 1) * (int)pf.sy + x0;
+        fg.tl[k] = row + x0 - 1; fg.tr[k] = row + x0 + 4;
+        if (lane == 0) fg.needl |= 1u << k;
+        if (lane == 31) fg.needr |= 1u << k;
+        if (x0 == 0) { fg.needl |= 1u << k; fg.tl[k] = pf.klo[0] == PHI_BC_PERIODIC ? row + nx - 1 : row; }
+        if (x0 + 4 >= nx) { fg.needr |= 1u << k; fg.tr[k] = pf.khi[0] == PHI_BC_PERIODIC ? row : row + nx - 1; }
+        if (!(fg.needl & (1u << k))) fg.tl[k] = 0;          // broadcast address: every lane loads, the shuffled value wins
+        if (!(fg.needr & (1u << k))) fg.tr[k] = 0;
+    }
+}
+
+// Producer of pass F.  Staged line slots: d (TY+4 lines from y0-2), r (TY+2 from y0-1), x (TY), d_{k-1} (TY).  Category 0 (d) is
+// fetched on every plane of the unit, 1 (r) on planes z0-1 .. z1, 2 (x, d_{k-1}) on the owned planes of x-update iterations.
+struct ProdUnitF {
+    long long yoff[4];
+    const float* base[4];
+    uint32_t dsto[4];
+    uint32_t nbytes[4];
+    unsigned m[3];
+    int tot[3];
+};
+
+__device__ __forceinline__ void prod_fused_setup(ProdUnitF& pu, const RingCfg& cfg, const DGrid& g, const DField& pf,
+                                                 const float* d, const float* r, const float* x, const float* dprev, int b, int y0)
+{
+    const int lane = threadIdx.x & 31, TY = cfg.TY;
+    const uint32_t row_bytes = (uint32_t)cfg.pitch * 4u;
+    const bool mergeable = cfg.merge && pf.sy == cfg.pitch;
+    const int rows[4] = {TY + 4, TY + 2, TY, TY};
+    const int ylo[4] = {y0 - 2, y0 - 1, y0, y0};
+    const float* src[4] = {d, r, x, dprev};
+    int cnt[3] = {0, 0, 0};
+    pu.m[0] = pu.m[1] = pu.m[2] = 0;
+#pragma unroll
+    for (int it = 0; it < 4; ++it) {
+        const int line = lane + 32 * it;
+        pu.yoff[it] = 0; pu.base[it] = nullptr; pu.dsto[it] = 0; pu.nbytes[it] = row_bytes;
+        int key = -1, yv = 0, first = 0;
+#pragma unroll
+        for (int arr = 0; arr < 4; ++arr) {
+            if (key < 0 && line >= first && line < first + rows[arr] && src[arr]) {
+                int yy = ylo[arr] + (line - first); float cv;
+                phi_resolve(yy, pf, 1, cv);                         // periodic in y: always a stored line
+                pu.yoff[it] = (long long)b * pf.sb + (long long)yy * pf.sy;
+                pu.base[it] = src[arr];
+                pu.dsto[it] = 4u * (uint32_t)(line * cfg.pitch);
+                key = arr; yv = yy;
+            }
+            first += rows[arr];
+        }
+        cnt[0] += key == 0; cnt[1] += key == 1; cnt[2] += key >= 2;       // categories: d, r, x and d_{k-1}
+        const int pkey = __shfl_up_sync(0xffffffffu, key, 1), pyv = __shfl_up_sync(0xffffffffu, yv, 1);
+        const bool cont = mergeable && key >= 0 && lane > 0 && pkey == key && pyv + 1 == yv;
+        const unsigned cm = __ballot_sync(0xffffffffu, cont);
+        if (key >= 0 && !cont) {
+            const unsigned follow = lane == 31 ? 0u : (cm >> (lane + 1));
+            pu.nbytes[it] = (uint32_t)__ffs(~follow) * row_bytes;
+            if (key == 0) pu.m[0] |= 1u << it; else if (key == 1) pu.m[1] |= 1u << it; else pu.m[2] |= 1u << it;
+        }
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) cnt[c] += __shfl_xor_sync(0xffffffffu, cnt[c], o);
+        pu.tot[c] = cnt[c];
+    }
+}
+
+__device__ __forceinline__ void ring_produce_fused(Ring& rg, const RingCfg& cfg, const DField& pf, const ProdUnitF& pu, int z, bool rplane, bool eplane)
+{
+    const int lane = threadIdx.x & 31;
+    const int slot = rg.pos.slot;
+    const uint32_t full = rg.full0 + 8 * slot;
+    const uint32_t sbase = rg.stage0_s + 4u * (uint32_t)(slot * cfg.stage_floats);
+    float cv;
+    phi_resolve(z, pf, 2, cv);                                      // periodic in z
+    const long long zoff = (long long)z * pf.sz;
+    const unsigned mask = pu.m[0] | (rplane ? pu.m[1] : 0u) | (eplane ? pu.m[2] : 0u);
+    const int cnt = pu.tot[0] + (rplane ? pu.tot[1] : 0) + (eplane ? pu.tot[2] : 0);
+    if (lane == 0) {
+        mbar_wait(rg.empty0 + 8 * slot, rg.pos.par ^ 1u);
+        mbar_expect_tx(full, (uint32_t)cnt * (uint32_t)cfg.pitch * 4u);
+    }
+    __syncwarp();
+#pragma unroll
+    for (int it = 0; it < 4; ++it)
+        if (mask & (1u << it)) bulk_g2s(sbase + pu.dsto[it], pu.base[it] + pu.yoff[it] + zoff, pu.nbytes[it], full);
+    rg.pos.next(cfg.R);
+}
+
+__device__ __forceinline__ float4 lds4(const float* s, int off) { return *reinterpret_cast<const float4*>(s + off); }
+__device__ __forceinline__ float dot4(const float4& a, const float4& b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }
+
+// 7-point stencil of the branch-free consumer (ring_compute_fast), same operation order
+__device__ __forceinline__ float4 stencil7(const float4& c, float xl, float xr, const float4& ym, const float4& yp, const float4& zm, const float4& zp,
+                                           float ix2, float iy2, float iz2, float cc)
+{
+    float4 q;
+    q.x = fmaf(ix2, xl + c.y, fmaf(iy2, ym.x + yp.x, -cc * c.x));
+    q.y = fmaf(ix2, c.x + c.z, fmaf(iy2, ym.y + yp.y, -cc * c.y));
+    q.z = fmaf(ix2, c.y + c.w, fmaf(iy2, ym.z + yp.z, -cc * c.z));
+    q.w = fmaf(ix2, c.z + xr, fmaf(iy2, ym.w + yp.w, -cc * c.w));
+    q.x = fmaf(iz2, zm.x + zp.x, q.x);
+    q.y = fmaf(iz2, zm.y + zp.y, q.y);
+    q.z = fmaf(iz2, zm.z + zp.z, q.z);
+    q.w = fmaf(iz2, zm.w + zp.w, q.w);
+    return q;
+}
+
+struct FusedPass {
+    const float* d; const float* r; const float* dprev;    // d_k, r_k, d_{k-1}
+    float* dn; float* rn; float* x;                       // d_{k+1}, r_{k+1}, solution (x == nullptr: no x update this iteration)
+    float alpha, aprev, beta;
+};
+
+// One unit of pass F: producer warp streams planes z0-2 .. z1+1, consumers march planes p = z0-1 .. z1 (d_{k+1} on the haloed
+// region) and, one plane behind, q_{k+1} on the owned planes.  acc: d.q, |r|^2, r.q, |q|^2 of this thread.
+__device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, const DGrid& g, const DField& pf, const FusedGroups& fg,
+                                                const FusedPass& P, float* tile, const RingUnit& u, float (&acc)[4])
+{
+    const int nz = u.z1 - u.z0;
+    if ((int)threadIdx.x >= cfg.consumers) {
+        ProdUnitF pu;
+        prod_fused_setup(pu, cfg, g, pf, P.d, P.r, P.x, P.dprev, u.b, u.y0);
+        for (int p = 0; p < nz + 4; ++p)
+            ring_produce_fused(rg, cfg, pf, pu, u.z0 - 2 + p, p >= 1 && p <= nz + 2, P.x && p >= 2 && p <= nz + 1);
+        return;
+    }
+    const int pitch = cfg.pitch, TY = cfg.TY;
+    const int rb = (TY + 4) * pitch, xb = (2 * TY + 6) * pitch - pitch, pb = (3 * TY + 6) * pitch - pitch;
+    const int tsz = (TY + 2) * pitch;
+    const float ix2 = g.inv_dx2[0], iy2 = g.inv_dx2[1], iz2 = g.inv_dx2[2];
+    const float cc = 2.f * (ix2 + iy2 + iz2);
+    const float alpha = P.alpha, aprev = P.aprev, beta = P.beta;
+    long long plane_off = (long long)u.b * pf.sb + (long long)u.y0 * pf.sy + (long long)u.z0 * pf.sz - pf.sz;   // plane z0 - 1
+
+    float4 dm[RING_GF], dc[RING_GF];             // d_k on planes p-1, p (own cells of the haloed region)
+    float4 n2[RING_GF], n1[RING_GF];             // d_{k+1} on planes p-2, p-1
+    float4 r1[RING_GF];                          // r_{k+1} on plane p-1
+    SlotIt cur = rg.pos, nxt = cur; nxt.next(cfg.R);
+    ring_wait_full(rg, cur); ring_wait_full(rg, nxt);
+    {
+        const float* s0 = ring_ptr(rg, cfg, cur);
+        const float* s1 = ring_ptr(rg, cfg, nxt);
+#pragma unroll
+        for (int k = 0; k < RING_GF; ++k) {
+            dm[k] = f4_splat(0.f); dc[k] = f4_splat(0.f);
+            if (fg.valid & (1u << k)) { dm[k] = lds4(s0, pitch + fg.t[k]); dc[k] = lds4(s1, pitch + fg.t[k]); }
+            n2[k] = n1[k] = r1[k] = f4_splat(0.f);
+        }
+    }
+    ring_release(rg, cur);
+    cur = nxt; nxt.next(cfg.R);
+    for (int i = 0; i < nz + 2; ++i) {               // plane p = z0 - 1 + i
+        const bool own = i >= 1 && i <= nz;
+        ring_wait_full(rg, nxt);
+        const float* sc = ring_ptr(rg, cfg, cur);
+        const float* sn = ring_ptr(rg, cfg, nxt);
+        float* tw = tile + (i % FUSED_TILE_BUFS) * tsz;
+        float4 n0[RING_GF], r0[RING_GF];
+#pragma unroll
+        for (int k = 0; k < RING_GF; ++k) {
+            n0[k] = r0[k] = f4_splat(0.f);
+            if (!(fg.valid & (1u << k))) continue;
+            const int o = pitch + fg.t[k];
+            const float4 c = dc[k];
+            const float4 ym = lds4(sc, o - pitch), yp = lds4(sc, o + pitch), zp = lds4(sn, o);
+            float xl = __shfl_up_sync(0xffffffffu, c.w, 1), xr = __shfl_down_sync(0xffffffffu, c.x, 1);
+            const float el = sc[pitch + fg.tl[k]], er = sc[pitch + fg.tr[k]];
+            xl = (fg.needl & (1u << k)) ? el : xl;
+            xr = (fg.needr & (1u << k)) ? er : xr;
+            const float4 q = stencil7(c, xl, xr, ym, yp, dm[k], zp, ix2, iy2, iz2, cc);
+            float4 rv = lds4(sc, rb + fg.t[k]);
+            rv.x = fmaf(-alpha, q.x, rv.x); rv.y = fmaf(-alpha, q.y, rv.y); rv.z = fmaf(-alpha, q.z, rv.z); rv.w = fmaf(-alpha, q.w, rv.w);
+            const float4 dv = make_float4(fmaf(beta, c.x, rv.x), fmaf(beta, c.y, rv.y), fmaf(beta, c.z, rv.z), fmaf(beta, c.w, rv.w));
+            *reinterpret_cast<float4*>(tw + fg.t[k]) = dv;
+            if (own && (fg.inner & (1u << k))) {
+                const long long off = plane_off + fg.goff[k];
+                *reinterpret_cast<float4*>(P.rn + off) = rv;
+                *reinterpret_cast<float4*>(P.dn + off) = dv;
+                acc[1] += dot4(rv, rv);
+                if (P.x) {
+                    float4 xv = lds4(sc, xb + fg.t[k]);
+                    const float4 dp = lds4(sc, pb + fg.t[k]);
+                    xv.x += aprev * dp.x; xv.y += aprev * dp.y; xv.z += aprev * dp.z; xv.w += aprev * dp.w;
+                    xv.x += alpha * c.x; xv.y += alpha * c.y; xv.z += alpha * c.z; xv.w += alpha * c.w;
+                    *reinterpret_cast<float4*>(P.x + off) = xv;
+                }
+            }
+            n0[k] = dv; r0[k] = rv;
+            dm[k] = c; dc[k] = zp;
+        }
+        ring_release(rg, cur);
+        asm volatile("bar.sync 1, %0;" ::"r"(cfg.consumers) : "memory");      // the tile of plane p is complete
+        if (i >= 2) {                                // q_{k+1} on plane p - 1 (owned: i - 1 in 1 .. nz)
+            const float* tp = tile + ((i - 1) % FUSED_TILE_BUFS) * tsz;
+#pragma unroll
+            for (int k = 0; k < RING_GF; ++k) {
+                if (!(fg.inner & (1u << k))) continue;
+                const float4 c = n1[k];
+                const float4 ym = lds4(tp, fg.t[k] - pitch), yp = lds4(tp, fg.t[k] + pitch);
+                float xl = __shfl_up_sync(0xffffffffu, c.w, 1), xr = __shfl_down_sync(0xffffffffu, c.x, 1);
+                const float el = tp[fg.tl[k]], er = tp[fg.tr[k]];
+                xl = (fg.needl & (1u << k)) ? el : xl;
+                xr = (fg.needr & (1u << k)) ? er : xr;
+                const float4 q = stencil7(c, xl, xr, ym, yp, n2[k], n0[k], ix2, iy2, iz2, cc);
+                acc[0] += dot4(c, q);
+                acc[2] += dot4(r1[k], q);
+                acc[3] += dot4(q, q);
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < RING_GF; ++k) { n2[k] = n1[k]; n1[k] = n0[k]; r1[k] = r0[k]; }
+        cur = nxt; nxt.next(cfg.R);
+        plane_off += pf.sz;
+    }
+    ring_release(rg, cur);
+    rg.pos = nxt;
+    asm volatile("bar.sync 1, %0;" ::"r"(cfg.consumers) : "memory");          // the next unit rewrites the tile
+}
+
+// prologue of the one-sweep solve: d_0 = r_0 is stored, sums d_0.A d_0 and |A d_0|^2 (alpha_0 and beta_1)
+struct REpiFusedStart {
+    float* d; float acc0, acc1;
+    __device__ __forceinline__ void set_plane(int, int) {}
+    __device__ __forceinline__ void set_acc(const float4&) {}
+    __device__ __forceinline__ void operator()(long long off, const float4& c, const float4& q, int, const float4&, const float4&, const float4&)
+    {
+        *reinterpret_cast<float4*>(d + off) = c;
+        acc0 += dot4(c, q);
+        acc1 += dot4(q, q);
+    }
+};
+
 // MASK (N4): static obstacles - a.acc is the accessible mask, staged as an extra haloed array (always the GENERIC consumer).
-template <int DIM, bool GENERIC, bool DIST, bool ADAPT, bool MASK = false>
+// FUSED: the one-sweep iteration (pass F above) replaces passes A and B.
+template <int DIM, bool GENERIC, bool DIST, bool ADAPT, bool MASK = false, bool FUSED = false>
 __global__ void __launch_bounds__(RING_THREADS, 1)
 k_cg_ring(CgRingArgs A)
 {
@@ -985,12 +1258,110 @@ k_cg_ring(CgRingArgs A)
     if (threadIdx.x == 0) { int any = 0; for (int b = 0; b < batch; ++b) any |= sh.cont[b]; *sh.any_cont = any; }
     __syncthreads();
 
+    if constexpr (FUSED) {
+        static_assert(DIM == 3 && !GENERIC && !DIST && !ADAPT && !MASK, "the one-sweep CG is 3-D, branch-free, single-GPU CG only");
+        // d_k lives in D[k % 3], r_k in Rb[k % 2]: pass k reads d_k, r_k with halos while other CTAs write d_{k+1}, r_{k+1}, and
+        // d_{k-1} is still needed for the x update
+        float* const D[3] = {a.d0, a.d1, A.d2};
+        float* const Rb[2] = {a.r, A.r1};
+        float* const tile = rg.stage0 + (size_t)cfg.R * cfg.stage_floats;
+        FusedGroups fg;
+        fused_groups_init(fg, cfg, g, a.pf);
+        if (*sh.any_cont) {                          // d_0 = r_0; alpha_0 = |r_0|^2 / d_0.A d_0, beta_1 from |A d_0|^2
+            const float* hsrc[2] = {a.r, nullptr};
+            const float* esrc[2] = {nullptr, nullptr};
+            sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
+                REpiFusedStart epi{D[0], 0.f, 0.f};
+                ring_process_unit<false, 3, 1, 0, true>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
+                acc0 += epi.acc0; acc1 += epi.acc1;
+            });
+            barrier_and_reduce(sh.cont);
+            for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+                if (!sh.cont[b]) continue;
+                const double dl = sh.delta[b], dq = sh.sum0[b];
+                const float al = (dq != 0.0) ? (float)(dl / dq) : 0.f;
+                const double nxt = dl - 2.0 * al * dq + (double)al * al * sh.sum1[b];
+                sh.alpha[b] = al;
+                sh.beta[b] = (dl != 0.0) ? (float)(nxt / dl) : 0.f;
+            }
+            __syncthreads();
+        }
+        const int upb = cfg.split ? (int)gridDim.x : cfg.units_per_batch;
+        int reg = 1;                                 // pass F sums go to partial slots 4 reg .. 4 reg + 3; the 2-sum sweeps used 0 .. 3
+        for (int k = 0; *sh.any_cont; ++k) {
+            FusedPass P;
+            P.d = D[k % 3]; P.r = Rb[k & 1]; P.dprev = D[(k + 2) % 3];
+            P.dn = D[(k + 1) % 3]; P.rn = Rb[(k + 1) & 1]; P.x = (k & 1) ? a.x : nullptr;
+            int cur_b = cfg.split ? 0 : -1;
+            float acc[4] = {0.f, 0.f, 0.f, 0.f};
+            RingUnit u;
+            for (int j = 0; ring_next_unit<3>(cfg, g, j, u); ++j) {
+                if (!sh.cont[u.b]) continue;
+                if (u.b != cur_b) {
+                    if (cur_b >= 0) { flush_partials(sh, a.partials, 2 * reg, batch, cur_b, acc[0], acc[1]);
+                                      flush_partials(sh, a.partials, 2 * reg + 1, batch, cur_b, acc[2], acc[3]); }
+                    cur_b = u.b; acc[0] = acc[1] = acc[2] = acc[3] = 0.f;
+                }
+                P.alpha = sh.alpha[u.b]; P.aprev = sh.aprev[u.b]; P.beta = sh.beta[u.b];
+                ring_fused_unit(rg, cfg, g, a.pf, fg, P, tile, u, acc);
+            }
+            if (cur_b >= 0) { flush_partials(sh, a.partials, 2 * reg, batch, cur_b, acc[0], acc[1]);
+                              flush_partials(sh, a.partials, 2 * reg + 1, batch, cur_b, acc[2], acc[3]); }
+            fence_proxy_async();
+            grid.sync();
+            fence_proxy_async();
+            reduce_partials(sh, a.partials, 2 * reg, batch, upb, sh.cont);
+            for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+                if (!sh.cont[b]) continue;
+                const double dn = sh.sum1[b], dq = sh.sum0[b];
+                sh.delta[b] = dn;
+                const int it = ++sh.iters[b];
+                const float rsq = fabsf((float)dn);
+                const bool conv = rsq <= sh.tol_sq[b];
+                const bool divg = !isfinite(rsq) || (rsq / sh.rsq0[b] > 1e5f && it >= 8);
+                sh.conv[b] = conv; sh.divg[b] = divg;
+                sh.cont[b] = (!conv && !divg && it < a.prm.max_iter) ? 1 : 0;
+                if (sh.cont[b]) {                    // an entry that stops keeps alpha_k: the x step it may still owe
+                    sh.aprev[b] = sh.alpha[b];
+                    sh.alpha[b] = (dq != 0.0) ? (float)(dn / dq) : 0.f;
+                }
+            }
+            __syncthreads();
+            reduce_partials(sh, a.partials, 2 * reg + 1, batch, upb, sh.cont);
+            for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+                if (!sh.cont[b]) continue;
+                const double dn = sh.delta[b], al = sh.alpha[b];
+                const double nxt = dn - 2.0 * al * sh.sum0[b] + al * al * sh.sum1[b];
+                sh.beta[b] = (dn != 0.0) ? (float)(nxt / dn) : 0.f;
+            }
+            __syncthreads();
+            if (threadIdx.x == 0) { int any = 0; for (int b = 0; b < batch; ++b) any |= sh.cont[b]; *sh.any_cont = any; }
+            __syncthreads();
+            reg ^= 1;
+        }
+        region = reg == 1 ? 2 : 0;                   // 2-sum slots that the last pass F did not use
+        // entries that stopped after an odd number of iterations still owe x the step alpha_k d_k of their last pass k
+        RingUnit u;
+        for (int k = 0; ring_next_unit<DIM>(cfg, g, k, u); ++k) {
+            const int it = sh.iters[u.b];
+            if (!(it & 1)) continue;
+            const float al = sh.alpha[u.b];
+            const float* dl = D[(it - 1) % 3];
+            ring_unit_cells<DIM>(cfg, g, a.pf, tg, u, [&](long long off, int) {
+                float4 xv = *reinterpret_cast<const float4*>(a.x + off);
+                const float4 dv = *reinterpret_cast<const float4*>(dl + off);
+                xv.x += al * dv.x; xv.y += al * dv.y; xv.z += al * dv.z; xv.w += al * dv.w;
+                *reinterpret_cast<float4*>(a.x + off) = xv;
+            });
+        }
+    }
+
     // a.prm.method == PHI_SOLVER_CG_ADAPTIVE (_linalg.py:93-128) reuses both passes: pass A forms d' = r - c d (beta = -c) and
     // sums d'.Ad' and d'.r, pass B applies the step (d'.r)/(d'.Ad') and sums |r|^2 and r.Ad' for the next c.
     float* dold = a.d0; float* dnew = a.d1;
     float* lo_dnew = cm.lo_d1; float* hi_dnew = cm.hi_d1; float* lo_dold = cm.lo_d0; float* hi_dold = cm.hi_d0;
     bool x_pending = false;      // all running entries are at the same iteration, so one flag describes them all
-    while (*sh.any_cont && comm_ok) {
+    while (!FUSED && *sh.any_cont && comm_ok) {
         if (cfg.dbg & 1) {} else if constexpr (!ADAPT) {   // pass A
             const float* hsrc[3] = {a.r, dold, MASK ? a.acc : nullptr};
             const float* esrc[2] = {nullptr, nullptr};
@@ -1081,7 +1452,7 @@ k_cg_ring(CgRingArgs A)
 
     // entries that stopped after an odd number of iterations still owe x their last step; odd iterations write d1
     RingUnit u;
-    for (int k = 0; ring_next_unit<DIM>(cfg, g, k, u); ++k) {
+    for (int k = 0; !FUSED && ring_next_unit<DIM>(cfg, g, k, u); ++k) {
         if (!(sh.iters[u.b] & 1)) continue;
         const float al = sh.alpha[u.b];
         ring_unit_cells<DIM>(cfg, g, a.pf, tg, u, [&](long long off, int nvalid) {
@@ -1126,8 +1497,9 @@ static const int kSmemBudget = 227 * 1024;           // opt-in shared memory per
 #define RING_UNIT_OVERHEAD 2.5
 
 // lines staged per stage = lines_a * TY + lines_b; returns false when the grid lines are too long for a useful ring
+// zhalo: halo planes a unit stages in z besides its own (2 for the stencil, 4 for the one-sweep CG)
 static bool ring_config(const DGrid& g, int lines_a, int lines_b, int reserve_bytes, int min_stages, int max_stages,
-                        int target_units, RingCfg* out, int consumers = RING_CONSUMERS)
+                        int target_units, RingCfg* out, int consumers = RING_CONSUMERS, int zhalo = 2)
 {
     RingCfg c;
     c.split = 0; c.Zm = 0; c.split_t = 0;
@@ -1174,7 +1546,7 @@ static bool ring_config(const DGrid& g, int lines_a, int lines_b, int reserve_by
             const long long units = (long long)c.nyt * nzc * g.batch;
             const long long rounds = (units + ctas - 1) / ctas;
             const double util = (double)units / (double)(rounds * ctas);
-            const double score = util / (1.0 + (2.0 + RING_UNIT_OVERHEAD) / zc);
+            const double score = util / (1.0 + (zhalo + RING_UNIT_OVERHEAD) / zc);
             if (score > best + 1e-9) { best = score; best_nzc = nzc; }
         }
         if (const char* e = getenv("PHICUDA_RING_NZC")) {                     // tuning knob
@@ -1247,18 +1619,39 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     if (!ring_config(g, mask ? 5 : 4, mask ? 6 : 2, cgs, g.dim == 3 ? (mask ? 3 : 4) : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
     const int threads = RING_THREADS;
     A.ring_smem_offset = cgs;
-    const size_t smem = (size_t)cgs + 128 + (size_t)A.cfg.R * A.cfg.stage_floats * 4;
     int per_sm = 0;
     cudaError_t e;
     const bool generic = mask || !ring_all_fast(g, l.pf, A.cfg);
     const bool dist = cm && cm->n > 1;
     const bool adapt = l.prm.method == PHI_SOLVER_CG_ADAPTIVE;
+    // one-sweep CG (pass F): 3-D, branch-free tiling, periodic y and z, one GPU, plain CG without matrix offset or obstacles.
+    // PHICUDA_CG_PASSES=2 forces the two-sweep kernel (A/B timing, tools/cg_passes_bench.py).
+    bool fused = false;
+    size_t tile_bytes = 0;
+    {
+        const char* e = getenv("PHICUDA_CG_PASSES");
+        const DField& pf = l.pf;
+        if (!(e && atoi(e) == 2) && g.dim == 3 && !generic && !dist && !adapt && !mask && l.prm.matrix_offset == 0.f
+            && pf.klo[1] == PHI_BC_PERIODIC && pf.khi[1] == PHI_BC_PERIODIC && pf.klo[2] == PHI_BC_PERIODIC && pf.khi[2] == PHI_BC_PERIODIC) {
+            // stage = d (TY+4) + r (TY+2) + x (TY) + d_{k-1} (TY) lines; the d_{k+1} tile is reserved at the largest TY ring_config may pick
+            RingCfg fc;
+            if (ring_config(g, 4, 6, cgs, 4, RING_MAX_STAGES, sms, &fc, RING_CONSUMERS, 4)
+                && ring_config(g, 4, 6, cgs + FUSED_TILE_BUFS * (fc.TY + 2) * fc.pitch * 4, 4, RING_MAX_STAGES, sms, &fc, RING_CONSUMERS, 4)
+                && ring_all_fast(g, pf, fc) && (fc.TY + 2) * fc.nx4 <= RING_GF * fc.consumers) {
+                fused = true;
+                A.cfg = fc;
+                tile_bytes = (size_t)FUSED_TILE_BUFS * (fc.TY + 2) * fc.pitch * 4;
+            }
+        }
+    }
+    const size_t smem = (size_t)cgs + 128 + (size_t)A.cfg.R * A.cfg.stage_floats * 4 + tile_bytes;
 #define CG_RING_FN2(D, GEN, DI) (adapt ? (const void*)k_cg_ring<D, GEN, DI, true> : (const void*)k_cg_ring<D, GEN, DI, false>)
 #define CG_RING_FN(D, GEN) (dist ? CG_RING_FN2(D, GEN, true) : CG_RING_FN2(D, GEN, false))
     const void* fn = g.dim == 3 ? (generic ? CG_RING_FN(3, true) : CG_RING_FN(3, false))
                                 : (generic ? CG_RING_FN(2, true) : CG_RING_FN(2, false));
     if (mask) fn = g.dim == 3 ? (dist ? (const void*)k_cg_ring<3, true, true, false, true> : (const void*)k_cg_ring<3, true, false, false, true>)
                               : (dist ? (const void*)k_cg_ring<2, true, true, false, true> : (const void*)k_cg_ring<2, true, false, false, true>);
+    if (fused) fn = (const void*)k_cg_ring<3, false, false, false, false, true>;
 #undef CG_RING_FN
 #undef CG_RING_FN2
     e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -1271,16 +1664,17 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
         const char* e = getenv("PHICUDA_RING_SPLIT");                       // tuning knob: 0 = never, 1 = whenever possible
         const int force = e ? atoi(e) : -1;
         const int nyt = A.cfg.nyt, nz = g.n[2];
+        const int zh = fused ? 4 : 2;                                         // z halo planes staged per unit
         if (g.dim == 3 && g.batch == 1 && force != 0 && grid <= CG_MAX_GRID && nyt < grid && nz >= 8) {
             const int spare = grid - nyt, T = (nyt + spare - 1) / spare;
             int best_zm = 0; double best = 1e30;
             for (int zm = 4; zm <= nz - 1; ++zm) {
-                const double main_c = zm + 2 + RING_UNIT_OVERHEAD, tail_c = T * (nz - zm + 2 + RING_UNIT_OVERHEAD);
+                const double main_c = zm + zh + RING_UNIT_OVERHEAD, tail_c = T * (nz - zm + zh + RING_UNIT_OVERHEAD);
                 const double cost = main_c > tail_c ? main_c : tail_c;
                 if (cost < best) { best = cost; best_zm = zm; }
             }
             const long long rounds = ((long long)A.cfg.total_units + grid - 1) / grid;
-            const double dflt = rounds * (A.cfg.ZC + 2 + RING_UNIT_OVERHEAD);
+            const double dflt = rounds * (A.cfg.ZC + zh + RING_UNIT_OVERHEAD);
             if (best_zm > 0 && (force == 1 || best < dflt * 0.97)) {
                 A.cfg.split = 1; A.cfg.Zm = best_zm; A.cfg.split_t = T;
                 A.cfg.nzc = 2; A.cfg.ZC = best_zm; A.cfg.units_per_batch = A.cfg.total_units = 2 * nyt;
@@ -1298,6 +1692,8 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     const size_t hoff = (size_t)g.halo * g.cext[0] * g.cext[1];       // pointers address the first owned plane
     a.r = (float*)ws + hoff; a.d0 = (float*)(ws + arr) + hoff; a.d1 = (float*)(ws + 2 * arr) + hoff;
     a.partials = (double*)(ws + 3 * arr);
+    const size_t pbytes = ((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double) + 255) / 256 * 256;
+    A.d2 = (float*)(ws + 3 * arr + pbytes) + hoff; A.r1 = (float*)(ws + 4 * arr + pbytes) + hoff;
     a.result = l.result; a.prm = l.prm;
     if (cm) A.cm = *cm; else { memset(&A.cm, 0, sizeof(A.cm)); A.cm.n = 1; A.cm.lower = A.cm.upper = -1; }
     // grid.sync + block-0 send is the default multi-GPU barrier; PHICUDA_COMM_MERGE=1 selects the merged barrier
@@ -1306,5 +1702,6 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(threads), args, smem, s);
     if (e != cudaSuccess) { phi_set_error("cg ring: cooperative launch failed: %s", cudaGetErrorString(e)); return (int)e; }
     note_ring_launch(PHI_KERNEL_CG_RING, A.cfg, generic, dist, adapt, grid, mask);
+    phi_note_cg_passes(fused ? 1 : 2);
     return 0;
 }
