@@ -208,6 +208,21 @@ int phicuda_cg_poisson_dist_f32(const PhiGrid* g, const PhiVBC* vbc, const float
 int phicuda_cg_poisson_dist_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const float* rhs, float* x, const float* accessible,
                                        const PhiCgParams* prm, PhiCgResult* result, PhiComm* comm, void* stream);
 
+/* ---- N5  diffuse.implicit (phi/physics/diffuse.py:63-95) ---------------------------------------------------------------
+ * Solves sharpen(x) = x - amount * laplace_bc(x) = y with CG, amount = diffusivity * dt, as the reference's solve_linear does:
+ * M x = y - bias, M = I - amount * L0 (L0: laplace with every constant ghost 0), bias = sharpen(0)
+ * (PhiML/phiml/math/_optimize.py:616-645).  Same persistent TMA-ring CG as the pressure solve (two sweeps per iteration,
+ * phicuda_last_cg_passes() reports 2), single GPU, no z-slabs.
+ * components = C in {1, 2, 3}: batch entry b is component b % C of a vector field (a CenteredGrid with a vector channel, or the
+ * components of a periodic StaggeredGrid) and uses bc->comp[b % C] (kinds must agree, constants may differ).  Every entry is its
+ * own system with its own stopping rule: the reference's tracer keeps the uncoupled vector dim out of the matrix and solves the
+ * components as a batch.  x: in = x0, out = solution; x == y is allowed (the reference's default x0 is the field itself).
+ * prm: method PHI_SOLVER_CG, balance_rhs = project_mean = 0, matrix_offset = 0.  result: `batch` records.
+ * workspace: phicuda_cg_workspace_bytes(g).  Grids whose lines do not fit the ring return PHI_ERR_UNSUPPORTED. */
+int phicuda_diffuse_implicit_f32(const PhiGrid* g, const PhiVBC* bc, int32_t components, float amount,
+                                 const float* y, float* x, const PhiCgParams* prm, PhiCgResult* result,
+                                 void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- A1  fluid.make_incompressible (phi/physics/fluid.py:94-162), no obstacles, order 2, staggered ------------------
  * div scratch: one centred array.  Equivalent to divergence + cg_poisson + grad_sub on the same stream. */
 int phicuda_make_incompressible_f32(const PhiGrid* g, const PhiVBC* vbc, float* const v[3], float* p, float* div,

@@ -76,6 +76,8 @@ PROTOTYPES = {
     'phicuda_cg_workspace_bytes': (C.c_size_t, [_P(PhiGrid)]),
     'phicuda_cg_poisson_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), C.c_void_p, C.c_void_p, _P(PhiCgParams), C.c_void_p,
                                          C.c_void_p, C.c_size_t, C.c_void_p]),
+    'phicuda_diffuse_implicit_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), C.c_int32, C.c_float, C.c_void_p, C.c_void_p, _P(PhiCgParams),
+                                               C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     'phicuda_make_incompressible_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), F3, C.c_void_p, C.c_void_p, _P(PhiCgParams),
                                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     'phicuda_divergence_masked_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), F3, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -121,8 +121,13 @@ class Domain:
         if self._ws is None:
             n = _lib.load().phicuda_cg_workspace_bytes(C.byref(self.grid))
             self._ws = torch.zeros(n, dtype=torch.uint8, device=self.device)
+        return self._ws, self.results()
+
+    def results(self):
+        """Device buffer of one PhiCgResult per batch entry (what read_results returns)."""
+        if self._result is None:
             self._result = torch.zeros(self.batch * 6, dtype=torch.int32, device=self.device)
-        return self._ws, self._result
+        return self._result
 
     def scratch(self):
         if self._scratch is None:
@@ -348,10 +353,11 @@ def cg_params(vbc, rtol=1e-5, atol=1e-5, max_iter=1000, matrix_offset=0.0, balan
     return prm
 
 
-def read_results(dom: Domain) -> np.ndarray:
-    """Synchronises and returns the per-batch solve results as a structured array."""
-    _, res = dom.workspace()
-    return res.cpu().numpy().view(_RESULT_DTYPE)
+def read_results(dom: Domain, components: int = 1) -> np.ndarray:
+    """Synchronises and returns the per-batch solve results as a structured array.  components = C > 1: the records of the last
+    diffuse_implicit of C components on `dom`, one per (batch entry, component), entry b * C + c."""
+    d = dom if components == 1 else dom._stacked[components]
+    return d.results().cpu().numpy().view(_RESULT_DTYPE)
 
 
 def cg_poisson(dom: Domain, vbc, rhs, x0=None, prm: PhiCgParams = None):
@@ -363,6 +369,43 @@ def cg_poisson(dom: Domain, vbc, rhs, x0=None, prm: PhiCgParams = None):
     _lib.check(_lib.load().phicuda_cg_poisson_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _ptr(rhs, dom.coff), _ptr(x, dom.coff), C.byref(prm),
                                                   _ptr(res), _ptr(ws), C.c_size_t(ws.numel()), _stream()))
     return x
+
+
+def diffuse_implicit(dom: Domain, spec, u, amount: float, rtol=1e-5, atol=1e-5, max_iter=1000, x0=None):
+    """diffuse.implicit (phi/physics/diffuse.py:63-95): solves x - amount * laplace(x) = u with CG, amount = diffusivity * dt.
+    u: a centred array with boundary spec `spec`, or a list of C <= 3 same-shaped component arrays (a vector CenteredGrid, or the
+    components of a periodic StaggeredGrid) with one spec or a list of per-component specs.  Every component of every batch entry is
+    its own system, as in the reference (its tracer keeps the uncoupled vector dim out of the matrix).  x0: start value of the same
+    form, default u (diffuse.py:93-94).  Returns new arrays in the form of u; the inputs are not modified.
+    read_results(dom, components=C) then holds one record per system, entry b * C + c = component c of batch entry b."""
+    require_cuda()
+    comps = list(u) if isinstance(u, (list, tuple)) else [u]
+    n = len(comps)
+    assert 1 <= n <= 3 and all(c.shape == comps[0].shape for c in comps), "1 to 3 components of the same shape"
+    assert dom.halo == 0, "implicit diffusion is not offered on z-slabs"
+    if n == 1:
+        sdom, y = dom, comps[0]
+    else:                                   # entry s * n + c = component c of system s
+        cache = dom.__dict__.setdefault('_stacked', {})
+        if n not in cache:
+            cache[n] = Domain(dom.res, dom.dx, dom.batch * n, device=dom.device)
+        sdom = cache[n]
+        y = torch.stack(comps, 1).reshape((dom.batch * n,) + tuple(comps[0].shape[1:]))
+    if x0 is None:
+        x = y.clone()
+    else:
+        x0s = list(x0) if isinstance(x0, (list, tuple)) else [x0]
+        x = x0s[0].clone() if n == 1 else torch.stack(x0s, 1).reshape(y.shape)
+    ws, _ = sdom.workspace()
+    prm = PhiCgParams()                     # plain CG; I - amount * L is not singular: no balancing, projection or offset
+    prm.rtol, prm.atol, prm.max_iter = rtol, atol, int(max_iter)
+    _lib.check(_lib.load().phicuda_diffuse_implicit_f32(C.byref(sdom.grid), C.byref(make_vbc(spec, n)), C.c_int32(n), C.c_float(amount),
+                                                        _ptr(y), _ptr(x), C.byref(prm), _ptr(sdom.results()), _ptr(ws), C.c_size_t(ws.numel()),
+                                                        _stream()))
+    if n == 1:
+        return x if not isinstance(u, (list, tuple)) else [x]
+    x = x.reshape((dom.batch, n) + tuple(comps[0].shape[1:]))
+    return [x[:, c].clone() for c in range(n)]
 
 
 def mul_faces(dom: Domain, vbc, v, mask):

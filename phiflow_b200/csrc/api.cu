@@ -1,4 +1,5 @@
 // C ABI of libphicuda.so (declared in include/phicuda.h): argument validation, descriptor construction, launch order.
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -413,6 +414,44 @@ int phicuda_cg_poisson_f32(const PhiGrid* g, const PhiVBC* vbc, const float* rhs
     CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &l.pf));
     l.rhs = rhs; l.x = x; l.prm = *prm; l.result = result; l.workspace = workspace; l.workspace_bytes = workspace_bytes;
     return phi_launch_cg(l, (cudaStream_t)stream);
+}
+
+int phicuda_diffuse_implicit_f32(const PhiGrid* g, const PhiVBC* bc, int32_t components, float amount, const float* y, float* x,
+                                 const PhiCgParams* prm, PhiCgResult* result, void* workspace, size_t workspace_bytes, void* stream)
+{
+    // every check runs before the first CUDA call
+    CgLaunch l; DField cf[3];
+    CHECK(phi_make_dgrid(g, &l.g));
+    if (!bc || !y || !x || !prm || !result || !workspace) { phi_set_error("diffuse_implicit: NULL argument"); return PHI_ERR_INVALID; }
+    if (components < 1 || components > 3) { phi_set_error("diffuse_implicit: components must be 1, 2 or 3, got %d", components); return PHI_ERR_INVALID; }
+    if (g->batch % components != 0) { phi_set_error("diffuse_implicit: batch %d is not a multiple of components %d", g->batch, components); return PHI_ERR_INVALID; }
+    if (!std::isfinite(amount)) { phi_set_error("diffuse_implicit: amount is not finite"); return PHI_ERR_INVALID; }
+    if (prm->method != PHI_SOLVER_CG) { phi_set_error("diffuse_implicit: only PHI_SOLVER_CG (the reference's Solve('CG'))"); return PHI_ERR_UNSUPPORTED; }
+    if (prm->balance_rhs || prm->project_mean || prm->matrix_offset != 0.f) {
+        phi_set_error("diffuse_implicit: I - a L is not singular - balance_rhs, project_mean and matrix_offset must be 0"); return PHI_ERR_INVALID;
+    }
+    if (g->halo != 0) { phi_set_error("diffuse_implicit: z-slab grids are not supported"); return PHI_ERR_UNSUPPORTED; }
+    for (int c = 0; c < components; ++c) {
+        CHECK(phi_make_centered(g, &bc->comp[c], &cf[c]));
+        for (int a = 0; a < g->dim; ++a)
+            if (bc->comp[c].lo[a] != bc->comp[0].lo[a] || bc->comp[c].hi[a] != bc->comp[0].hi[a]) {
+                phi_set_error("diffuse_implicit: boundary kinds must agree between components (axis %d)", a); return PHI_ERR_UNSUPPORTED;
+            }
+    }
+    if (workspace_bytes < phi_cg_workspace_bytes(l.g)) { phi_set_error("diffuse_implicit: workspace %zu < %zu bytes", workspace_bytes, phi_cg_workspace_bytes(l.g)); return PHI_ERR_WORKSPACE; }
+    if (!phi_ring_enabled() || !phi_cg_ring_fits(l.g)) {
+        phi_set_error("diffuse_implicit: the grid does not fit the TMA-ring CG (batch <= 1024, grid lines short enough); this operator has no other kernel");
+        return PHI_ERR_UNSUPPORTED;
+    }
+    PhiBC zero = bc->comp[0];                                    // L0: the operator sees the kinds, the constants go into the bias
+    for (int a = 0; a < 3; ++a) { zero.clo[a] = 0.f; zero.chi[a] = 0.f; }
+    CHECK(phi_make_centered(g, &zero, &l.pf));
+    for (int c = components; c < 3; ++c) cf[c] = l.pf;
+    l.rhs = y; l.x = x; l.prm = *prm; l.result = result; l.workspace = workspace; l.workspace_bytes = workspace_bytes;
+    l.helm = true; l.helm_amount = amount;
+    const int e = phi_launch_diffuse_implicit(l, components, cf, (cudaStream_t)stream);
+    if (e == -100) { phi_set_error("diffuse_implicit: the grid does not fit the TMA-ring CG on this device"); return PHI_ERR_UNSUPPORTED; }
+    return cuda_fail(e, "diffuse_implicit");
 }
 
 // div -> CG -> v = vin - grad p.  vin/vout may be the same arrays (make_incompressible) or scratch -> state (fused step).

@@ -41,6 +41,8 @@ struct CgLaunch {
     PhiCgParams prm; PhiCgResult* result;
     void* workspace; size_t workspace_bytes;
     const float* acc = nullptr;    // N4: accessible mask
+    bool helm = false;             // N5 diffuse.implicit: operator I - helm_amount * L instead of L (pf carries L0: constants zeroed)
+    float helm_amount = 0.f;
 };
 size_t phi_cg_workspace_bytes(const DGrid& g);
 // TMA ring fast paths (ring_kernels.cu); return -100 when the shape does not fit and the caller must fall back
@@ -59,3 +61,7 @@ struct CommDev {                      // device view of the multi-GPU communicat
 int phi_launch_cg_ring(const CgLaunch& a, const CommDev* cm, cudaStream_t s);
 bool phi_ring_enabled();
 int phi_launch_cg(const CgLaunch& a, cudaStream_t s);
+// N5 diffuse.implicit on the ring CG (ring_kernels.cu): host-only fit test, and the solve (bias pre-pass + k_cg_ring<..., HELM>);
+// cf[c] = boundary with constants of component c (batch entry b is component b % C).  -100: the grid does not fit the ring.
+bool phi_cg_ring_fits(const DGrid& g);
+int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField cf[3], cudaStream_t s);

@@ -729,6 +729,20 @@ struct REpiPassB {
     }
 };
 
+// diffuse.implicit (N5): the stencil result q = L0 c of the value c becomes M c = c - a L0 c right before the wrapped epilogue,
+// so the residual sweep and both CG passes (d.Md, r -= alpha Md) see the Helmholtz operator M = I - a L0.
+template <class Epi>
+struct REpiHelm {
+    Epi& e; float a;
+    __device__ __forceinline__ void set_plane(int z, int nz) { e.set_plane(z, nz); }
+    __device__ __forceinline__ void set_acc(const float4& m) { e.set_acc(m); }
+    __device__ __forceinline__ void operator()(long long off, const float4& c, const float4& q, int nvalid, const float4& e0, const float4& e1, const float4& e2)
+    {
+        const float4 m = make_float4(fmaf(-a, q.x, c.x), fmaf(-a, q.y, c.y), fmaf(-a, q.z, c.z), fmaf(-a, q.w, c.w));
+        e(off, c, m, nvalid, e0, e1, e2);
+    }
+};
+
 // ---- laplace -----------------------------------------------------------------------------------------------------------
 template <int DIM, bool AXPY, bool GENERIC>
 __global__ void __launch_bounds__(RING_THREADS, 2)
@@ -756,6 +770,7 @@ struct CgRingArgs {
     int comm_merge;              // multi-GPU: 1 = merged barrier + all-reduce (comm_barrier_allreduce), 0 = grid.sync + comm_allreduce
     CommDev cm;
     float* d2; float* r1;        // one-sweep CG: third direction buffer, second residual buffer
+    float helm_a;                // HELM (diffuse.implicit): operator I - helm_a * L0
 };
 
 __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p)
@@ -1150,10 +1165,12 @@ struct REpiFusedStart {
 
 // MASK (N4): static obstacles - a.acc is the accessible mask, staged as an extra haloed array (always the GENERIC consumer).
 // FUSED: the one-sweep iteration (pass F above) replaces passes A and B.
-template <int DIM, bool GENERIC, bool DIST, bool ADAPT, bool MASK = false, bool FUSED = false>
+// HELM (N5, diffuse.implicit): two-sweep CG on M = I - A.helm_a * L0 (REpiHelm); every batch entry is its own system.
+template <int DIM, bool GENERIC, bool DIST, bool ADAPT, bool MASK = false, bool FUSED = false, bool HELM = false>
 __global__ void __launch_bounds__(RING_THREADS, 1)
 k_cg_ring(CgRingArgs A)
 {
+    static_assert(!HELM || (!DIST && !ADAPT && !MASK && !FUSED), "the Helmholtz operator runs on the single-GPU two-sweep CG only");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const CgArgs& a = A.a;
     const RingCfg& cfg = A.cfg;
@@ -1238,7 +1255,10 @@ k_cg_ring(CgRingArgs A)
         const float* esrc[2] = {a.rhs, nullptr};
         sweep(nullptr, [&](const RingUnit& u, float& acc0, float& acc1) {
             REpiResidual0<PH> epi{a.r, sh.mean[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r), adaptive};
-            ring_process_unit<GENERIC, DIM, 1, 1, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
+            if constexpr (HELM) {
+                REpiHelm<REpiResidual0<PH>> he{epi, A.helm_a};
+                ring_process_unit<GENERIC, DIM, 1, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he);
+            } else ring_process_unit<GENERIC, DIM, 1, 1, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
             acc0 += epi.acc0; acc1 += epi.acc1;
         });
     }
@@ -1367,7 +1387,10 @@ k_cg_ring(CgRingArgs A)
             const float* esrc[2] = {nullptr, nullptr};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
                 REpiPassA<PH> epi{dnew, 0.f, 0.f, peer_halo(lo_dnew, hi_dnew)};
-                ring_process_unit<GENERIC, DIM, 2, 0, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, epi);
+                if constexpr (HELM) {
+                    REpiHelm<REpiPassA<PH>> he{epi, A.helm_a};
+                    ring_process_unit<GENERIC, DIM, 2, 0>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, he);
+                } else ring_process_unit<GENERIC, DIM, 2, 0, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, epi);
                 acc0 += epi.acc0; acc1 += epi.acc1;
             });
         } else {                                    // pass A of CG-adaptive: additionally d'.r (r once more, element-wise)
@@ -1406,7 +1429,10 @@ k_cg_ring(CgRingArgs A)
                     acc0 += epi.acc0; acc1 += epi.acc1;
                 } else {
                     REpiPassBr<PH> epi{a.r, sh.alpha[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
-                    ring_process_unit<GENERIC, DIM, 1, 1, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
+                    if constexpr (HELM) {
+                        REpiHelm<REpiPassBr<PH>> he{epi, A.helm_a};
+                        ring_process_unit<GENERIC, DIM, 1, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he);
+                    } else ring_process_unit<GENERIC, DIM, 1, 1, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
                     acc0 += epi.acc0;
                 }
             });
@@ -1420,7 +1446,10 @@ k_cg_ring(CgRingArgs A)
                     acc0 += epi.acc0; acc1 += epi.acc1;
                 } else {
                     REpiPassB<PH> epi{a.x, a.r, sh.alpha[u.b], sh.aprev[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
-                    ring_process_unit<GENERIC, DIM, 1, 3, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
+                    if constexpr (HELM) {
+                        REpiHelm<REpiPassB<PH>> he{epi, A.helm_a};
+                        ring_process_unit<GENERIC, DIM, 1, 3>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he);
+                    } else ring_process_unit<GENERIC, DIM, 1, 3, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
                     acc0 += epi.acc0;
                 }
             });
@@ -1624,6 +1653,8 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     const bool generic = mask || !ring_all_fast(g, l.pf, A.cfg);
     const bool dist = cm && cm->n > 1;
     const bool adapt = l.prm.method == PHI_SOLVER_CG_ADAPTIVE;
+    const bool helm = l.helm;                         // diffuse.implicit: single-GPU two-sweep CG on I - a L0, no obstacles
+    if (helm && (dist || adapt || mask)) return -100;
     // one-sweep CG (pass F): 3-D, branch-free tiling, periodic y and z, one GPU, plain CG without matrix offset or obstacles.
     // PHICUDA_CG_PASSES=2 forces the two-sweep kernel (A/B timing, tools/cg_passes_bench.py).
     bool fused = false;
@@ -1631,7 +1662,7 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     {
         const char* e = getenv("PHICUDA_CG_PASSES");
         const DField& pf = l.pf;
-        if (!(e && atoi(e) == 2) && g.dim == 3 && !generic && !dist && !adapt && !mask && l.prm.matrix_offset == 0.f
+        if (!(e && atoi(e) == 2) && g.dim == 3 && !generic && !dist && !adapt && !mask && !helm && l.prm.matrix_offset == 0.f
             && pf.klo[1] == PHI_BC_PERIODIC && pf.khi[1] == PHI_BC_PERIODIC && pf.klo[2] == PHI_BC_PERIODIC && pf.khi[2] == PHI_BC_PERIODIC) {
             // stage = d (TY+4) + r (TY+2) + x (TY) + d_{k-1} (TY) lines; the d_{k+1} tile is reserved at the largest TY ring_config may pick
             RingCfg fc;
@@ -1652,6 +1683,8 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     if (mask) fn = g.dim == 3 ? (dist ? (const void*)k_cg_ring<3, true, true, false, true> : (const void*)k_cg_ring<3, true, false, false, true>)
                               : (dist ? (const void*)k_cg_ring<2, true, true, false, true> : (const void*)k_cg_ring<2, true, false, false, true>);
     if (fused) fn = (const void*)k_cg_ring<3, false, false, false, false, true>;
+    if (helm) fn = g.dim == 3 ? (generic ? (const void*)k_cg_ring<3, true, false, false, false, false, true> : (const void*)k_cg_ring<3, false, false, false, false, false, true>)
+                              : (generic ? (const void*)k_cg_ring<2, true, false, false, false, false, true> : (const void*)k_cg_ring<2, false, false, false, false, false, true>);
 #undef CG_RING_FN
 #undef CG_RING_FN2
     e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -1694,6 +1727,7 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     a.partials = (double*)(ws + 3 * arr);
     const size_t pbytes = ((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double) + 255) / 256 * 256;
     A.d2 = (float*)(ws + 3 * arr + pbytes) + hoff; A.r1 = (float*)(ws + 4 * arr + pbytes) + hoff;
+    A.helm_a = l.helm_amount;
     a.result = l.result; a.prm = l.prm;
     if (cm) A.cm = *cm; else { memset(&A.cm, 0, sizeof(A.cm)); A.cm.n = 1; A.cm.lower = A.cm.upper = -1; }
     // grid.sync + block-0 send is the default multi-GPU barrier; PHICUDA_COMM_MERGE=1 selects the merged barrier
@@ -1704,4 +1738,72 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     note_ring_launch(PHI_KERNEL_CG_RING, A.cfg, generic, dist, adapt, grid, mask);
     phi_note_cg_passes(fused ? 1 : 2);
     return 0;
+}
+
+// ---- N5 diffuse.implicit --------------------------------------------------------------------------------------------------
+// The reference solves sharpen(x) = x - a L_bc(x) = y as the affine system M x = y - bias with M = I - a L0 (L0: L_bc with every
+// constant ghost 0) and bias = sharpen(0) = -a L_bc(0) (PhiML/phiml/math/_optimize.py:622, 645).  The bias is non-zero only in
+// cells next to a constant side with a non-zero value; this pass forms y' = y - bias = y + a L_bc(0) for every entry, with the
+// constants of the entry's component (entry b is component b % C).
+struct HelmConsts { float clo[3][3], chi[3][3]; };      // [component][axis]
+
+__global__ void k_helm_bias(DGrid g, DField f, int C, float amount, HelmConsts hc, const float* __restrict__ y, float* __restrict__ out)
+{
+    const long long plane = (long long)g.n[0] * g.n[1], cells = plane * g.n[2], total = cells * g.batch;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int b = (int)(i / cells);
+        const long long r = i - b * cells;
+        const int z = (int)(r / plane), yy = (int)((r - z * plane) / g.n[0]), x = (int)(r - z * plane - (long long)yy * g.n[0]);
+        const int idx[3] = {x, yy, z};
+        const int c = b % C;
+        float lap = 0.f;                        // L_bc(0): sum over axes of (lower ghost + upper ghost) / dx^2
+        for (int ax = 0; ax < g.dim; ++ax) {
+            float gs = 0.f;
+            if (idx[ax] == 0 && f.klo[ax] == PHI_BC_CONST) gs += hc.clo[c][ax];
+            if (idx[ax] == g.n[ax] - 1 && f.khi[ax] == PHI_BC_CONST) gs += hc.chi[c][ax];
+            lap += gs * g.inv_dx2[ax];
+        }
+        const long long off = b * f.sb + z * f.sz + (long long)yy * f.sy + x;
+        out[off] = fmaf(amount, lap, y[off]);
+    }
+}
+
+// the grid fits the persistent ring CG (host-only test, no CUDA call)
+bool phi_cg_ring_fits(const DGrid& g)
+{
+    if (g.batch > CG_MAX_BATCH || g.halo != 0) return false;
+    RingCfg c;
+    const int cgs = (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128);
+    return ring_config(g, 4, 2, cgs, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, 1, &c);
+}
+
+// l.pf: boundary kinds with zeroed constants (L0); cf[c]: the boundary with its constants of component c = entry % C (bias).  y'
+// lives in the workspace buffer of the one-sweep CG's third direction, which the two-sweep solve does not touch.  -100: the grid
+// does not fit.
+int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField cf[3], cudaStream_t s)
+{
+    const DGrid& g = l.g;
+    HelmConsts hc;
+    bool bias = false;
+    for (int c = 0; c < 3; ++c)
+        for (int ax = 0; ax < 3; ++ax) {
+            const bool used = c < C && ax < g.dim;
+            hc.clo[c][ax] = used && cf[c].klo[ax] == PHI_BC_CONST ? cf[c].clo[ax] : 0.f;
+            hc.chi[c][ax] = used && cf[c].khi[ax] == PHI_BC_CONST ? cf[c].chi[ax] : 0.f;
+            bias = bias || hc.clo[c][ax] != 0.f || hc.chi[c][ax] != 0.f;
+        }
+    CgLaunch m = l;
+    if (bias && l.helm_amount != 0.f) {
+        const size_t arr = ((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float) + 255) / 256 * 256;
+        const size_t pbytes = ((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double) + 255) / 256 * 256;
+        float* yb = (float*)((unsigned char*)l.workspace + 3 * arr + pbytes);
+        const long long total = (long long)g.n[0] * g.n[1] * g.n[2] * g.batch;
+        const long long want = (total + 255) / 256, cap = (long long)phi_sm_count() * 8;
+        const int blocks = (int)(want < cap ? want : cap);
+        k_helm_bias<<<blocks, 256, 0, s>>>(g, l.pf, C, l.helm_amount, hc, l.rhs, yb);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return (int)e;
+        m.rhs = yb;
+    }
+    return phi_launch_cg_ring(m, nullptr, s);
 }

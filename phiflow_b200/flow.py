@@ -5,12 +5,13 @@
 Mirrored (same names, argument meaning and error behaviour; reference file:line in each docstring):
     Box, Sphere, CenteredGrid, StaggeredGrid, extrapolation (ZERO, ONE, PERIODIC, ZERO_GRADIENT, BOUNDARY, combine_sides),
     Solve, SolveTape, NotConverged, Diverged, field.{divergence, laplace, spatial_gradient}, resample,
-    advect.{semi_lagrangian, mac_cormack, advect}, diffuse.explicit, fluid.{make_incompressible, incompressible_step},
+    advect.{semi_lagrangian, mac_cormack, advect}, diffuse.{explicit, implicit}, fluid.{make_incompressible, incompressible_step},
     write / read (field.write / field.read: the reference's .npz field files, see field_io.py).
 Fields hold device tensors in the library layout (DESIGN.md section 2); `.numpy()` returns the reference's (x, y[, z]) arrays.
 Anything outside the fast path raises NotImplementedError (where the reference-side façade would fall through to stock
 PhiFlow, INTEGRATION.md section 2).  No CPU fallback.
 """
+import numbers
 from builtins import range as builtins_range
 from types import SimpleNamespace
 from typing import Sequence
@@ -639,7 +640,38 @@ def explicit(fld, diffusivity: float, dt: float, substeps: int = 1):
     return fld.with_values(data)
 
 
-diffuse = SimpleNamespace(explicit=explicit)
+def implicit(fld, diffusivity: float, dt: float, solve: Solve = None):
+    """diffuse.implicit (phi/physics/diffuse.py:63-95): solves  x - diffusivity * dt * laplace(x) = fld  with CG (Solve('CG'), x0 = fld
+    unless solve.x0 is given), the constant boundary values entering as the bias of the affine system (_optimize.py:622, 645).
+    A scalar CenteredGrid with any boundary, or a PERIODIC StaggeredGrid whose components are solved as separate systems, as the
+    reference does (one record per batch entry and component, entry b * dim + c).  Returns a new field; SolveTape records,
+    NotConverged and Diverged as for make_incompressible."""
+    solve = solve or Solve('CG')
+    plain = lambda v: isinstance(v, numbers.Real) and not isinstance(v, bool)
+    _require(plain(diffusivity) and plain(dt), "implicit diffusion with a Field / vector / per-batch diffusivity or dt")
+    _require(solve.method == 'CG', f"solver '{solve.method}' for implicit diffusion")
+    amount = float(diffusivity) * float(dt)
+    if isinstance(fld, StaggeredGrid):
+        # the reference supports only PERIODIC here; ZERO and BOUNDARY are "not yet supported" (tests/commit/physics/test_diffuse.py:25,28)
+        _require(all(s == 'periodic' for a in fld.axes for s in (fld.boundary.side(a, False), fld.boundary.side(a, True))),
+                 "implicit diffusion of a non-periodic StaggeredGrid")
+        if solve.x0 is not None:
+            _require(isinstance(solve.x0, StaggeredGrid) and solve.x0._same_grid(fld), "x0 on a different grid")
+        data = ops.diffuse_implicit(fld.dom, fld.vspec, fld.data, amount, solve.rel_tol, solve.abs_tol, solve.max_iterations,
+                                    x0=solve.x0.data if solve.x0 is not None else None)
+        _finish_solve(fld.dom, solve, ops.read_results(fld.dom, len(fld.data)))
+        return fld.with_values(data)
+    _require(isinstance(fld, CenteredGrid) and fld.vector_scale is None, "implicit diffusion of this field type")
+    if solve.x0 is not None:
+        _require(isinstance(solve.x0, CenteredGrid) and solve.x0._same_grid(fld), "x0 on a different grid")
+    data = ops.diffuse_implicit(fld.dom, fld.spec, fld.data, amount, solve.rel_tol, solve.abs_tol, solve.max_iterations,
+                                x0=solve.x0.data if solve.x0 is not None else None)
+    _finish_solve(fld.dom, solve)
+    return fld.with_values(data)
+
+
+
+diffuse = SimpleNamespace(explicit=explicit, implicit=implicit)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -656,8 +688,8 @@ def _cg_params(v: StaggeredGrid, solve: Solve, masked=False):
                          matrix_offset=0.0 if adaptive else solve.matrix_offset, method='CG-adaptive' if adaptive else 'CG')
 
 
-def _finish_solve(dom, solve: Solve):
-    info = SolveInfo(solve, ops.read_results(dom))
+def _finish_solve(dom, solve: Solve, raw=None):
+    info = SolveInfo(solve, ops.read_results(dom) if raw is None else raw)
     for tape in _TAPES:
         tape.records.append((solve, info))
     if info.diverged.any() and Diverged not in solve.suppress:           # SolveInfo.convergence_check (_optimize.py:190-204)

@@ -344,6 +344,60 @@ def divergence(values, ext, dx, dims, resolution):
     return push_centered(dom, ENGINE.divergence(dom, vspec, v), batch_shape, dims)
 
 
+def diffuse_implicit(values, ext, dx, dims, resolution, amount: float, staggered: bool, rel_tol=1e-5, abs_tol=1e-5, max_iterations=1000,
+                     x0=None):
+    """diffuse.implicit (phi/physics/diffuse.py:63-95) on the VALUES of a grid: a scalar CenteredGrid, a CenteredGrid with one channel
+    dim of <= 3 components, or a PERIODIC StaggeredGrid.  Every component of every batch entry is its own system, as in the reference,
+    whose tracer (PhiML/phiml/math/_trace.py) keeps the uncoupled vector dim out of the matrix.  x0: values of the same
+    form (default: `values`).  Returns (new values, info dict with one record per system, ordered (batch entry, component), and
+    'components': the vector dim, or None for a scalar field)."""
+    math, _ = _phiml()
+    if math.get_precision() != 32:
+        raise NotEligible(f"precision {math.get_precision()} (fast path: 32; never silently downcast)")
+    if len(dims) not in (2, 3):
+        raise NotEligible(f"{len(dims)}-D grids")
+    if staggered:
+        vspec = to_vspec(ext, dims)
+        if any(s != 'periodic' for ax in (vspec[0] if isinstance(vspec, list) else vspec) for s in ax):
+            raise NotEligible("implicit diffusion of a non-periodic StaggeredGrid (the reference supports PERIODIC only, "
+                              "tests/commit/physics/test_diffuse.py:25,28)")
+        comps = split_components(values, dims)
+        x0c = split_components(x0, dims) if x0 is not None else None
+        names, spec = list(dims), vspec
+    else:
+        chan = values.shape.channel
+        if chan.rank > 1 or chan.volume > 3:
+            raise NotEligible(f"channel dims {chan} (fast path: scalar or one channel dim of <= 3 components)")
+        names = list(chan.get_item_names(chan.name) or range(chan.volume)) if chan.rank else [None]
+        comps = [values[{chan.name: n}] for n in names] if chan.rank else [values]
+        x0c = ([x0[{chan.name: n}] for n in names] if chan.rank else [x0]) if x0 is not None else None
+        specs = [to_spec(ext, dims, component=n if isinstance(n, str) else None) for n in names]
+        kinds = [[tuple(s if isinstance(s, str) else 'c' for s in ax) for ax in sp] for sp in specs]
+        if any(k != kinds[0] for k in kinds):
+            raise NotEligible("boundary kinds differ between vector components")
+        spec = specs if len(specs) > 1 else specs[0]
+    batch_shape = _batch_of(*comps, *(x0c or []))
+    dom = _domain(tuple(resolution), _dx_tuple(dx, dims), max(1, batch_shape.volume), None)
+    u = [pull_centered(dom, c, batch_shape, dims) for c in comps]
+    x = [pull_centered(dom, c, batch_shape, dims) for c in x0c] if x0c is not None else None
+    out = ENGINE.diffuse_implicit(dom, spec, u if len(u) > 1 or staggered else u[0], float(amount), rel_tol, abs_tol, max_iterations,
+                                  x0=(x if len(u) > 1 or staggered else x[0]) if x is not None else None)
+    out = out if isinstance(out, list) else [out]
+    res = ENGINE.read_results(dom, components=len(u)) if len(u) > 1 else ENGINE.read_results(dom)
+    info = {k: np.array(res[k]) for k in ('iterations', 'converged', 'diverged', 'residual_sq', 'tol_sq')}
+    pushed = [push_centered(dom, t, batch_shape, dims) for t in out]
+    from phiml.math import dual
+    info['components'] = dual(vector=tuple(dims)) if staggered else (values.shape.channel if values.shape.channel.rank else None)
+    if staggered:
+        return math.stack(pushed, dual(vector=tuple(dims))), info
+    if not values.shape.channel.rank:
+        return pushed[0], info
+    chan = values.shape.channel
+    item_names = chan.get_item_names(chan.name)
+    from phiml.math import channel
+    return math.stack(pushed, channel(**{chan.name: tuple(item_names) if item_names else len(pushed)})), info
+
+
 def grid_sample_native(grid: torch.Tensor, coords: torch.Tensor, mode: str):
     """Backend.grid_sample contract (PhiML/phiml/backend/_backend.py:1578-1593): grid (batch, x, y[, z], channel), coordinates
     (batch, points..., d) in index space, mode in 'zeros' | 'boundary' | 'periodic'.  Anything else -> NotImplemented, the

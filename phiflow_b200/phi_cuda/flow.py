@@ -49,17 +49,21 @@ def _fall(name, reason, stock, *args, **kwargs):
     return stock(*args, **kwargs)
 
 
-def _report(solve, info, x):
+def _report(solve, info, x, components=None):
     """SolveTape / NotConverged / Diverged protocol of math.solve_linear (PhiML/phiml/math/_optimize.py:190-204, 735-743).
     `x` is the pressure Field; the per-entry records of the kernel become Tensors over its batch dims.  The kernel keeps |r|^2 per
     entry, not the residual vector: `SolveInfo.residual` holds the residual NORM per entry (the "Max residual" of the not-converged
-    message is then that norm)."""
+    message is then that norm).  components: the vector dim when every component was its own system (records ordered (batch entry,
+    component)), as SolveInfo has them for the reference's batched solves."""
     import numpy as _np
     from phiml.math._optimize import SolveInfo, _SOLVE_TAPES
     batch_shape = x.values.shape.batch
 
     def per_entry(a):
         a = _np.asarray(a)
+        if components is not None:
+            groups = ([batch_shape] if batch_shape.rank else []) + [components]
+            return _math.reshaped_tensor(a.reshape([max(1, batch_shape.volume)] * bool(batch_shape.rank) + [components.volume]), groups, convert=False)
         return _math.reshaped_tensor(a, [batch_shape], convert=False) if batch_shape.rank else _math.wrap(a.reshape(-1)[0])
     # one non-batch dim, so that per-entry slices stay Tensors like a real residual vector does (_optimize.py:207-214)
     residual = _math.expand(per_entry(_np.sqrt(_np.maximum(info['residual_sq'], 0.0))), _math.channel(l2_norm=1))
@@ -165,6 +169,45 @@ def divergence(field, order=2, implicit=None, upwind=None):
     return _CenteredGrid(out, field.extrapolation.spatial_gradient(), field.bounds, field.resolution)
 
 
+def _number(v):
+    """float of a plain number or a phiml scalar Tensor, else NotEligible (Fields, vectors, per-batch values run on the stock path)."""
+    if isinstance(v, bool):
+        raise NotEligible("boolean diffusivity / dt")
+    if isinstance(v, (int, float)):
+        return float(v)
+    if isinstance(v, _math.Tensor) and v.shape.rank == 0:
+        return float(v)
+    raise NotEligible(f"diffusivity / dt {type(v).__name__} that is not a plain number (Field, vector or per-batch values)")
+
+
+def implicit(field, diffusivity, dt, solve=Solve('CG'), gradient=None, upwind=None, correct_skew=True, gradient_for_diffusivity=True):  # noqa: F405
+    """diffuse.implicit (phi/physics/diffuse.py:63-95), fast path for scalar / <= 3-channel CenteredGrids and periodic StaggeredGrids on
+    uniform grids with a numeric diffusivity and dt, Solve('CG') without preconditioner, fp32."""
+    stock = _diffuse.implicit
+    original_solve = solve
+    try:
+        if not isinstance(field, _Field) or not field.is_grid:
+            raise NotEligible("not a grid")
+        if gradient is not None or upwind is not None:
+            raise NotEligible("gradient / upwind (FVM arguments)")
+        amount = _number(diffusivity) * _number(dt)
+        solve = solve.with_defaults('solve')
+        if solve.method != 'CG' or solve.preconditioner is not None:
+            raise NotEligible(f"solver '{solve.method}' / preconditioner {solve.preconditioner} (fast path: Solve('CG'))")
+        dims, res, dx = _grid_info(field)
+        x0 = solve.x0.values if isinstance(solve.x0, _Field) else None
+        if solve.x0 is not None and x0 is None:
+            raise NotEligible("x0 that is not a Field")
+        values, info = _adapter.diffuse_implicit(field.values, field.extrapolation, dx, dims, res, amount, field.is_staggered,
+                                                 rel_tol=float(solve.rel_tol), abs_tol=float(solve.abs_tol),
+                                                 max_iterations=int(_math.max(solve.max_iterations)), x0=x0)
+    except (NotEligible, TypeError, ValueError) as why:
+        return _fall('diffuse.implicit', why, stock, field, diffusivity, dt, original_solve, gradient, upwind, correct_skew, gradient_for_diffusivity)
+    out = field.with_values(values)
+    _report(solve, info, out, info.pop('components'))
+    return out
+
+
 def _clone(module, **replacements):
     clone = _types.ModuleType(module.__name__, module.__doc__)
     clone.__dict__.update({k: v for k, v in module.__dict__.items() if not k.startswith('__')})
@@ -177,4 +220,4 @@ advect = _clone(_advect, semi_lagrangian=semi_lagrangian, mac_cormack=mac_cormac
                 advect=lambda field, velocity, dt, integrator=_advect.euler: (semi_lagrangian(field, velocity, dt, integrator)
                                                                              if isinstance(field, _Field) and field.is_grid else _advect.advect(field, velocity, dt, integrator)))
 field = _clone(_field, laplace=laplace, divergence=divergence)
-diffuse = _diffuse
+diffuse = _clone(_diffuse, implicit=implicit)
