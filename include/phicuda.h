@@ -130,6 +130,11 @@ int phicuda_last_launch_info(PhiLaunchInfo* out);
 /* Sweeps over the grid per iteration of this thread's most recent CG launch: 1 = one-sweep ring CG (3-D, periodic y and z,
  * one GPU, plain CG), 2 = two-sweep kernels (every other case, or PHICUDA_CG_PASSES=2); 0 before the first CG launch. */
 int phicuda_last_cg_passes(void);
+/* Operator of this thread's most recent CG launch (0 before the first one). */
+#define PHI_CG_OP_POISSON           1   /* laplace / masked laplace (pressure solves, cg_poisson) */
+#define PHI_CG_OP_HELMHOLTZ         2   /* I - a L0 (diffuse.implicit, plain-number diffusivity) */
+#define PHI_CG_OP_HELMHOLTZ_VARYING 3   /* I + D0 with face coefficients min(-dt k) (diffuse.implicit, varying diffusivity) */
+int phicuda_last_cg_operator(void);
 
 /* ---- A7  field.laplace order 2 (phi/field/_field_math.py:118-145 -> PhiML/phiml/math/_nd.py:825-861) ------------- */
 /* y = sum_d (x[i-1] + x[i+1] - 2 x[i]) / dx_d^2, ghost cells from `bc`.  8 B/cell. */
@@ -222,6 +227,21 @@ int phicuda_cg_poisson_dist_masked_f32(const PhiGrid* g, const PhiVBC* vbc, cons
 int phicuda_diffuse_implicit_f32(const PhiGrid* g, const PhiVBC* bc, int32_t components, float amount,
                                  const float* y, float* x, const PhiCgParams* prm, PhiCgResult* result,
                                  void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- N6  diffuse.implicit with a spatially varying diffusivity (phi/physics/diffuse.py:48-59, 90-95, 129-141) ---------------
+ * Solves sharpen(x) = explicit(x, k, -dt) = y for a scalar centred field: w = fl(-dt * k) per cell, every face takes
+ * f = min(w_lo, w_hi) and sharpen(x) = x + sum_d [f_{i+1/2} (x_{i+1} - x_i) - f_{i-1/2} (x_i - x_{i-1})] / dx_d^2.  The coefficient
+ * ghosts follow the field's boundary `bc`, not k's own (amount.at(u), phi/field/_resample.py:56-63): PERIODIC wraps,
+ * ZERO_GRADIENT copies the edge, a constant side with value c gives f_b = min(w_edge, c).  For dt > 0 the faces therefore take the
+ * MAXIMUM of k.  Solved as M x = y - bias with CG (x0 = x on entry, x == y allowed), M = I + D0 (value ghosts of constant sides
+ * 0), bias = sum over constant sides of f_b c / dx^2.  Every batch entry is its own system.
+ * diffusivity: centred array(s) in the grid's layout, diffusivity_batch = 1 (one k for every entry) or g->batch.
+ * prm: method PHI_SOLVER_CG, balance_rhs = project_mean = 0, matrix_offset = 0.  Same persistent TMA-ring CG as N5 (two sweeps,
+ * about 38 B/cell per iteration), phicuda_last_cg_operator() reports PHI_CG_OP_HELMHOLTZ_VARYING.  Single GPU, no z-slabs;
+ * grids that do not fit the ring return PHI_ERR_UNSUPPORTED.  workspace: phicuda_cg_workspace_bytes(g). */
+int phicuda_diffuse_implicit_varying_f32(const PhiGrid* g, const PhiBC* bc, const float* diffusivity, int32_t diffusivity_batch,
+                                         float dt, const float* y, float* x, const PhiCgParams* prm, PhiCgResult* result,
+                                         void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- A1  fluid.make_incompressible (phi/physics/fluid.py:94-162), no obstacles, order 2, staggered ------------------
  * div scratch: one centred array.  Equivalent to divergence + cg_poisson + grad_sub on the same stream. */

@@ -61,6 +61,7 @@ PROTOTYPES = {
     'phicuda_device_info': (C.c_int, [C.c_char_p, C.c_size_t, _P(C.c_int), _P(C.c_int), _P(C.c_int)]),
     'phicuda_last_launch_info': (C.c_int, [_P(PhiLaunchInfo)]),
     'phicuda_last_cg_passes': (C.c_int, []),
+    'phicuda_last_cg_operator': (C.c_int, []),
     'phicuda_max_abs_velocity_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), F3, C.c_void_p, C.c_void_p]),
     'phicuda_laplace_f32': (C.c_int, [_P(PhiGrid), _P(PhiBC), C.c_void_p, C.c_void_p, C.c_void_p]),
     'phicuda_laplace_axpy_f32': (C.c_int, [_P(PhiGrid), _P(PhiBC), C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]),
@@ -78,6 +79,8 @@ PROTOTYPES = {
                                          C.c_void_p, C.c_size_t, C.c_void_p]),
     'phicuda_diffuse_implicit_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), C.c_int32, C.c_float, C.c_void_p, C.c_void_p, _P(PhiCgParams),
                                                C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'phicuda_diffuse_implicit_varying_f32': (C.c_int, [_P(PhiGrid), _P(PhiBC), C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_void_p,
+                                                       _P(PhiCgParams), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     'phicuda_make_incompressible_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), F3, C.c_void_p, C.c_void_p, _P(PhiCgParams),
                                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     'phicuda_divergence_masked_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), F3, C.c_void_p, C.c_void_p, C.c_void_p]),

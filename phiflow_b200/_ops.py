@@ -335,6 +335,15 @@ def last_launch_info() -> dict:
     return out
 
 
+CG_OPERATORS = {0: None, 1: 'poisson', 2: 'helmholtz', 3: 'helmholtz_varying'}       # include/phicuda.h PHI_CG_OP_*
+
+
+def last_cg_operator():
+    """Operator of this thread's most recent CG launch: 'poisson', 'helmholtz' (diffuse_implicit), 'helmholtz_varying'
+    (diffuse_implicit_varying), or None before the first one."""
+    return CG_OPERATORS[int(_lib.load().phicuda_last_cg_operator())]
+
+
 def _is_flexible(vspec) -> bool:
     spec = vspec[0] if isinstance(vspec, list) else vspec
     return any(side == ZG for ax in spec for side in ax)
@@ -406,6 +415,27 @@ def diffuse_implicit(dom: Domain, spec, u, amount: float, rtol=1e-5, atol=1e-5, 
         return x if not isinstance(u, (list, tuple)) else [x]
     x = x.reshape((dom.batch, n) + tuple(comps[0].shape[1:]))
     return [x[:, c].clone() for c in range(n)]
+
+
+def diffuse_implicit_varying(dom: Domain, spec, u, k, dt: float, rtol=1e-5, atol=1e-5, max_iter=1000, x0=None):
+    """diffuse.implicit(u, k, dt) with a spatially varying diffusivity (phi/physics/diffuse.py:90-95, 129-141): solves
+    sharpen(x) = explicit(x, k, -dt) = u with CG.  Every face takes min(-dt k_lo, -dt k_hi), whose ghosts follow u's boundary `spec`
+    (a constant side with value c gives min(-dt k_edge, c)); for dt > 0 that is the face MAXIMUM of k.
+    u: centred array of `dom`; k: centred array with 1 (shared by every entry) or dom.batch entries.  x0: start value, default u.
+    Returns a new array; the inputs are not modified.  read_results(dom) then holds one record per batch entry."""
+    require_cuda()
+    assert dom.halo == 0, "implicit diffusion is not offered on z-slabs"
+    assert tuple(u.shape) == dom._shape(dom.cext), f"u: shape {tuple(u.shape)} is not a centred array of the domain"
+    assert k.dtype == torch.float32 and k.is_contiguous() and tuple(k.shape[1:]) == tuple(u.shape[1:]) and k.shape[0] in (1, dom.batch), \
+        f"k: shape {tuple(k.shape)} is not a centred array of the domain with 1 or {dom.batch} entries"
+    x = (u if x0 is None else x0).clone()
+    ws, _ = dom.workspace()
+    prm = PhiCgParams()                     # plain CG; I + D0 is not singular: no balancing, projection or offset
+    prm.rtol, prm.atol, prm.max_iter = rtol, atol, int(max_iter)
+    _lib.check(_lib.load().phicuda_diffuse_implicit_varying_f32(C.byref(dom.grid), C.byref(make_bc(spec)), _ptr(k), C.c_int32(k.shape[0]),
+                                                                C.c_float(dt), _ptr(u), _ptr(x), C.byref(prm), _ptr(dom.results()), _ptr(ws),
+                                                                C.c_size_t(ws.numel()), _stream()))
+    return x
 
 
 def mul_faces(dom: Domain, vbc, v, mask):

@@ -21,6 +21,8 @@ static thread_local PhiLaunchInfo g_last_launch = {};
 void phi_note_launch(const PhiLaunchInfo& info) { g_last_launch = info; }
 static thread_local int g_last_cg_passes = 0;
 void phi_note_cg_passes(int passes) { g_last_cg_passes = passes; }
+static thread_local int g_last_cg_operator = 0;
+void phi_note_cg_operator(int op) { g_last_cg_operator = op; }
 
 bool phi_ring_enabled()
 {
@@ -200,6 +202,7 @@ int phicuda_last_launch_info(PhiLaunchInfo* out)
 }
 
 int phicuda_last_cg_passes(void) { return g_last_cg_passes; }
+int phicuda_last_cg_operator(void) { return g_last_cg_operator; }
 
 int phicuda_device_info(char* name, size_t name_len, int* sm_count, int* cc_major, int* cc_minor)
 {
@@ -452,6 +455,43 @@ int phicuda_diffuse_implicit_f32(const PhiGrid* g, const PhiVBC* bc, int32_t com
     const int e = phi_launch_diffuse_implicit(l, components, cf, (cudaStream_t)stream);
     if (e == -100) { phi_set_error("diffuse_implicit: the grid does not fit the TMA-ring CG on this device"); return PHI_ERR_UNSUPPORTED; }
     return cuda_fail(e, "diffuse_implicit");
+}
+
+int phicuda_diffuse_implicit_varying_f32(const PhiGrid* g, const PhiBC* bc, const float* diffusivity, int32_t diffusivity_batch,
+                                         float dt, const float* y, float* x, const PhiCgParams* prm, PhiCgResult* result,
+                                         void* workspace, size_t workspace_bytes, void* stream)
+{
+    // every check runs before the first CUDA call
+    CgLaunch l; DField cf;
+    CHECK(phi_make_dgrid(g, &l.g));
+    if (!bc || !diffusivity || !y || !x || !prm || !result || !workspace) { phi_set_error("diffuse_implicit_varying: NULL argument"); return PHI_ERR_INVALID; }
+    if (diffusivity_batch != 1 && diffusivity_batch != g->batch) {
+        phi_set_error("diffuse_implicit_varying: diffusivity_batch must be 1 or the grid's batch %d, got %d", g->batch, diffusivity_batch); return PHI_ERR_INVALID;
+    }
+    if (!std::isfinite(dt)) { phi_set_error("diffuse_implicit_varying: dt is not finite"); return PHI_ERR_INVALID; }
+    if (prm->method != PHI_SOLVER_CG) { phi_set_error("diffuse_implicit_varying: only PHI_SOLVER_CG (the reference's Solve('CG'))"); return PHI_ERR_UNSUPPORTED; }
+    if (prm->balance_rhs || prm->project_mean || prm->matrix_offset != 0.f) {
+        phi_set_error("diffuse_implicit_varying: I + D0 is not singular - balance_rhs, project_mean and matrix_offset must be 0"); return PHI_ERR_INVALID;
+    }
+    if (g->halo != 0) { phi_set_error("diffuse_implicit_varying: z-slab grids are not supported"); return PHI_ERR_UNSUPPORTED; }
+    CHECK(phi_make_centered(g, bc, &cf));
+    if (workspace_bytes < phi_cg_workspace_bytes(l.g)) { phi_set_error("diffuse_implicit_varying: workspace %zu < %zu bytes", workspace_bytes, phi_cg_workspace_bytes(l.g)); return PHI_ERR_WORKSPACE; }
+    if (!phi_ring_enabled() || !phi_cg_ring_fits(l.g, true)) {
+        phi_set_error("diffuse_implicit_varying: the grid does not fit the TMA-ring CG (batch <= 1024, grid lines short enough); this operator has no other kernel");
+        return PHI_ERR_UNSUPPORTED;
+    }
+    PhiBC zero = *bc;                                            // D0: the value ghosts of constant sides are 0, the constants go into
+    for (int a = 0; a < 3; ++a) { zero.clo[a] = 0.f; zero.chi[a] = 0.f; }    // the bias and the coefficient ghosts
+    CHECK(phi_make_centered(g, &zero, &l.pf));
+    l.rhs = y; l.x = x; l.prm = *prm; l.result = result; l.workspace = workspace; l.workspace_bytes = workspace_bytes;
+    l.helm = true; l.helm_k = diffusivity; l.helm_k_bcast = diffusivity_batch == 1 && g->batch > 1; l.helm_ndt = -dt;
+    for (int a = 0; a < 3; ++a) {
+        l.helm_kclo[a] = a < g->dim && cf.klo[a] == PHI_BC_CONST ? cf.clo[a] : 0.f;
+        l.helm_kchi[a] = a < g->dim && cf.khi[a] == PHI_BC_CONST ? cf.chi[a] : 0.f;
+    }
+    const int e = phi_launch_diffuse_implicit_varying(l, (cudaStream_t)stream);
+    if (e == -100) { phi_set_error("diffuse_implicit_varying: the grid does not fit the TMA-ring CG on this device"); return PHI_ERR_UNSUPPORTED; }
+    return cuda_fail(e, "diffuse_implicit_varying");
 }
 
 // div -> CG -> v = vin - grad p.  vin/vout may be the same arrays (make_incompressible) or scratch -> state (fused step).

@@ -345,6 +345,7 @@ int phi_launch_cg(const CgLaunch& l, cudaStream_t s)
     err = cudaLaunchCooperativeKernel(cg_kernel(g.dim, mask), dim3(grid), dim3(PHI_WARPS_PER_CTA * 32), args, smem, s);
     if (err != cudaSuccess) { phi_set_error("cg: cooperative launch failed: %s", cudaGetErrorString(err)); return (int)err; }
     phi_note_cg_passes(2);
+    phi_note_cg_operator(PHI_CG_OP_POISSON);
     PhiLaunchInfo li = {}; li.kernel = PHI_KERNEL_CG_MARCH; li.generic = 1; li.masked = mask; li.total_units = a.um.total_units; li.grid_ctas = grid;
     phi_note_launch(li);
     return 0;

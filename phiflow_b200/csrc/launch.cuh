@@ -43,6 +43,12 @@ struct CgLaunch {
     const float* acc = nullptr;    // N4: accessible mask
     bool helm = false;             // N5 diffuse.implicit: operator I - helm_amount * L instead of L (pf carries L0: constants zeroed)
     float helm_amount = 0.f;
+    // N6 (with helm): varying diffusivity k, operator I + D0 with face coefficients min(fl(helm_ndt k)); helm_kclo / helm_kchi are
+    // the real boundary constants (coefficient ghosts; pf has them zeroed for the value ghosts)
+    const float* helm_k = nullptr;
+    bool helm_k_bcast = false;     // one k (entry 0) for every batch entry
+    float helm_ndt = 0.f;          // -dt
+    float helm_kclo[3] = {0.f, 0.f, 0.f}, helm_kchi[3] = {0.f, 0.f, 0.f};
 };
 size_t phi_cg_workspace_bytes(const DGrid& g);
 // TMA ring fast paths (ring_kernels.cu); return -100 when the shape does not fit and the caller must fall back
@@ -63,5 +69,8 @@ bool phi_ring_enabled();
 int phi_launch_cg(const CgLaunch& a, cudaStream_t s);
 // N5 diffuse.implicit on the ring CG (ring_kernels.cu): host-only fit test, and the solve (bias pre-pass + k_cg_ring<..., HELM>);
 // cf[c] = boundary with constants of component c (batch entry b is component b % C).  -100: the grid does not fit the ring.
-bool phi_cg_ring_fits(const DGrid& g);
+// xslot: the launch stages one more haloed array (N6: the diffusivity).
+bool phi_cg_ring_fits(const DGrid& g, bool xslot = false);
 int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField cf[3], cudaStream_t s);
+// N6 diffuse.implicit with a varying diffusivity (ring_kernels.cu): bias pre-pass + k_cg_ring<..., HELM, VARK>.  -100: no fit.
+int phi_launch_diffuse_implicit_varying(const CgLaunch& l, cudaStream_t s);

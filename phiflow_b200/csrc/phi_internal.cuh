@@ -337,3 +337,4 @@ int phi_sm_count();                      // SMs of the current device
 void phi_set_error(const char* fmt, ...);
 void phi_note_launch(const PhiLaunchInfo& info);
 void phi_note_cg_passes(int passes);       // sweeps per iteration of the last CG launch (phicuda_last_cg_passes)
+void phi_note_cg_operator(int op);         // PHI_CG_OP_* of the last CG launch (phicuda_last_cg_operator)

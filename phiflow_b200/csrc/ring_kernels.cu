@@ -127,10 +127,11 @@ struct ProdUnit {
 };
 
 // hactive: bit k set = haloed slot k is fetched (slot 1 idles in the first CG iteration; with obstacles the last slot is the mask)
-template <int DIM>
+// KSLOT (varying diffusivity): the last haloed slot is read from batch entry kb instead of b (kb = 0 broadcasts one k to all entries)
+template <int DIM, bool KSLOT = false>
 __device__ __forceinline__ void prod_unit_setup(ProdUnit& pu, const RingCfg& cfg, const DGrid& g, const DField& pf,
                                                 unsigned hactive, int NHslots, int NE, const float* const* hsrc, const float* const* esrc,
-                                                int b, int y0)
+                                                int b, int y0, int kb = 0)
 {
     const int lane = threadIdx.x & 31, hrows = cfg.TY + 2;
     const uint32_t row_bytes = (uint32_t)cfg.pitch * 4u;
@@ -147,7 +148,7 @@ __device__ __forceinline__ void prod_unit_setup(ProdUnit& pu, const RingCfg& cfg
             const int arr = r / hrows, j = r - arr * hrows;
             int yy = y0 - 1 + j; float cv;
             if (((hactive >> arr) & 1u) && yy <= g.n[1] && phi_resolve(yy, pf, 1, cv)) {
-                pu.yoff[it] = (long long)b * pf.sb + (long long)yy * pf.sy;
+                pu.yoff[it] = (long long)((KSLOT && arr == NHslots - 1) ? kb : b) * pf.sb + (long long)yy * pf.sy;
                 pu.base[it] = hsrc[arr];
                 pu.dsto[it] = 4u * (uint32_t)((arr * hrows + j) * cfg.pitch);
                 key = arr; yv = yy; halo_line = true; ch++;
@@ -285,15 +286,18 @@ __device__ __forceinline__ void groups_tile(ThreadGroups& tg, const RingCfg& cfg
 // MASK (N4, static obstacles): the last haloed slot of a stage holds the accessible mask; the stencil becomes
 //   q_c = sum_faces min(acc_c, acc_nb) * (v_nb - v_c) / dx^2 for fluid cells, q_c = v_c inside obstacles
 // (fluid.masked_laplace, phi/physics/fluid.py:197-202); constant (Dirichlet) ghost cells count as accessible.
-template <int DIM, int NH, int NE, bool MASK = false, class Epi>
+// VARK (N6, varying diffusivity): the last haloed slot holds the diffusivity k; the same face-minimum stencil runs on the
+// coefficients w = fl(epi.ndt * k) (ndt = -dt), a constant side's ghost coefficient is its boundary constant epi.kclo / epi.kchi
+// itself, and there is no obstacle override: q_c = sum_faces min(w_c, w_nb) * (v_nb - v_c) / dx^2 (phi/physics/diffuse.py:129-141).
+template <int DIM, int NH, int NE, bool MASK = false, bool VARK = false, class Epi>
 __device__ __forceinline__ void ring_compute(const RingCfg& cfg, const DGrid& g, const DField& pf, const ThreadGroups& tg,
                                              const float* sm, const float* sc, const float* sp, float beta,
                                              long long plane_off, int z, Epi& epi)
 {
     const int pitch = cfg.pitch;
     const int h1 = (cfg.TY + 2) * pitch;                 // offset of the second haloed array inside a stage
-    const int aoff = NH * (cfg.TY + 2) * pitch;          // MASK: offset of the accessible mask
-    const int e0off = (NH + (MASK ? 1 : 0)) * (cfg.TY + 2) * pitch;
+    const int aoff = NH * (cfg.TY + 2) * pitch;          // MASK: offset of the accessible mask (VARK: of the diffusivity)
+    const int e0off = (NH + ((MASK || VARK) ? 1 : 0)) * (cfg.TY + 2) * pitch;
     const int e1off = e0off + cfg.TY * pitch;
     const float ix2 = g.inv_dx2[0], iy2 = g.inv_dx2[1], iz2 = g.inv_dx2[2];
     const bool zm_const = DIM == 3 && z == 0 && pf.klo[2] == PHI_BC_CONST;
@@ -382,6 +386,39 @@ __device__ __forceinline__ void ring_compute(const RingCfg& cfg, const DGrid& g,
             if (ac.z == 0.f) q.z = c.z;
             if (ac.w == 0.f) q.w = c.w;
             epi.set_acc(ac);
+        } else if constexpr (VARK) {
+            // the diffusivity travels like the mask (same slot and staged lines); each staged k becomes w = fl(ndt k), rounded as the
+            // reference rounds k * (-dt); a constant side's ghost coefficient is its boundary constant itself
+            const float* am = sm + aoff; const float* ac_ = sc + aoff; const float* ap = sp + aoff;
+            const float ndt = epi.ndt;
+            auto cw = [ndt](float v) { return __fmul_rn(ndt, v); };
+            auto cw4 = [ndt](const float4& v) { return make_float4(__fmul_rn(ndt, v.x), __fmul_rn(ndt, v.y), __fmul_rn(ndt, v.z), __fmul_rn(ndt, v.w)); };
+            const float4 ac = cw4(*reinterpret_cast<const float4*>(ac_ + rc));
+            const int row = rc - (tg.eoff[k] - tg.j[k] * pitch);
+            const int nx = g.n[0];
+            float axl = (f & GF_XLO) ? (pf.klo[0] == PHI_BC_PERIODIC ? cw(ac_[row + nx - 1]) : (pf.klo[0] == PHI_BC_ZERO_GRADIENT ? ac.x : epi.kclo[0])) : cw(ac_[rc - 1]);
+            float axr = (f & GF_XHI) ? (pf.khi[0] == PHI_BC_PERIODIC ? cw(ac_[row]) : (pf.khi[0] == PHI_BC_ZERO_GRADIENT ? f4_get(ac, nvalid - 1) : epi.kchi[0])) : cw(ac_[rc + 4]);
+            const float4 al4 = make_float4(axl, ac.x, ac.y, ac.z);
+            float4 ar4 = make_float4(ac.y, ac.z, ac.w, axr);
+            if (nvalid < 4) f4_set(ar4, nvalid - 1, axr);
+            const float4 l4 = make_float4(xl, c.x, c.y, c.z);
+            const float4 aym = (f & GF_YLOC) ? f4_splat(epi.kclo[1]) : cw4(*reinterpret_cast<const float4*>(ac_ + rc - pitch));
+            const float4 ayp = (f & GF_YHIC) ? f4_splat(epi.kchi[1]) : cw4(*reinterpret_cast<const float4*>(ac_ + rc + pitch));
+            auto term = [](float vn, float vc, float an, float a0) { return fminf(an, a0) * (vn - vc); };
+            q.x = (term(l4.x, c.x, al4.x, ac.x) + term(r4.x, c.x, ar4.x, ac.x)) * ix2 + (term(ym.x, c.x, aym.x, ac.x) + term(yp.x, c.x, ayp.x, ac.x)) * iy2;
+            q.y = (term(l4.y, c.y, al4.y, ac.y) + term(r4.y, c.y, ar4.y, ac.y)) * ix2 + (term(ym.y, c.y, aym.y, ac.y) + term(yp.y, c.y, ayp.y, ac.y)) * iy2;
+            q.z = (term(l4.z, c.z, al4.z, ac.z) + term(r4.z, c.z, ar4.z, ac.z)) * ix2 + (term(ym.z, c.z, aym.z, ac.z) + term(yp.z, c.z, ayp.z, ac.z)) * iy2;
+            q.w = (term(l4.w, c.w, al4.w, ac.w) + term(r4.w, c.w, ar4.w, ac.w)) * ix2 + (term(ym.w, c.w, aym.w, ac.w) + term(yp.w, c.w, ayp.w, ac.w)) * iy2;
+            if (DIM == 3) {
+                const float4 zm = zm_const ? f4_splat(pf.clo[2]) : val4(sm, rc);
+                const float4 zp = zp_const ? f4_splat(pf.chi[2]) : val4(sp, rc);
+                const float4 azm = zm_const ? f4_splat(epi.kclo[2]) : cw4(*reinterpret_cast<const float4*>(am + rc));
+                const float4 azp = zp_const ? f4_splat(epi.kchi[2]) : cw4(*reinterpret_cast<const float4*>(ap + rc));
+                q.x += (term(zm.x, c.x, azm.x, ac.x) + term(zp.x, c.x, azp.x, ac.x)) * iz2;
+                q.y += (term(zm.y, c.y, azm.y, ac.y) + term(zp.y, c.y, azp.y, ac.y)) * iz2;
+                q.z += (term(zm.z, c.z, azm.z, ac.z) + term(zp.z, c.z, azp.z, ac.z)) * iz2;
+                q.w += (term(zm.w, c.w, azm.w, ac.w) + term(zp.w, c.w, azp.w, ac.w)) * iz2;
+            }
         } else {
         q.x = (xl + r4.x - 2.f * c.x) * ix2 + (ym.x + yp.x - 2.f * c.x) * iy2;
         q.y = (c.x + r4.y - 2.f * c.y) * ix2 + (ym.y + yp.y - 2.f * c.y) * iy2;
@@ -469,13 +506,13 @@ __device__ __forceinline__ void ring_compute_fast(const RingCfg& cfg, const DGri
     zs.have = MARCH && DIM == 3 && G <= 2;
 }
 
-template <bool GENERIC, int DIM, int NH, int NE, bool MARCH, bool MASK = false, class Epi>
+template <bool GENERIC, int DIM, int NH, int NE, bool MARCH, bool MASK = false, bool VARK = false, class Epi>
 __device__ __forceinline__ void ring_compute_any(const RingCfg& cfg, const DGrid& g, const DField& pf, const ThreadGroups& tg,
                                                  bool fast, const float* sm, const float* sc, const float* sp, float beta,
                                                  long long plane_off, int z, Epi& epi, ZMarch& zs)
 {
     if (cfg.dbg & 4) return;
-    if (MASK) { zs.have = false; ring_compute<DIM, NH, NE, true>(cfg, g, pf, tg, sm, sc, sp, beta, plane_off, z, epi); return; }
+    if (MASK || VARK) { zs.have = false; ring_compute<DIM, NH, NE, MASK, VARK>(cfg, g, pf, tg, sm, sc, sp, beta, plane_off, z, epi); return; }
     if (!GENERIC || fast) {
         if (cfg.groups == 4) { ring_compute_fast<DIM, NH, NE, 4, MARCH>(cfg, g, tg, sm, sc, sp, beta, plane_off, epi, zs); return; }
         if (cfg.groups == 2) { ring_compute_fast<DIM, NH, NE, 2, MARCH>(cfg, g, tg, sm, sc, sp, beta, plane_off, epi, zs); return; }
@@ -521,7 +558,7 @@ __device__ __forceinline__ bool ring_next_unit(const RingCfg& cfg, const DGrid& 
 }
 
 // consumers, 3-D: march through the planes of one unit.  G > 0: every plane takes the branch-free path with G groups.
-template <bool GENERIC, int NH, int NE, bool MARCH, int G, bool MASK = false, class Epi>
+template <bool GENERIC, int NH, int NE, bool MARCH, int G, bool MASK = false, bool VARK = false, class Epi>
 __device__ __forceinline__ void ring_consume_planes(Ring& rg, const RingCfg& cfg, const DGrid& g, const DField& pf, const ThreadGroups& tg,
                                                     bool tile_fast, float beta, long long plane_off, const RingUnit& u, Epi& epi)
 {
@@ -540,7 +577,7 @@ __device__ __forceinline__ void ring_consume_planes(Ring& rg, const RingCfg& cfg
                                                                      beta, plane_off, epi, zs);
         } else {
             const bool fast = tile_fast && !(z == 0 && pf.klo[2] == PHI_BC_CONST) && !(z == g.n[2] - 1 && pf.khi[2] == PHI_BC_CONST);
-            ring_compute_any<GENERIC, 3, NH, NE, MARCH, MASK>(cfg, g, pf, tg, fast, ring_ptr(rg, cfg, a), ring_ptr(rg, cfg, bq), ring_ptr(rg, cfg, c2),
+            ring_compute_any<GENERIC, 3, NH, NE, MARCH, MASK, VARK>(cfg, g, pf, tg, fast, ring_ptr(rg, cfg, a), ring_ptr(rg, cfg, bq), ring_ptr(rg, cfg, c2),
                                                               beta, plane_off, z, epi, zs);
         }
         ring_release(rg, a);
@@ -552,17 +589,19 @@ __device__ __forceinline__ void ring_consume_planes(Ring& rg, const RingCfg& cfg
 }
 
 // MASK: hsrc[NH] is the accessible mask; it occupies the haloed slot after the NH value arrays.
-template <bool GENERIC, int DIM, int NH, int NE, bool MARCH = true, bool MASK = false, class Epi>
+// VARK: hsrc[NH] is the diffusivity, in the same slot; it is read from batch entry kb (0 when one k serves every entry).
+template <bool GENERIC, int DIM, int NH, int NE, bool MARCH = true, bool MASK = false, bool VARK = false, class Epi>
 __device__ __forceinline__ void ring_process_unit(Ring& rg, const RingCfg& cfg, const DGrid& g, const DField& pf,
                                                   ThreadGroups& tg,
                                                   const float* const* hsrc, const float* const* esrc, float beta,
-                                                  const RingUnit& u, Epi& epi)
+                                                  const RingUnit& u, Epi& epi, int kb = 0)
 {
+    constexpr bool XSLOT = MASK || VARK;                            // one more haloed array after the NH value arrays
     const bool producer = (int)threadIdx.x >= cfg.consumers;
     if (producer) {
         const int nh = (NH == 2 && beta == 0.f) ? 1 : NH;          // first CG iteration: d' = r, old direction not read
         ProdUnit pu;
-        prod_unit_setup<DIM>(pu, cfg, g, pf, ((1u << nh) - 1u) | (MASK ? (1u << NH) : 0u), NH + (MASK ? 1 : 0), NE, hsrc, esrc, u.b, u.y0);
+        prod_unit_setup<DIM, VARK>(pu, cfg, g, pf, ((1u << nh) - 1u) | (XSLOT ? (1u << NH) : 0u), NH + (XSLOT ? 1 : 0), NE, hsrc, esrc, u.b, u.y0, kb);
         if (DIM == 3) {
             const int nz = u.z1 - u.z0;
             for (int p = 0; p < nz + 2; ++p)
@@ -573,7 +612,7 @@ __device__ __forceinline__ void ring_process_unit(Ring& rg, const RingCfg& cfg, 
         return;
     }
     const int ny = g.n[1];
-    const bool tile_fast = !MASK && (!GENERIC || tg.fast_ok && u.y0 + cfg.TY <= ny
+    const bool tile_fast = !XSLOT && (!GENERIC || tg.fast_ok && u.y0 + cfg.TY <= ny
                            && !(u.y0 == 0 && pf.klo[1] == PHI_BC_CONST) && !(u.y0 + cfg.TY == ny && pf.khi[1] == PHI_BC_CONST));
     if (GENERIC) groups_tile(tg, cfg, g, pf, u.y0);      // also needed on fast tiles: planes with constant z ghosts take the slow path
     long long plane_off = (long long)u.b * pf.sb + (long long)u.y0 * pf.sy + (DIM == 3 ? (long long)u.z0 * pf.sz : 0);
@@ -582,14 +621,14 @@ __device__ __forceinline__ void ring_process_unit(Ring& rg, const RingCfg& cfg, 
         if (!GENERIC && cfg.groups == 2) ring_consume_planes<GENERIC, NH, NE, MARCH, 2>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi);
         else if (!GENERIC && cfg.groups == 4) ring_consume_planes<GENERIC, NH, NE, MARCH, 4>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi);
         else if (!GENERIC) ring_consume_planes<GENERIC, NH, NE, MARCH, 1>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi);
-        else ring_consume_planes<GENERIC, NH, NE, MARCH, 0, MASK>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi);
+        else ring_consume_planes<GENERIC, NH, NE, MARCH, 0, MASK, VARK>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi);
     } else {
         const SlotIt a = rg.pos;
         ring_wait_full(rg, a);
         const float* sc = ring_ptr(rg, cfg, a);
         epi.set_plane(-1, 0);
         ZMarch zs; zs.have = false;
-        ring_compute_any<GENERIC, DIM, NH, NE, MARCH, MASK>(cfg, g, pf, tg, tile_fast, sc, sc, sc, beta, plane_off, 0, epi, zs);
+        ring_compute_any<GENERIC, DIM, NH, NE, MARCH, MASK, VARK>(cfg, g, pf, tg, tile_fast, sc, sc, sc, beta, plane_off, 0, epi, zs);
         ring_release(rg, a);
         rg.pos.next(cfg.R);
     }
@@ -743,6 +782,21 @@ struct REpiHelm {
     }
 };
 
+// diffuse.implicit with a varying diffusivity (N6): the VARK consumer delivers q = D0 c, the face-minimum stencil on the
+// coefficients w = fl(ndt k) (ndt = -dt, ghosts of constant sides: kclo / kchi, which the consumer reads from here), so that
+// M c = c + q (sharpen = explicit(x, k, -dt), phi/physics/diffuse.py:90-95).  No rhs balancing: set_acc is not forwarded.
+template <class Epi>
+struct REpiVarHelm {
+    Epi& e; float ndt; float kclo[3], kchi[3];
+    __device__ __forceinline__ void set_plane(int z, int nz) { e.set_plane(z, nz); }
+    __device__ __forceinline__ void set_acc(const float4&) {}
+    __device__ __forceinline__ void operator()(long long off, const float4& c, const float4& q, int nvalid, const float4& e0, const float4& e1, const float4& e2)
+    {
+        const float4 m = make_float4(c.x + q.x, c.y + q.y, c.z + q.z, c.w + q.w);
+        e(off, c, m, nvalid, e0, e1, e2);
+    }
+};
+
 // ---- laplace -----------------------------------------------------------------------------------------------------------
 template <int DIM, bool AXPY, bool GENERIC>
 __global__ void __launch_bounds__(RING_THREADS, 2)
@@ -771,7 +825,16 @@ struct CgRingArgs {
     CommDev cm;
     float* d2; float* r1;        // one-sweep CG: third direction buffer, second residual buffer
     float helm_a;                // HELM (diffuse.implicit): operator I - helm_a * L0
+    const float* k; int kbcast;  // VARK (varying diffusivity): k per batch entry, or (kbcast) entry 0 for all
+    float ndt;                   // VARK: -dt
+    float kclo[3], kchi[3];      // VARK: boundary constants of the constant sides (ghost coefficients; pf has them zeroed)
 };
+
+template <class Epi>
+__device__ __forceinline__ REpiVarHelm<Epi> var_helm(Epi& e, const CgRingArgs& A)
+{
+    return REpiVarHelm<Epi>{e, A.ndt, {A.kclo[0], A.kclo[1], A.kclo[2]}, {A.kchi[0], A.kchi[1], A.kchi[2]}};
+}
 
 __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p)
 {
@@ -1166,11 +1229,13 @@ struct REpiFusedStart {
 // MASK (N4): static obstacles - a.acc is the accessible mask, staged as an extra haloed array (always the GENERIC consumer).
 // FUSED: the one-sweep iteration (pass F above) replaces passes A and B.
 // HELM (N5, diffuse.implicit): two-sweep CG on M = I - A.helm_a * L0 (REpiHelm); every batch entry is its own system.
-template <int DIM, bool GENERIC, bool DIST, bool ADAPT, bool MASK = false, bool FUSED = false, bool HELM = false>
+// VARK (N6, with HELM): the operator is M = I + D0 of a varying diffusivity A.k (REpiVarHelm, the VARK consumer) instead.
+template <int DIM, bool GENERIC, bool DIST, bool ADAPT, bool MASK = false, bool FUSED = false, bool HELM = false, bool VARK = false>
 __global__ void __launch_bounds__(RING_THREADS, 1)
 k_cg_ring(CgRingArgs A)
 {
     static_assert(!HELM || (!DIST && !ADAPT && !MASK && !FUSED), "the Helmholtz operator runs on the single-GPU two-sweep CG only");
+    static_assert(!VARK || (HELM && GENERIC), "the varying-diffusivity operator is a Helmholtz operator on the generic consumer");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const CgArgs& a = A.a;
     const RingCfg& cfg = A.cfg;
@@ -1251,11 +1316,14 @@ k_cg_ring(CgRingArgs A)
     }
 
     {   // r0 = y - (A + c 11^T) x0
-        const float* hsrc[2] = {a.x, MASK ? a.acc : nullptr};
+        const float* hsrc[2] = {a.x, MASK ? a.acc : (VARK ? A.k : nullptr)};
         const float* esrc[2] = {a.rhs, nullptr};
         sweep(nullptr, [&](const RingUnit& u, float& acc0, float& acc1) {
             REpiResidual0<PH> epi{a.r, sh.mean[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r), adaptive};
-            if constexpr (HELM) {
+            if constexpr (VARK) {
+                auto he = var_helm(epi, A);
+                ring_process_unit<GENERIC, DIM, 1, 1, true, false, true>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he, A.kbcast ? 0 : u.b);
+            } else if constexpr (HELM) {
                 REpiHelm<REpiResidual0<PH>> he{epi, A.helm_a};
                 ring_process_unit<GENERIC, DIM, 1, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he);
             } else ring_process_unit<GENERIC, DIM, 1, 1, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
@@ -1383,11 +1451,14 @@ k_cg_ring(CgRingArgs A)
     bool x_pending = false;      // all running entries are at the same iteration, so one flag describes them all
     while (!FUSED && *sh.any_cont && comm_ok) {
         if (cfg.dbg & 1) {} else if constexpr (!ADAPT) {   // pass A
-            const float* hsrc[3] = {a.r, dold, MASK ? a.acc : nullptr};
+            const float* hsrc[3] = {a.r, dold, MASK ? a.acc : (VARK ? A.k : nullptr)};
             const float* esrc[2] = {nullptr, nullptr};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
                 REpiPassA<PH> epi{dnew, 0.f, 0.f, peer_halo(lo_dnew, hi_dnew)};
-                if constexpr (HELM) {
+                if constexpr (VARK) {
+                    auto he = var_helm(epi, A);
+                    ring_process_unit<GENERIC, DIM, 2, 0, true, false, true>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, he, A.kbcast ? 0 : u.b);
+                } else if constexpr (HELM) {
                     REpiHelm<REpiPassA<PH>> he{epi, A.helm_a};
                     ring_process_unit<GENERIC, DIM, 2, 0>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, he);
                 } else ring_process_unit<GENERIC, DIM, 2, 0, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, epi);
@@ -1420,7 +1491,7 @@ k_cg_ring(CgRingArgs A)
         }
         __syncthreads();
         if (cfg.dbg & 2) {} else if (!x_pending) {   // pass B, odd iteration: r only, the x update is deferred
-            const float* hsrc[2] = {dnew, MASK ? a.acc : nullptr};
+            const float* hsrc[2] = {dnew, MASK ? a.acc : (VARK ? A.k : nullptr)};
             const float* esrc[3] = {a.r, nullptr, nullptr};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
                 if constexpr (ADAPT) {
@@ -1429,7 +1500,10 @@ k_cg_ring(CgRingArgs A)
                     acc0 += epi.acc0; acc1 += epi.acc1;
                 } else {
                     REpiPassBr<PH> epi{a.r, sh.alpha[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
-                    if constexpr (HELM) {
+                    if constexpr (VARK) {
+                        auto he = var_helm(epi, A);
+                        ring_process_unit<GENERIC, DIM, 1, 1, true, false, true>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he, A.kbcast ? 0 : u.b);
+                    } else if constexpr (HELM) {
                         REpiHelm<REpiPassBr<PH>> he{epi, A.helm_a};
                         ring_process_unit<GENERIC, DIM, 1, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he);
                     } else ring_process_unit<GENERIC, DIM, 1, 1, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
@@ -1437,7 +1511,7 @@ k_cg_ring(CgRingArgs A)
                 }
             });
         } else {            // pass B, even iteration: x += alpha_prev d_prev + alpha d
-            const float* hsrc[2] = {dnew, MASK ? a.acc : nullptr};
+            const float* hsrc[2] = {dnew, MASK ? a.acc : (VARK ? A.k : nullptr)};
             const float* esrc[3] = {a.x, a.r, dold};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
                 if constexpr (ADAPT) {
@@ -1446,7 +1520,10 @@ k_cg_ring(CgRingArgs A)
                     acc0 += epi.acc0; acc1 += epi.acc1;
                 } else {
                     REpiPassB<PH> epi{a.x, a.r, sh.alpha[u.b], sh.aprev[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
-                    if constexpr (HELM) {
+                    if constexpr (VARK) {
+                        auto he = var_helm(epi, A);
+                        ring_process_unit<GENERIC, DIM, 1, 3, true, false, true>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he, A.kbcast ? 0 : u.b);
+                    } else if constexpr (HELM) {
                         REpiHelm<REpiPassB<PH>> he{epi, A.helm_a};
                         ring_process_unit<GENERIC, DIM, 1, 3>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he);
                     } else ring_process_unit<GENERIC, DIM, 1, 3, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
@@ -1640,21 +1717,24 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     if (g.batch > CG_MAX_BATCH) return -100;
     const bool mask = l.acc != nullptr;
     if (mask && (l.prm.method == PHI_SOLVER_CG_ADAPTIVE || l.prm.matrix_offset != 0.f)) return -100;
+    const bool vark = l.helm_k != nullptr;            // varying diffusivity: k is staged like the obstacle mask
+    const bool xslot = mask || vark;
     CgRingArgs A;
     const int cgs = (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128);
     const int sms = phi_sm_count();
-    // lines staged per stage: pass B (even) = 1 haloed + 3 element-wise arrays = 4 TY + 2; with the obstacle mask as an extra
-    // haloed array 5 TY + 4 (pass A: 3 haloed = 3 TY + 6)
-    if (!ring_config(g, mask ? 5 : 4, mask ? 6 : 2, cgs, g.dim == 3 ? (mask ? 3 : 4) : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
+    // lines staged per stage: pass B (even) = 1 haloed + 3 element-wise arrays = 4 TY + 2; with the obstacle mask (or the
+    // diffusivity) as an extra haloed array 5 TY + 4 (pass A: 3 haloed = 3 TY + 6)
+    if (!ring_config(g, xslot ? 5 : 4, xslot ? 6 : 2, cgs, g.dim == 3 ? (xslot ? 3 : 4) : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
     const int threads = RING_THREADS;
     A.ring_smem_offset = cgs;
     int per_sm = 0;
     cudaError_t e;
-    const bool generic = mask || !ring_all_fast(g, l.pf, A.cfg);
+    const bool generic = xslot || !ring_all_fast(g, l.pf, A.cfg);
     const bool dist = cm && cm->n > 1;
     const bool adapt = l.prm.method == PHI_SOLVER_CG_ADAPTIVE;
     const bool helm = l.helm;                         // diffuse.implicit: single-GPU two-sweep CG on I - a L0, no obstacles
     if (helm && (dist || adapt || mask)) return -100;
+    if (vark && !helm) return -100;
     // one-sweep CG (pass F): 3-D, branch-free tiling, periodic y and z, one GPU, plain CG without matrix offset or obstacles.
     // PHICUDA_CG_PASSES=2 forces the two-sweep kernel (A/B timing, tools/cg_passes_bench.py).
     bool fused = false;
@@ -1685,6 +1765,7 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     if (fused) fn = (const void*)k_cg_ring<3, false, false, false, false, true>;
     if (helm) fn = g.dim == 3 ? (generic ? (const void*)k_cg_ring<3, true, false, false, false, false, true> : (const void*)k_cg_ring<3, false, false, false, false, false, true>)
                               : (generic ? (const void*)k_cg_ring<2, true, false, false, false, false, true> : (const void*)k_cg_ring<2, false, false, false, false, false, true>);
+    if (vark) fn = g.dim == 3 ? (const void*)k_cg_ring<3, true, false, false, false, false, true, true> : (const void*)k_cg_ring<2, true, false, false, false, false, true, true>;
 #undef CG_RING_FN
 #undef CG_RING_FN2
     e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -1728,6 +1809,8 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     const size_t pbytes = ((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double) + 255) / 256 * 256;
     A.d2 = (float*)(ws + 3 * arr + pbytes) + hoff; A.r1 = (float*)(ws + 4 * arr + pbytes) + hoff;
     A.helm_a = l.helm_amount;
+    A.k = l.helm_k; A.kbcast = l.helm_k_bcast ? 1 : 0; A.ndt = l.helm_ndt;
+    for (int d = 0; d < 3; ++d) { A.kclo[d] = l.helm_kclo[d]; A.kchi[d] = l.helm_kchi[d]; }
     a.result = l.result; a.prm = l.prm;
     if (cm) A.cm = *cm; else { memset(&A.cm, 0, sizeof(A.cm)); A.cm.n = 1; A.cm.lower = A.cm.upper = -1; }
     // grid.sync + block-0 send is the default multi-GPU barrier; PHICUDA_COMM_MERGE=1 selects the merged barrier
@@ -1737,6 +1820,7 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     if (e != cudaSuccess) { phi_set_error("cg ring: cooperative launch failed: %s", cudaGetErrorString(e)); return (int)e; }
     note_ring_launch(PHI_KERNEL_CG_RING, A.cfg, generic, dist, adapt, grid, mask);
     phi_note_cg_passes(fused ? 1 : 2);
+    phi_note_cg_operator(vark ? PHI_CG_OP_HELMHOLTZ_VARYING : (helm ? PHI_CG_OP_HELMHOLTZ : PHI_CG_OP_POISSON));
     return 0;
 }
 
@@ -1768,13 +1852,38 @@ __global__ void k_helm_bias(DGrid g, DField f, int C, float amount, HelmConsts h
     }
 }
 
-// the grid fits the persistent ring CG (host-only test, no CUDA call)
-bool phi_cg_ring_fits(const DGrid& g)
+// N6, varying diffusivity: bias = sharpen(0) = sum over constant sides of f_b c / dx^2 with f_b = min(fl(ndt k_edge), c) (the
+// coefficient ghost of a constant side is c itself); this pass forms y' = y - bias.  k: entry b, or entry 0 when kbcast.
+__global__ void k_helm_bias_var(DGrid g, DField f, float ndt, HelmConsts hc, const float* __restrict__ k, int kbcast,
+                                const float* __restrict__ y, float* __restrict__ out)
+{
+    const long long plane = (long long)g.n[0] * g.n[1], cells = plane * g.n[2], total = cells * g.batch;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int b = (int)(i / cells);
+        const long long r = i - b * cells;
+        const int z = (int)(r / plane), yy = (int)((r - z * plane) / g.n[0]), x = (int)(r - z * plane - (long long)yy * g.n[0]);
+        const int idx[3] = {x, yy, z};
+        const long long cell = z * f.sz + (long long)yy * f.sy + x;
+        const float w = __fmul_rn(ndt, k[(kbcast ? 0 : b) * f.sb + cell]);
+        float bias = 0.f;
+        for (int ax = 0; ax < g.dim; ++ax) {
+            float s = 0.f;
+            if (idx[ax] == 0 && f.klo[ax] == PHI_BC_CONST) { const float c = hc.clo[0][ax]; s += fminf(w, c) * c; }
+            if (idx[ax] == g.n[ax] - 1 && f.khi[ax] == PHI_BC_CONST) { const float c = hc.chi[0][ax]; s += fminf(w, c) * c; }
+            bias += s * g.inv_dx2[ax];
+        }
+        const long long off = b * f.sb + cell;
+        out[off] = y[off] - bias;
+    }
+}
+
+// the grid fits the persistent ring CG (host-only test, no CUDA call); xslot: with one more haloed array (the diffusivity)
+bool phi_cg_ring_fits(const DGrid& g, bool xslot)
 {
     if (g.batch > CG_MAX_BATCH || g.halo != 0) return false;
     RingCfg c;
     const int cgs = (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128);
-    return ring_config(g, 4, 2, cgs, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, 1, &c);
+    return ring_config(g, xslot ? 5 : 4, xslot ? 6 : 2, cgs, g.dim == 3 ? (xslot ? 3 : 4) : 2, RING_MAX_STAGES, 1, &c);
 }
 
 // l.pf: boundary kinds with zeroed constants (L0); cf[c]: the boundary with its constants of component c = entry % C (bias).  y'
@@ -1801,6 +1910,36 @@ int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField cf[3], cu
         const long long want = (total + 255) / 256, cap = (long long)phi_sm_count() * 8;
         const int blocks = (int)(want < cap ? want : cap);
         k_helm_bias<<<blocks, 256, 0, s>>>(g, l.pf, C, l.helm_amount, hc, l.rhs, yb);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return (int)e;
+        m.rhs = yb;
+    }
+    return phi_launch_cg_ring(m, nullptr, s);
+}
+
+// N6: l.pf: boundary kinds with zeroed constants (value ghosts of D0); l.helm_kclo / helm_kchi: the real constants (coefficient
+// ghosts and bias).  y' goes to the same workspace buffer as for N5.  The bias pre-pass runs whenever a constant is non-zero - also
+// for dt = 0, where f_b = min(-0, c) = c for c < 0.  -100: the grid does not fit.
+int phi_launch_diffuse_implicit_varying(const CgLaunch& l, cudaStream_t s)
+{
+    const DGrid& g = l.g;
+    HelmConsts hc;
+    memset(&hc, 0, sizeof(hc));
+    bool bias = false;
+    for (int ax = 0; ax < g.dim; ++ax) {
+        hc.clo[0][ax] = l.pf.klo[ax] == PHI_BC_CONST ? l.helm_kclo[ax] : 0.f;
+        hc.chi[0][ax] = l.pf.khi[ax] == PHI_BC_CONST ? l.helm_kchi[ax] : 0.f;
+        bias = bias || hc.clo[0][ax] != 0.f || hc.chi[0][ax] != 0.f;
+    }
+    CgLaunch m = l;
+    if (bias) {
+        const size_t arr = ((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float) + 255) / 256 * 256;
+        const size_t pbytes = ((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double) + 255) / 256 * 256;
+        float* yb = (float*)((unsigned char*)l.workspace + 3 * arr + pbytes);
+        const long long total = (long long)g.n[0] * g.n[1] * g.n[2] * g.batch;
+        const long long want = (total + 255) / 256, cap = (long long)phi_sm_count() * 8;
+        const int blocks = (int)(want < cap ? want : cap);
+        k_helm_bias_var<<<blocks, 256, 0, s>>>(g, l.pf, l.helm_ndt, hc, l.helm_k, l.helm_k_bcast ? 1 : 0, l.rhs, yb);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return (int)e;
         m.rhs = yb;

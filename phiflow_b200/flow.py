@@ -3,7 +3,7 @@
 (the surface `from phi.flow import *` gives a grid-fluid notebook: phi/flow.py:13-28), backed by the CUDA kernels.
 
 Mirrored (same names, argument meaning and error behaviour; reference file:line in each docstring):
-    Box, Sphere, CenteredGrid, StaggeredGrid, extrapolation (ZERO, ONE, PERIODIC, ZERO_GRADIENT, BOUNDARY, combine_sides),
+    Box, Sphere, union, CenteredGrid, StaggeredGrid, extrapolation (ZERO, ONE, PERIODIC, ZERO_GRADIENT, BOUNDARY, combine_sides),
     Solve, SolveTape, NotConverged, Diverged, field.{divergence, laplace, spatial_gradient}, resample,
     advect.{semi_lagrangian, mac_cormack, advect}, diffuse.{explicit, implicit}, fluid.{make_incompressible, incompressible_step},
     write / read (field.write / field.read: the reference's .npz field files, see field_io.py).
@@ -23,7 +23,7 @@ from . import _ops as ops
 from . import field_io
 from . import scene as _scene
 
-__all__ = ['Scene', 'vec', 'batch', 'iterate', 'jit_compile', 'Box', 'Sphere', 'CenteredGrid', 'StaggeredGrid', 'extrapolation', 'ZERO', 'ONE', 'PERIODIC', 'ZERO_GRADIENT',
+__all__ = ['Scene', 'vec', 'batch', 'iterate', 'jit_compile', 'Box', 'Sphere', 'union', 'CenteredGrid', 'StaggeredGrid', 'extrapolation', 'ZERO', 'ONE', 'PERIODIC', 'ZERO_GRADIENT',
            'BOUNDARY', 'combine_sides', 'Solve', 'SolveTape', 'NotConverged', 'Diverged', 'ConvergenceException', 'field',
            'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read']
 
@@ -166,6 +166,29 @@ class Sphere:
         (phi/geom/_sphere.py:107-120, vec_length eps=1e-3)."""
         d = np.sqrt(np.maximum(np.sum((pts - np.asarray(self.center, np.float32)) ** 2, -1, dtype=np.float32), np.float32(1e-6)))
         return np.clip(np.float32(0.5) - (d - np.float32(self.radius)) / np.float32(cell_radius), 0, 1).astype(np.float32)
+
+
+class Union:
+    """union(Box(...), Box(...))  (phi/geom/_geom_ops.py:297-320): a point lies inside when it lies inside any member."""
+
+    def __init__(self, *geometries):
+        self.geometries = tuple(geometries)
+
+    def lies_inside(self, pts):
+        ok = np.zeros(pts.shape[:-1], bool)
+        for g in self.geometries:
+            ok |= g.lies_inside(pts)
+        return ok
+
+
+def union(*geometries):
+    """geom.union (phi/geom/_geom_ops.py:297-320): union(Box(x=(0, 10), y=(2, 3)), Box(x=(4.5, 5.5), y=(1, 4))) as Heat_Flow.ipynb builds its
+    bars.  Usable where a hard geometry mask is sampled (CenteredGrid(values=union(...)))."""
+    flat = []
+    for g in (geometries[0] if len(geometries) == 1 and isinstance(geometries[0], (list, tuple)) else geometries):
+        _require(isinstance(g, (Box, Sphere, Union)), f"union of {type(g).__name__}")
+        flat += list(g.geometries) if isinstance(g, Union) else [g]
+    return Union(*flat)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -318,7 +341,7 @@ class CenteredGrid(_Grid):
         self.vector_scale = _scale                       # s * (0, 0.1): a centred vector field that is a scalar times constants
         if _data is not None:
             self.data = _data
-        elif isinstance(values, (Box, Sphere)):
+        elif isinstance(values, (Box, Sphere, Union)):
             self.data = self.dom.centered_from_numpy(values.lies_inside(self.points()).astype(np.float32))
         elif np.isscalar(values):
             self.data = self.dom.alloc_centered()
@@ -645,9 +668,13 @@ def implicit(fld, diffusivity: float, dt: float, solve: Solve = None):
     unless solve.x0 is given), the constant boundary values entering as the bias of the affine system (_optimize.py:622, 645).
     A scalar CenteredGrid with any boundary, or a PERIODIC StaggeredGrid whose components are solved as separate systems, as the
     reference does (one record per batch entry and component, entry b * dim + c).  Returns a new field; SolveTape records,
-    NotConverged and Diverged as for make_incompressible."""
+    NotConverged and Diverged as for make_incompressible.
+    A CenteredGrid diffusivity on the same grid (batch 1 or the field's) diffuses a scalar CenteredGrid with a spatially varying k
+    (diffuse.py:129-141, Heat_Flow.ipynb): see _implicit_varying."""
     solve = solve or Solve('CG')
     plain = lambda v: isinstance(v, numbers.Real) and not isinstance(v, bool)
+    if isinstance(diffusivity, CenteredGrid) and isinstance(fld, CenteredGrid):
+        return _implicit_varying(fld, diffusivity, dt, solve)
     _require(plain(diffusivity) and plain(dt), "implicit diffusion with a Field / vector / per-batch diffusivity or dt")
     _require(solve.method == 'CG', f"solver '{solve.method}' for implicit diffusion")
     amount = float(diffusivity) * float(dt)
@@ -669,6 +696,24 @@ def implicit(fld, diffusivity: float, dt: float, solve: Solve = None):
     _finish_solve(fld.dom, solve)
     return fld.with_values(data)
 
+
+def _implicit_varying(fld, k, dt, solve: Solve):
+    """diffuse.implicit(fld, k, dt) with a CenteredGrid diffusivity k (phi/physics/diffuse.py:48-59, 90-95, 129-141): solves
+    sharpen(x) = explicit(x, k, -dt) = fld with CG.  Every face takes min(-dt k_lo, -dt k_hi) - for dt > 0 the face MAXIMUM of k - and
+    the coefficient ghosts follow fld's boundary, not k's own (amount.at(u), phi/field/_resample.py:56-63): a constant side with
+    value c gives min(-dt k_edge, c).  k must lie on fld's grid (no resampling) with batch 1 or fld's batch."""
+    _require(isinstance(dt, numbers.Real) and not isinstance(dt, bool), "implicit diffusion with a Field / vector / per-batch dt")
+    _require(solve.method == 'CG', f"solver '{solve.method}' for implicit diffusion")
+    _require(fld.vector_scale is None and k.vector_scale is None, "implicit diffusion of a vector field with a varying diffusivity")
+    _require(k.res == fld.res and k.lower == fld.lower and k.upper == fld.upper,
+             "a diffusivity on a different grid (it would need resampling)")
+    _require(k.batch in (1, fld.batch), f"a diffusivity with batch {k.batch} for a field with batch {fld.batch}")
+    if solve.x0 is not None:
+        _require(isinstance(solve.x0, CenteredGrid) and solve.x0._same_grid(fld), "x0 on a different grid")
+    data = ops.diffuse_implicit_varying(fld.dom, fld.spec, fld.data, k.data, float(dt), solve.rel_tol, solve.abs_tol, solve.max_iterations,
+                                        x0=solve.x0.data if solve.x0 is not None else None)
+    _finish_solve(fld.dom, solve)
+    return fld.with_values(data)
 
 
 diffuse = SimpleNamespace(explicit=explicit, implicit=implicit)

@@ -398,6 +398,42 @@ def diffuse_implicit(values, ext, dx, dims, resolution, amount: float, staggered
     return math.stack(pushed, channel(**{chan.name: tuple(item_names) if item_names else len(pushed)})), info
 
 
+def diffuse_implicit_varying(values, ext, dx, dims, resolution, diffusivity, dt: float, rel_tol=1e-5, abs_tol=1e-5, max_iterations=1000,
+                             x0=None):
+    """diffuse.implicit with a spatially varying diffusivity (phi/physics/diffuse.py:48-59, 90-95, 129-141) on the VALUES of a scalar
+    CenteredGrid.  diffusivity: the values of k on the same grid (the field's spatial dims and sizes, no channel dim, batch dims a
+    subset of the field's).  Every face takes min(-dt k_lo, -dt k_hi); the coefficient ghosts follow `ext` (amount.at(u),
+    phi/field/_resample.py:56-63).  Returns (new values, info dict with one record per batch entry)."""
+    math, _ = _phiml()
+    if math.get_precision() != 32:
+        raise NotEligible(f"precision {math.get_precision()} (fast path: 32; never silently downcast)")
+    if len(dims) not in (2, 3):
+        raise NotEligible(f"{len(dims)}-D grids")
+    if values.shape.channel.rank:
+        raise NotEligible(f"channel dims {values.shape.channel} with a varying diffusivity (the reference supports scalar fields only)")
+    if diffusivity.shape.channel.rank or diffusivity.shape.dual.rank or diffusivity.shape.instance.rank:
+        raise NotEligible(f"diffusivity dims {diffusivity.shape} (fast path: one value per cell; no anisotropic diffusivity)")
+    if tuple(sorted(diffusivity.shape.spatial.names)) != tuple(sorted(dims)) or \
+            any(diffusivity.shape.get_size(d) != n for d, n in zip(dims, resolution)):
+        raise NotEligible(f"diffusivity on a different grid ({diffusivity.shape.spatial}; it would need resampling)")
+    batch_shape = _batch_of(values, *([x0] if x0 is not None else []))
+    kb = diffusivity.shape.batch
+    if any(n not in batch_shape.names for n in kb.names):
+        raise NotEligible(f"diffusivity batch dims {kb} that the field does not have")
+    spec = to_spec(ext, dims)
+    dom = _domain(tuple(resolution), _dx_tuple(dx, dims), max(1, batch_shape.volume), None)
+    u = pull_centered(dom, values, batch_shape, dims)
+    x = pull_centered(dom, x0, batch_shape, dims) if x0 is not None else None
+    if kb.rank:
+        k = pull_centered(dom, diffusivity, batch_shape, dims)             # one k per entry (expanded over the field's other batch dims)
+    else:
+        k = pull_centered(_domain(tuple(resolution), _dx_tuple(dx, dims), 1, None), diffusivity, kb, dims)    # one k for every entry
+    out = ENGINE.diffuse_implicit_varying(dom, spec, u, k, float(dt), rel_tol, abs_tol, max_iterations, x0=x)
+    res = ENGINE.read_results(dom)
+    info = {k_: np.array(res[k_]) for k_ in ('iterations', 'converged', 'diverged', 'residual_sq', 'tol_sq')}
+    return push_centered(dom, out, batch_shape, dims), info
+
+
 def grid_sample_native(grid: torch.Tensor, coords: torch.Tensor, mode: str):
     """Backend.grid_sample contract (PhiML/phiml/backend/_backend.py:1578-1593): grid (batch, x, y[, z], channel), coordinates
     (batch, points..., d) in index space, mode in 'zeros' | 'boundary' | 'periodic'.  Anything else -> NotImplemented, the

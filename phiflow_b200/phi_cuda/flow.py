@@ -190,6 +190,10 @@ def implicit(field, diffusivity, dt, solve=Solve('CG'), gradient=None, upwind=No
             raise NotEligible("not a grid")
         if gradient is not None or upwind is not None:
             raise NotEligible("gradient / upwind (FVM arguments)")
+        k_values = _varying_diffusivity(field, diffusivity)
+        if k_values is not None:
+            return _implicit_varying(field, k_values, dt, solve, stock, (field, diffusivity, dt, original_solve, gradient, upwind,
+                                                                         correct_skew, gradient_for_diffusivity))
         amount = _number(diffusivity) * _number(dt)
         solve = solve.with_defaults('solve')
         if solve.method != 'CG' or solve.preconditioner is not None:
@@ -205,6 +209,48 @@ def implicit(field, diffusivity, dt, solve=Solve('CG'), gradient=None, upwind=No
         return _fall('diffuse.implicit', why, stock, field, diffusivity, dt, original_solve, gradient, upwind, correct_skew, gradient_for_diffusivity)
     out = field.with_values(values)
     _report(solve, info, out, info.pop('components'))
+    return out
+
+
+def _varying_diffusivity(field, diffusivity):
+    """The values of a spatially varying diffusivity (diffuse.py:129-141: a centred Field, or a Tensor with spatial dims), None for
+    anything else (plain numbers and per-batch values take the numeric path).  A Field must lie on `field`'s grid: the fast path does
+    not resample (amount.at(u), phi/field/_resample.py:56-63, is then the identity apart from the boundary takeover)."""
+    if isinstance(diffusivity, _Field):
+        if not diffusivity.is_grid or diffusivity.is_staggered:
+            raise NotEligible("a diffusivity Field that is not a CenteredGrid (it would need resampling)")
+        try:
+            same = _grid_info(diffusivity)[:2] == _grid_info(field)[:2] and bool(diffusivity.bounds == field.bounds)
+        except (TypeError, ValueError, AttributeError):
+            same = False
+        if not same:
+            raise NotEligible("a diffusivity on a different grid (bounds / resolution; it would need resampling)")
+        return diffusivity.values
+    if isinstance(diffusivity, _math.Tensor) and diffusivity.shape.spatial.rank:
+        return diffusivity
+    return None
+
+
+def _implicit_varying(field, k_values, dt, solve, stock, stock_args):
+    """diffuse.implicit with a varying diffusivity, fast path for a scalar CenteredGrid (its values' channel-free shape), Solve('CG')."""
+    try:
+        if field.is_staggered:
+            raise NotEligible("StaggeredGrid with a varying diffusivity (the reference raises NotImplementedError, diffuse.py:137-138)")
+        dt = _number(dt)
+        solve = solve.with_defaults('solve')
+        if solve.method != 'CG' or solve.preconditioner is not None:
+            raise NotEligible(f"solver '{solve.method}' / preconditioner {solve.preconditioner} (fast path: Solve('CG'))")
+        dims, res, dx = _grid_info(field)
+        x0 = solve.x0.values if isinstance(solve.x0, _Field) else None
+        if solve.x0 is not None and x0 is None:
+            raise NotEligible("x0 that is not a Field")
+        values, info = _adapter.diffuse_implicit_varying(field.values, field.extrapolation, dx, dims, res, k_values, dt,
+                                                         rel_tol=float(solve.rel_tol), abs_tol=float(solve.abs_tol),
+                                                         max_iterations=int(_math.max(solve.max_iterations)), x0=x0)
+    except (NotEligible, TypeError, ValueError) as why:
+        return _fall('diffuse.implicit', why, stock, *stock_args)
+    out = field.with_values(values)
+    _report(solve, info, out)
     return out
 
 
