@@ -29,12 +29,13 @@ struct CgShared {                   // per-thread view of the CTA's shared memor
     int* iters;
     int* any_cont;
     unsigned char *cont, *conv, *divg;
+    float* bprev;                  // beta of the previous iteration (one-sweep ring CG: r_k = d_k - beta_k d_{k-1})
 };
 
 __host__ __device__ inline size_t cg_smem_bytes(int batch)
 {
     const size_t b8 = ((size_t)batch + 1) / 2 * 2;      // keep 8-byte alignment of what follows
-    return 2 * 32 * sizeof(double) + 3 * b8 * sizeof(double) + 7 * b8 * sizeof(float)
+    return 2 * 32 * sizeof(double) + 3 * b8 * sizeof(double) + 8 * b8 * sizeof(float)
          + (b8 + 2) * sizeof(int) + 3 * (b8 + 16);
 }
 
@@ -58,7 +59,8 @@ __device__ __forceinline__ CgShared cg_carve(unsigned char* base, int batch)
     sh.any_cont = (int*)p; p += 2 * sizeof(int);
     sh.cont = p; p += b8 + 16;
     sh.conv = p; p += b8;
-    sh.divg = p;
+    sh.divg = p; p += (b8 + 3) / 4 * 4;            // divg starts 4-byte aligned (b8 is even)
+    sh.bprev = (float*)p;
     return sh;
 }
 

@@ -299,13 +299,13 @@ static int cg_grid_size(int dim, int batch, bool mask, int* blocks_per_sm_out)
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-// workspace layout: r | d0 | d1 | partials[4][2][batch][max_grid] | d2 | r1  (d2, r1 and partial slots 4..7: one-sweep ring CG)
+// workspace layout: r | d0 | d1 | partials[4][2][batch][max_grid] | d2  (d2 and partial slots 4..7: one-sweep ring CG)
 
 size_t phi_cg_workspace_bytes(const DGrid& g)
 {
     const size_t pf_sb = (size_t)g.cext[0] * g.cext[1] * g.cext[2];
     const size_t arr = align_up((size_t)pf_sb * g.batch * sizeof(float), 256);
-    return 5 * arr + align_up((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double), 256);
+    return 4 * arr + align_up((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double), 256);
 }
 
 int phi_launch_cg(const CgLaunch& l, cudaStream_t s)

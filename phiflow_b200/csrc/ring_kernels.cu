@@ -823,7 +823,7 @@ struct CgRingArgs {
     int ring_smem_offset;        // byte offset of the ring inside dynamic shared memory (after the CgShared block)
     int comm_merge;              // multi-GPU: 1 = merged barrier + all-reduce (comm_barrier_allreduce), 0 = grid.sync + comm_allreduce
     CommDev cm;
-    float* d2; float* r1;        // one-sweep CG: third direction buffer, second residual buffer
+    float* d2;                   // one-sweep CG: third direction buffer
     float helm_a;                // HELM (diffuse.implicit): operator I - helm_a * L0
     const float* k; int kbcast;  // VARK (varying diffusivity): k per batch entry, or (kbcast) entry 0 for all
     float ndt;                   // VARK: -dt
@@ -964,11 +964,13 @@ __device__ __forceinline__ void ring_unit_cells(const RingCfg& cfg, const DGrid&
 // and sums d_{k+1}.q_{k+1}, |r_{k+1}|^2, r_{k+1}.q_{k+1}, |q_{k+1}|^2.  After the one grid barrier alpha_{k+1} = |r_{k+1}|^2 / d.q and
 // beta_{k+2} = (|r_{k+1}|^2 - 2 alpha r.q + alpha^2 |q|^2) / |r_{k+1}|^2 (= |r_{k+2}|^2 / |r_{k+1}|^2 in exact arithmetic).  The
 // stopping rule still uses the true |r_{k+1}|^2, and the look-ahead is rebuilt from it every iteration, so its rounding does not
-// accumulate.  Bytes per iteration: d_k, r_k read, d_{k+1}, r_{k+1} written (16 B/cell) + x += alpha_{k-1} d_{k-1} + alpha_k d_k
-// every second iteration (12 B/cell) = 22 B/cell, against 30 for the two sweeps of k_cg_ring.
-// Stage layout: d_k (TY+4 lines: halo 2 in y, because d_{k+1} is needed on the halo lines), r_k (TY+2 lines), x and d_{k-1} (TY
-// lines each, fetched on x-update iterations only).  d_{k+1} of each plane goes to a triple-buffered shared tile (TY+2 lines) from
-// which the q_{k+1} stencil takes its y and warp-edge x neighbours; consumers sync on a named barrier once per plane.
+// accumulate.  r is not stored: the previous pass formed d_k = r_k + beta_k d_{k-1}, so r_k = d_k - beta_k d_{k-1} is recovered in
+// registers (its rounding error is relative to |d_k|, a small multiple of |r_k|, and does not grow with k; r_0 = d_0).  Bytes per
+// iteration: d_k, d_{k-1} read, d_{k+1} written (12 B/cell) + x += alpha_{k-1} d_{k-1} + alpha_k d_k every second iteration, with
+// d_{k-1} already staged (8 B/cell) = 16 B/cell, against 30 for the two sweeps of k_cg_ring.
+// Stage layout: d_k (TY+4 lines: halo 2 in y, because d_{k+1} is needed on the halo lines), d_{k-1} (TY+2 lines, not fetched in
+// iteration 0), x (TY lines, fetched on x-update iterations only).  d_{k+1} of each plane goes to a triple-buffered shared tile
+// (TY+2 lines) from which the q_{k+1} stencil takes its y and warp-edge x neighbours; consumers sync on a named barrier once per plane.
 // Only for 3-D, the branch-free tiling, periodic y and z, one GPU, CG without matrix offset or obstacles (phi_launch_cg_ring).
 #define RING_GF 3                // consumer groups per thread on the haloed (TY+2)-line region: (TY + 2) * nx4 <= RING_GF * 256
 #define FUSED_TILE_BUFS 3
@@ -1003,8 +1005,9 @@ __device__ __forceinline__ void fused_groups_init(FusedGroups& fg, const RingCfg
     }
 }
 
-// Producer of pass F.  Staged line slots: d (TY+4 lines from y0-2), r (TY+2 from y0-1), x (TY), d_{k-1} (TY).  Category 0 (d) is
-// fetched on every plane of the unit, 1 (r) on planes z0-1 .. z1, 2 (x, d_{k-1}) on the owned planes of x-update iterations.
+// Producer of pass F.  Staged line slots: d_k (TY+4 lines from y0-2), d_{k-1} (TY+2 from y0-1), x (TY).  Category 0 (d_k) is fetched
+// on every plane of the unit, 1 (d_{k-1}) on planes z0-1 .. z1, 2 (x) on the owned planes of x-update iterations.  A null source
+// (d_{k-1} in iteration 0, x on other iterations) is not fetched.
 struct ProdUnitF {
     long long yoff[4];
     const float* base[4];
@@ -1015,14 +1018,14 @@ struct ProdUnitF {
 };
 
 __device__ __forceinline__ void prod_fused_setup(ProdUnitF& pu, const RingCfg& cfg, const DGrid& g, const DField& pf,
-                                                 const float* d, const float* r, const float* x, const float* dprev, int b, int y0)
+                                                 const float* d, const float* dprev, const float* x, int b, int y0)
 {
     const int lane = threadIdx.x & 31, TY = cfg.TY;
     const uint32_t row_bytes = (uint32_t)cfg.pitch * 4u;
     const bool mergeable = cfg.merge && pf.sy == cfg.pitch;
-    const int rows[4] = {TY + 4, TY + 2, TY, TY};
-    const int ylo[4] = {y0 - 2, y0 - 1, y0, y0};
-    const float* src[4] = {d, r, x, dprev};
+    const int rows[3] = {TY + 4, TY + 2, TY};
+    const int ylo[3] = {y0 - 2, y0 - 1, y0};
+    const float* src[3] = {d, dprev, x};
     int cnt[3] = {0, 0, 0};
     pu.m[0] = pu.m[1] = pu.m[2] = 0;
 #pragma unroll
@@ -1031,7 +1034,7 @@ __device__ __forceinline__ void prod_fused_setup(ProdUnitF& pu, const RingCfg& c
         pu.yoff[it] = 0; pu.base[it] = nullptr; pu.dsto[it] = 0; pu.nbytes[it] = row_bytes;
         int key = -1, yv = 0, first = 0;
 #pragma unroll
-        for (int arr = 0; arr < 4; ++arr) {
+        for (int arr = 0; arr < 3; ++arr) {
             if (key < 0 && line >= first && line < first + rows[arr] && src[arr]) {
                 int yy = ylo[arr] + (line - first); float cv;
                 phi_resolve(yy, pf, 1, cv);                         // periodic in y: always a stored line
@@ -1042,7 +1045,7 @@ __device__ __forceinline__ void prod_fused_setup(ProdUnitF& pu, const RingCfg& c
             }
             first += rows[arr];
         }
-        cnt[0] += key == 0; cnt[1] += key == 1; cnt[2] += key >= 2;       // categories: d, r, x and d_{k-1}
+        cnt[0] += key == 0; cnt[1] += key == 1; cnt[2] += key == 2;       // categories: d_k, d_{k-1}, x
         const int pkey = __shfl_up_sync(0xffffffffu, key, 1), pyv = __shfl_up_sync(0xffffffffu, yv, 1);
         const bool cont = mergeable && key >= 0 && lane > 0 && pkey == key && pyv + 1 == yv;
         const unsigned cm = __ballot_sync(0xffffffffu, cont);
@@ -1060,7 +1063,7 @@ __device__ __forceinline__ void prod_fused_setup(ProdUnitF& pu, const RingCfg& c
     }
 }
 
-__device__ __forceinline__ void ring_produce_fused(Ring& rg, const RingCfg& cfg, const DField& pf, const ProdUnitF& pu, int z, bool rplane, bool eplane)
+__device__ __forceinline__ void ring_produce_fused(Ring& rg, const RingCfg& cfg, const DField& pf, const ProdUnitF& pu, int z, bool pplane, bool eplane)
 {
     const int lane = threadIdx.x & 31;
     const int slot = rg.pos.slot;
@@ -1069,8 +1072,8 @@ __device__ __forceinline__ void ring_produce_fused(Ring& rg, const RingCfg& cfg,
     float cv;
     phi_resolve(z, pf, 2, cv);                                      // periodic in z
     const long long zoff = (long long)z * pf.sz;
-    const unsigned mask = pu.m[0] | (rplane ? pu.m[1] : 0u) | (eplane ? pu.m[2] : 0u);
-    const int cnt = pu.tot[0] + (rplane ? pu.tot[1] : 0) + (eplane ? pu.tot[2] : 0);
+    const unsigned mask = pu.m[0] | (pplane ? pu.m[1] : 0u) | (eplane ? pu.m[2] : 0u);
+    const int cnt = pu.tot[0] + (pplane ? pu.tot[1] : 0) + (eplane ? pu.tot[2] : 0);
     if (lane == 0) {
         mbar_wait(rg.empty0 + 8 * slot, rg.pos.par ^ 1u);
         mbar_expect_tx(full, (uint32_t)cnt * (uint32_t)cfg.pitch * 4u);
@@ -1102,9 +1105,9 @@ __device__ __forceinline__ float4 stencil7(const float4& c, float xl, float xr, 
 }
 
 struct FusedPass {
-    const float* d; const float* r; const float* dprev;    // d_k, r_k, d_{k-1}
-    float* dn; float* rn; float* x;                       // d_{k+1}, r_{k+1}, solution (x == nullptr: no x update this iteration)
-    float alpha, aprev, beta;
+    const float* d; const float* dprev;                   // d_k, d_{k-1} (nullptr in iteration 0, where r_0 = d_0)
+    float* dn; float* x;                                  // d_{k+1}, solution (x == nullptr: no x update this iteration)
+    float alpha, aprev, beta, bprev;                      // alpha_k, alpha_{k-1}, beta_{k+1}, beta_k
 };
 
 // One unit of pass F: producer warp streams planes z0-2 .. z1+1, consumers march planes p = z0-1 .. z1 (d_{k+1} on the haloed
@@ -1115,17 +1118,18 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
     const int nz = u.z1 - u.z0;
     if ((int)threadIdx.x >= cfg.consumers) {
         ProdUnitF pu;
-        prod_fused_setup(pu, cfg, g, pf, P.d, P.r, P.x, P.dprev, u.b, u.y0);
+        prod_fused_setup(pu, cfg, g, pf, P.d, P.dprev, P.x, u.b, u.y0);
         for (int p = 0; p < nz + 4; ++p)
             ring_produce_fused(rg, cfg, pf, pu, u.z0 - 2 + p, p >= 1 && p <= nz + 2, P.x && p >= 2 && p <= nz + 1);
         return;
     }
     const int pitch = cfg.pitch, TY = cfg.TY;
-    const int rb = (TY + 4) * pitch, xb = (2 * TY + 6) * pitch - pitch, pb = (3 * TY + 6) * pitch - pitch;
+    const int pb = (TY + 4) * pitch, xb = (2 * TY + 6) * pitch - pitch;
     const int tsz = (TY + 2) * pitch;
     const float ix2 = g.inv_dx2[0], iy2 = g.inv_dx2[1], iz2 = g.inv_dx2[2];
     const float cc = 2.f * (ix2 + iy2 + iz2);
-    const float alpha = P.alpha, aprev = P.aprev, beta = P.beta;
+    const float alpha = P.alpha, aprev = P.aprev, beta = P.beta, bprev = P.bprev;
+    const bool has_prev = P.dprev != nullptr;
     long long plane_off = (long long)u.b * pf.sb + (long long)u.y0 * pf.sy + (long long)u.z0 * pf.sz - pf.sz;   // plane z0 - 1
 
     float4 dm[RING_GF], dc[RING_GF];             // d_k on planes p-1, p (own cells of the haloed region)
@@ -1164,18 +1168,20 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
             xl = (fg.needl & (1u << k)) ? el : xl;
             xr = (fg.needr & (1u << k)) ? er : xr;
             const float4 q = stencil7(c, xl, xr, ym, yp, dm[k], zp, ix2, iy2, iz2, cc);
-            float4 rv = lds4(sc, rb + fg.t[k]);
+            float4 rv = c, dp = f4_splat(0.f);                 // r_k = d_k - beta_k d_{k-1}; r_0 = d_0 (d_{k-1} slot not staged)
+            if (has_prev) {
+                dp = lds4(sc, pb + fg.t[k]);
+                rv = make_float4(fmaf(-bprev, dp.x, c.x), fmaf(-bprev, dp.y, c.y), fmaf(-bprev, dp.z, c.z), fmaf(-bprev, dp.w, c.w));
+            }
             rv.x = fmaf(-alpha, q.x, rv.x); rv.y = fmaf(-alpha, q.y, rv.y); rv.z = fmaf(-alpha, q.z, rv.z); rv.w = fmaf(-alpha, q.w, rv.w);
             const float4 dv = make_float4(fmaf(beta, c.x, rv.x), fmaf(beta, c.y, rv.y), fmaf(beta, c.z, rv.z), fmaf(beta, c.w, rv.w));
             *reinterpret_cast<float4*>(tw + fg.t[k]) = dv;
             if (own && (fg.inner & (1u << k))) {
                 const long long off = plane_off + fg.goff[k];
-                *reinterpret_cast<float4*>(P.rn + off) = rv;
                 *reinterpret_cast<float4*>(P.dn + off) = dv;
                 acc[1] += dot4(rv, rv);
-                if (P.x) {
+                if (P.x) {                                   // odd k: d_{k-1} is staged
                     float4 xv = lds4(sc, xb + fg.t[k]);
-                    const float4 dp = lds4(sc, pb + fg.t[k]);
                     xv.x += aprev * dp.x; xv.y += aprev * dp.y; xv.z += aprev * dp.z; xv.w += aprev * dp.w;
                     xv.x += alpha * c.x; xv.y += alpha * c.y; xv.z += alpha * c.z; xv.w += alpha * c.w;
                     *reinterpret_cast<float4*>(P.x + off) = xv;
@@ -1348,10 +1354,8 @@ k_cg_ring(CgRingArgs A)
 
     if constexpr (FUSED) {
         static_assert(DIM == 3 && !GENERIC && !DIST && !ADAPT && !MASK, "the one-sweep CG is 3-D, branch-free, single-GPU CG only");
-        // d_k lives in D[k % 3], r_k in Rb[k % 2]: pass k reads d_k, r_k with halos while other CTAs write d_{k+1}, r_{k+1}, and
-        // d_{k-1} is still needed for the x update
+        // d_k lives in D[k % 3]: pass k reads d_k and d_{k-1} with halos while other CTAs write d_{k+1}.  a.r holds r_0 only.
         float* const D[3] = {a.d0, a.d1, A.d2};
-        float* const Rb[2] = {a.r, A.r1};
         float* const tile = rg.stage0 + (size_t)cfg.R * cfg.stage_floats;
         FusedGroups fg;
         fused_groups_init(fg, cfg, g, a.pf);
@@ -1371,6 +1375,7 @@ k_cg_ring(CgRingArgs A)
                 const double nxt = dl - 2.0 * al * dq + (double)al * al * sh.sum1[b];
                 sh.alpha[b] = al;
                 sh.beta[b] = (dl != 0.0) ? (float)(nxt / dl) : 0.f;
+                sh.bprev[b] = 0.f;
             }
             __syncthreads();
         }
@@ -1378,8 +1383,8 @@ k_cg_ring(CgRingArgs A)
         int reg = 1;                                 // pass F sums go to partial slots 4 reg .. 4 reg + 3; the 2-sum sweeps used 0 .. 3
         for (int k = 0; *sh.any_cont; ++k) {
             FusedPass P;
-            P.d = D[k % 3]; P.r = Rb[k & 1]; P.dprev = D[(k + 2) % 3];
-            P.dn = D[(k + 1) % 3]; P.rn = Rb[(k + 1) & 1]; P.x = (k & 1) ? a.x : nullptr;
+            P.d = D[k % 3]; P.dprev = k > 0 ? D[(k + 2) % 3] : nullptr;
+            P.dn = D[(k + 1) % 3]; P.x = (k & 1) ? a.x : nullptr;
             int cur_b = cfg.split ? 0 : -1;
             float acc[4] = {0.f, 0.f, 0.f, 0.f};
             RingUnit u;
@@ -1390,7 +1395,7 @@ k_cg_ring(CgRingArgs A)
                                       flush_partials(sh, a.partials, 2 * reg + 1, batch, cur_b, acc[2], acc[3]); }
                     cur_b = u.b; acc[0] = acc[1] = acc[2] = acc[3] = 0.f;
                 }
-                P.alpha = sh.alpha[u.b]; P.aprev = sh.aprev[u.b]; P.beta = sh.beta[u.b];
+                P.alpha = sh.alpha[u.b]; P.aprev = sh.aprev[u.b]; P.beta = sh.beta[u.b]; P.bprev = sh.bprev[u.b];
                 ring_fused_unit(rg, cfg, g, a.pf, fg, P, tile, u, acc);
             }
             if (cur_b >= 0) { flush_partials(sh, a.partials, 2 * reg, batch, cur_b, acc[0], acc[1]);
@@ -1411,6 +1416,7 @@ k_cg_ring(CgRingArgs A)
                 sh.cont[b] = (!conv && !divg && it < a.prm.max_iter) ? 1 : 0;
                 if (sh.cont[b]) {                    // an entry that stops keeps alpha_k: the x step it may still owe
                     sh.aprev[b] = sh.alpha[b];
+                    sh.bprev[b] = sh.beta[b];
                     sh.alpha[b] = (dq != 0.0) ? (float)(dn / dq) : 0.f;
                 }
             }
@@ -1744,10 +1750,10 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
         const DField& pf = l.pf;
         if (!(e && atoi(e) == 2) && g.dim == 3 && !generic && !dist && !adapt && !mask && !helm && l.prm.matrix_offset == 0.f
             && pf.klo[1] == PHI_BC_PERIODIC && pf.khi[1] == PHI_BC_PERIODIC && pf.klo[2] == PHI_BC_PERIODIC && pf.khi[2] == PHI_BC_PERIODIC) {
-            // stage = d (TY+4) + r (TY+2) + x (TY) + d_{k-1} (TY) lines; the d_{k+1} tile is reserved at the largest TY ring_config may pick
+            // stage = d_k (TY+4) + d_{k-1} (TY+2) + x (TY) lines; the d_{k+1} tile is reserved at the largest TY ring_config may pick
             RingCfg fc;
-            if (ring_config(g, 4, 6, cgs, 4, RING_MAX_STAGES, sms, &fc, RING_CONSUMERS, 4)
-                && ring_config(g, 4, 6, cgs + FUSED_TILE_BUFS * (fc.TY + 2) * fc.pitch * 4, 4, RING_MAX_STAGES, sms, &fc, RING_CONSUMERS, 4)
+            if (ring_config(g, 3, 6, cgs, 4, RING_MAX_STAGES, sms, &fc, RING_CONSUMERS, 4)
+                && ring_config(g, 3, 6, cgs + FUSED_TILE_BUFS * (fc.TY + 2) * fc.pitch * 4, 4, RING_MAX_STAGES, sms, &fc, RING_CONSUMERS, 4)
                 && ring_all_fast(g, pf, fc) && (fc.TY + 2) * fc.nx4 <= RING_GF * fc.consumers) {
                 fused = true;
                 A.cfg = fc;
@@ -1807,7 +1813,7 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     a.r = (float*)ws + hoff; a.d0 = (float*)(ws + arr) + hoff; a.d1 = (float*)(ws + 2 * arr) + hoff;
     a.partials = (double*)(ws + 3 * arr);
     const size_t pbytes = ((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double) + 255) / 256 * 256;
-    A.d2 = (float*)(ws + 3 * arr + pbytes) + hoff; A.r1 = (float*)(ws + 4 * arr + pbytes) + hoff;
+    A.d2 = (float*)(ws + 3 * arr + pbytes) + hoff;
     A.helm_a = l.helm_amount;
     A.k = l.helm_k; A.kbcast = l.helm_k_bcast ? 1 : 0; A.ndt = l.helm_ndt;
     for (int d = 0; d < 3; ++d) { A.kclo[d] = l.helm_kclo[d]; A.kchi[d] = l.helm_kchi[d]; }

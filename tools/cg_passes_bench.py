@@ -6,8 +6,9 @@
 The plume of bench.py is advanced `--warmup` steps; then, `--rounds` times, each form (PHICUDA_CG_PASSES unset = one sweep per
 iteration where it applies, =2 = two sweeps) runs the next plume step from the same saved state, in alternating order.  Reported per
 form: the pressure solve's time (CUDA events recorded by the library around the solve), its iterations, and the achieved HBM rate
-for the algorithmic byte counts cells * (22 it + 40) (one-sweep: 16 B/cell per iteration + the x update every second iteration;
-set-up passes 32 + the q_0 sweep 8) and cells * (30 it + 32) (two-sweep, the count bench.py reports)."""
+for the algorithmic byte counts cells * (16 it + 40) (one-sweep: d_k, d_{k-1} read and d_{k+1} written, 12 B/cell per iteration, +
+the x read and write every second iteration; set-up passes 32 + the q_0 sweep 8) and cells * (30 it + 32) (two-sweep, the count
+bench.py reports)."""
 import argparse
 import json
 import os
@@ -78,7 +79,7 @@ def main():
             'step_ms_median': float(np.median([r['step_ms'] for r in rs])),
             'iterations': sorted(set(int(i) for i in it)),
             'ms_per_iteration': float(np.median(ms / it)),
-            'gbs_at_22B': float(np.median(cells * (22.0 * it + 40.0) / t / 1e9)),
+            'gbs_at_16B': float(np.median(cells * (16.0 * it + 40.0) / t / 1e9)),
             'gbs_at_30B': float(np.median(cells * (30.0 * it + 32.0) / t / 1e9)),
             'ring': {k: rs[0][k] for k in ('TY', 'stages', 'split', 'grid_ctas')}}
     out['speedup_cg_median'] = out['2_sweep']['cg_ms_per_solve']['median'] / out['1_sweep']['cg_ms_per_solve']['median']
