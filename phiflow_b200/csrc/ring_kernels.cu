@@ -1731,6 +1731,9 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     // lines staged per stage: pass B (even) = 1 haloed + 3 element-wise arrays = 4 TY + 2; with the obstacle mask (or the
     // diffusivity) as an extra haloed array 5 TY + 4 (pass A: 3 haloed = 3 TY + 6)
     if (!ring_config(g, xslot ? 5 : 4, xslot ? 6 : 2, cgs, g.dim == 3 ? (xslot ? 3 : 4) : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
+    // pass A of CG-adaptive stages 2 haloed + 1 element-wise array = 3 TY + 4 lines: one line more than 4 TY + 2 at TY = 1
+    if (l.prm.method == PHI_SOLVER_CG_ADAPTIVE && !xslot && A.cfg.TY == 1
+        && !ring_config(g, 4, 3, cgs, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
     const int threads = RING_THREADS;
     A.ring_smem_offset = cgs;
     int per_sm = 0;
