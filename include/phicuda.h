@@ -266,7 +266,7 @@ int phicuda_make_incompressible_centered_host_f32(const PhiGrid* g, const PhiVBC
  * make_incompressible_masked = divergence * active, CG on masked_laplace (faces touching an obstacle carry no flux,
  * obstacle cells are identity rows), v -= hard_bcs * grad p.  The caller applies apply_boundary_conditions first
  * (v *= 1 - obstacle mask at faces: phicuda_mul_faces_f32).  The solve runs on the TMA-ring kernel with the mask staged as an
- * extra haloed array (k_cg_ring<..., MASK>; 5 lines per tile line and stage instead of 4); grids whose lines do not fit the
+ * extra haloed array (k_cg_ring<..., CgOp::Masked>; 5 lines per tile line and stage instead of 4); grids whose lines do not fit the
  * ring fall back to the register-marching kernel. */
 int phicuda_mul_faces_f32(const PhiGrid* g, const PhiVBC* vbc, float* const v[3], const float* const mask[3], void* stream);
 /* the two stencil pieces of the masked projection on their own (z-slab runs exchange halo planes between them):

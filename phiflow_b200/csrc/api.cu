@@ -380,7 +380,7 @@ int phicuda_cg_poisson_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const flo
     CHECK(accessible_field(g, vbc, &af));
     CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &l.pf));
     l.rhs = rhs; l.x = x; l.prm = *prm; l.result = result; l.workspace = workspace; l.workspace_bytes = workspace_bytes;
-    l.acc = accessible;
+    l.op.kind = CgOp::Masked; l.op.mask = accessible;
     return phi_launch_cg(l, (cudaStream_t)stream);
 }
 
@@ -403,7 +403,7 @@ size_t phicuda_cg_workspace_bytes(const PhiGrid* g)
 {
     DGrid dg;
     if (phi_make_dgrid(g, &dg)) return 0;
-    return phi_cg_workspace_bytes(dg);
+    return phi_cg_workspace(dg, nullptr).bytes;
 }
 
 int phicuda_cg_poisson_f32(const PhiGrid* g, const PhiVBC* vbc, const float* rhs, float* x,
@@ -441,8 +441,9 @@ int phicuda_diffuse_implicit_f32(const PhiGrid* g, const PhiVBC* bc, int32_t com
                 phi_set_error("diffuse_implicit: boundary kinds must agree between components (axis %d)", a); return PHI_ERR_UNSUPPORTED;
             }
     }
-    if (workspace_bytes < phi_cg_workspace_bytes(l.g)) { phi_set_error("diffuse_implicit: workspace %zu < %zu bytes", workspace_bytes, phi_cg_workspace_bytes(l.g)); return PHI_ERR_WORKSPACE; }
-    if (!phi_ring_enabled() || !phi_cg_ring_fits(l.g)) {
+    const size_t ws_need = phi_cg_workspace(l.g, nullptr).bytes;
+    if (workspace_bytes < ws_need) { phi_set_error("diffuse_implicit: workspace %zu < %zu bytes", workspace_bytes, ws_need); return PHI_ERR_WORKSPACE; }
+    if (!phi_ring_enabled() || !phi_cg_ring_fits(l.g, CgOp::Helmholtz)) {
         phi_set_error("diffuse_implicit: the grid does not fit the TMA-ring CG (batch <= 1024, grid lines short enough); this operator has no other kernel");
         return PHI_ERR_UNSUPPORTED;
     }
@@ -451,7 +452,7 @@ int phicuda_diffuse_implicit_f32(const PhiGrid* g, const PhiVBC* bc, int32_t com
     CHECK(phi_make_centered(g, &zero, &l.pf));
     for (int c = components; c < 3; ++c) cf[c] = l.pf;
     l.rhs = y; l.x = x; l.prm = *prm; l.result = result; l.workspace = workspace; l.workspace_bytes = workspace_bytes;
-    l.helm = true; l.helm_amount = amount;
+    l.op.kind = CgOp::Helmholtz; l.op.amount = amount;
     const int e = phi_launch_diffuse_implicit(l, components, cf, (cudaStream_t)stream);
     if (e == -100) { phi_set_error("diffuse_implicit: the grid does not fit the TMA-ring CG on this device"); return PHI_ERR_UNSUPPORTED; }
     return cuda_fail(e, "diffuse_implicit");
@@ -475,8 +476,9 @@ int phicuda_diffuse_implicit_varying_f32(const PhiGrid* g, const PhiBC* bc, cons
     }
     if (g->halo != 0) { phi_set_error("diffuse_implicit_varying: z-slab grids are not supported"); return PHI_ERR_UNSUPPORTED; }
     CHECK(phi_make_centered(g, bc, &cf));
-    if (workspace_bytes < phi_cg_workspace_bytes(l.g)) { phi_set_error("diffuse_implicit_varying: workspace %zu < %zu bytes", workspace_bytes, phi_cg_workspace_bytes(l.g)); return PHI_ERR_WORKSPACE; }
-    if (!phi_ring_enabled() || !phi_cg_ring_fits(l.g, true)) {
+    const size_t ws_need = phi_cg_workspace(l.g, nullptr).bytes;
+    if (workspace_bytes < ws_need) { phi_set_error("diffuse_implicit_varying: workspace %zu < %zu bytes", workspace_bytes, ws_need); return PHI_ERR_WORKSPACE; }
+    if (!phi_ring_enabled() || !phi_cg_ring_fits(l.g, CgOp::HelmholtzVarying)) {
         phi_set_error("diffuse_implicit_varying: the grid does not fit the TMA-ring CG (batch <= 1024, grid lines short enough); this operator has no other kernel");
         return PHI_ERR_UNSUPPORTED;
     }
@@ -484,12 +486,12 @@ int phicuda_diffuse_implicit_varying_f32(const PhiGrid* g, const PhiBC* bc, cons
     for (int a = 0; a < 3; ++a) { zero.clo[a] = 0.f; zero.chi[a] = 0.f; }    // the bias and the coefficient ghosts
     CHECK(phi_make_centered(g, &zero, &l.pf));
     l.rhs = y; l.x = x; l.prm = *prm; l.result = result; l.workspace = workspace; l.workspace_bytes = workspace_bytes;
-    l.helm = true; l.helm_k = diffusivity; l.helm_k_bcast = diffusivity_batch == 1 && g->batch > 1; l.helm_ndt = -dt;
+    l.op.kind = CgOp::HelmholtzVarying; l.op.k = diffusivity; l.op.kbcast = diffusivity_batch == 1 && g->batch > 1; l.op.ndt = -dt;
     for (int a = 0; a < 3; ++a) {
-        l.helm_kclo[a] = a < g->dim && cf.klo[a] == PHI_BC_CONST ? cf.clo[a] : 0.f;
-        l.helm_kchi[a] = a < g->dim && cf.khi[a] == PHI_BC_CONST ? cf.chi[a] : 0.f;
+        l.op.kclo[a] = a < g->dim && cf.klo[a] == PHI_BC_CONST ? cf.clo[a] : 0.f;
+        l.op.kchi[a] = a < g->dim && cf.khi[a] == PHI_BC_CONST ? cf.chi[a] : 0.f;
     }
-    const int e = phi_launch_diffuse_implicit_varying(l, (cudaStream_t)stream);
+    const int e = phi_launch_diffuse_implicit(l, 1, &cf, (cudaStream_t)stream);
     if (e == -100) { phi_set_error("diffuse_implicit_varying: the grid does not fit the TMA-ring CG on this device"); return PHI_ERR_UNSUPPORTED; }
     return cuda_fail(e, "diffuse_implicit_varying");
 }

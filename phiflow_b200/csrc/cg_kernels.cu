@@ -299,21 +299,28 @@ static int cg_grid_size(int dim, int batch, bool mask, int* blocks_per_sm_out)
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
-// workspace layout: r | d0 | d1 | partials[4][2][batch][max_grid] | d2  (d2 and partial slots 4..7: one-sweep ring CG)
-
-size_t phi_cg_workspace_bytes(const DGrid& g)
+CgWorkspace phi_cg_workspace(const DGrid& g, void* base)
 {
-    const size_t pf_sb = (size_t)g.cext[0] * g.cext[1] * g.cext[2];
-    const size_t arr = align_up((size_t)pf_sb * g.batch * sizeof(float), 256);
-    return 4 * arr + align_up((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double), 256);
+    const size_t arr = align_up((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float), 256);
+    const size_t pbytes = align_up((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double), 256);
+    CgWorkspace w = {};
+    w.bytes = 4 * arr + pbytes;
+    if (!base) return w;
+    unsigned char* ws = (unsigned char*)base;
+    const size_t hoff = (size_t)g.halo * g.cext[0] * g.cext[1];
+    w.r = (float*)ws + hoff; w.d0 = (float*)(ws + arr) + hoff; w.d1 = (float*)(ws + 2 * arr) + hoff;
+    w.partials = (double*)(ws + 3 * arr);
+    w.d2 = (float*)(ws + 3 * arr + pbytes) + hoff;
+    return w;
 }
 
 int phi_launch_cg(const CgLaunch& l, cudaStream_t s)
 {
     const DGrid& g = l.g;
     if (g.batch > CG_MAX_BATCH) { phi_set_error("cg: batch %d exceeds %d (split the batch)", g.batch, CG_MAX_BATCH); return PHI_ERR_UNSUPPORTED; }
-    if (l.workspace_bytes < phi_cg_workspace_bytes(g)) { phi_set_error("cg: workspace %zu < %zu bytes", l.workspace_bytes, phi_cg_workspace_bytes(g)); return PHI_ERR_WORKSPACE; }
-    const bool mask = l.acc != nullptr;              // obstacles: register-marching kernel (the TMA ring has no mask variant yet)
+    const CgWorkspace w = phi_cg_workspace(g, l.workspace);
+    if (l.workspace_bytes < w.bytes) { phi_set_error("cg: workspace %zu < %zu bytes", l.workspace_bytes, w.bytes); return PHI_ERR_WORKSPACE; }
+    const bool mask = l.op.kind == CgOp::Masked;
     const bool adaptive = l.prm.method == PHI_SOLVER_CG_ADAPTIVE;
     if (l.prm.method != PHI_SOLVER_CG && !adaptive) { phi_set_error("cg: unknown solver method %d", l.prm.method); return PHI_ERR_INVALID; }
     if (adaptive && l.prm.matrix_offset != 0.f) { phi_set_error("cg: CG-adaptive does not take a matrix_offset"); return PHI_ERR_UNSUPPORTED; }
@@ -326,18 +333,14 @@ int phi_launch_cg(const CgLaunch& l, cudaStream_t s)
     int per_sm = 0;
     int grid = cg_grid_size(g.dim, g.batch, mask, &per_sm);
     if (grid <= 0) { phi_set_error("cg: kernel does not fit on the device (occupancy 0)"); return PHI_ERR_INVALID; }
-    const size_t pf_sb = (size_t)g.cext[0] * g.cext[1] * g.cext[2];
     CgArgs a;
     a.g = g; a.pf = l.pf;
     a.um = phi_make_unit_map(g, grid * 8);
     if (grid > a.um.total_units) grid = a.um.total_units;
     if (grid > CG_MAX_GRID) grid = CG_MAX_GRID;
-    const size_t arr = align_up((size_t)pf_sb * g.batch * sizeof(float), 256);
-    unsigned char* ws = (unsigned char*)l.workspace;
-    a.rhs = l.rhs; a.x = l.x; a.acc = l.acc;
+    a.rhs = l.rhs; a.x = l.x; a.acc = l.op.mask;
     if (g.halo != 0) { phi_set_error("cg: z-slab grids need the TMA ring kernel (grid lines too long)"); return PHI_ERR_UNSUPPORTED; }
-    a.r = (float*)ws; a.d0 = (float*)(ws + arr); a.d1 = (float*)(ws + 2 * arr);
-    a.partials = (double*)(ws + 3 * arr);
+    a.r = w.r; a.d0 = w.d0; a.d1 = w.d1; a.partials = w.partials;
     a.result = l.result; a.prm = l.prm;
     void* args[] = {&a};
     const size_t smem = cg_smem_bytes(g.batch);

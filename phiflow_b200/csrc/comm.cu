@@ -15,7 +15,7 @@ struct PhiComm {
     unsigned char* local;
     size_t bytes;
     unsigned char* peer[PHI_MAX_RANKS];
-    size_t off_flags, off_seq, off_mbox, off_ws, arr_bytes, ws_bytes;
+    size_t off_flags, off_seq, off_mbox, off_ws, ws_bytes;
     PhiGrid grid;
 };
 
@@ -37,8 +37,7 @@ int phicuda_comm_create(int rank, int nranks, const PhiGrid* g, PhiComm** comm, 
     c->off_seq = 256;
     c->off_mbox = 512;
     c->off_ws = align_up(c->off_mbox + (size_t)2 * PHI_MAX_RANKS * 2 * CG_MAX_BATCH * sizeof(double), 256);
-    c->ws_bytes = phi_cg_workspace_bytes(dg);
-    c->arr_bytes = align_up((size_t)dg.cext[0] * dg.cext[1] * dg.cext[2] * dg.batch * sizeof(float), 256);
+    c->ws_bytes = phi_cg_workspace(dg, nullptr).bytes;
     c->bytes = c->off_ws + c->ws_bytes;
     cudaError_t ce = cudaMalloc((void**)&c->local, c->bytes);
     if (ce != cudaSuccess) { phi_set_error("comm_create: cudaMalloc(%zu) failed: %s", c->bytes, cudaGetErrorString(ce)); delete c; return (int)ce; }
@@ -105,7 +104,8 @@ static int cg_dist(const PhiGrid* g, const PhiVBC* vbc, const float* rhs, float*
     int e = phi_make_dgrid(g, &l.g); if (e) return e;
     e = phi_pressure_bc(vbc, g->dim, &pbc); if (e) return e;
     e = phi_make_centered(g, &pbc, &l.pf); if (e) return e;
-    l.rhs = rhs; l.x = x; l.prm = *prm; l.result = result; l.acc = accessible;
+    l.rhs = rhs; l.x = x; l.prm = *prm; l.result = result;
+    if (accessible) { l.op.kind = CgOp::Masked; l.op.mask = accessible; }
     l.workspace = c->local + c->off_ws; l.workspace_bytes = c->ws_bytes;
     CommDev cm;
     memset(&cm, 0, sizeof(cm));
@@ -120,10 +120,8 @@ static int cg_dist(const PhiGrid* g, const PhiVBC* vbc, const float* rhs, float*
     cm.seq = (unsigned long long*)(c->local + c->off_seq);
     cm.arrive = (unsigned*)(c->local + c->off_seq + 64);
     { cudaError_t ce = cudaMemsetAsync(cm.arrive, 0, sizeof(unsigned), (cudaStream_t)stream); if (ce != cudaSuccess) { phi_set_error("cg_dist: memset failed: %s", cudaGetErrorString(ce)); return (int)ce; } }
-    const size_t hoff = (size_t)g->halo * g->cext[0] * g->cext[1];
-    auto vec = [&](int q, int k) -> float* { return (float*)(c->peer[q] + c->off_ws + (size_t)k * c->arr_bytes) + hoff; };
-    if (cm.lower >= 0) { cm.lo_r = vec(cm.lower, 0); cm.lo_d0 = vec(cm.lower, 1); cm.lo_d1 = vec(cm.lower, 2); }
-    if (cm.upper >= 0) { cm.hi_r = vec(cm.upper, 0); cm.hi_d0 = vec(cm.upper, 1); cm.hi_d1 = vec(cm.upper, 2); }
+    if (cm.lower >= 0) { const CgWorkspace w = phi_cg_workspace(l.g, c->peer[cm.lower] + c->off_ws); cm.lo_r = w.r; cm.lo_d0 = w.d0; cm.lo_d1 = w.d1; }
+    if (cm.upper >= 0) { const CgWorkspace w = phi_cg_workspace(l.g, c->peer[cm.upper] + c->off_ws); cm.hi_r = w.r; cm.hi_d0 = w.d0; cm.hi_d1 = w.d1; }
     if (c->n > 1 && (cm.lower < 0 && cm.upper < 0)) { phi_set_error("cg_dist: %d ranks but no PHI_BC_HALO side on the z axis", c->n); return PHI_ERR_INVALID; }
     e = phi_launch_cg_ring(l, &cm, (cudaStream_t)stream);
     if (e == -100) { phi_set_error("cg_dist: the grid does not fit the TMA ring kernel"); return PHI_ERR_UNSUPPORTED; }

@@ -35,22 +35,41 @@ int phi_wide_laplace(const DGrid& g, const DField vfields0[3], const DField& pf,
                      void* workspace, size_t ws_bytes, cudaStream_t s);
 bool phi_scalar_kernels();      // PHICUDA_SCALAR_KERNELS=1: diagnostics, forces the one-thread-per-sample kernels of round 1
 
+// The operator A of a CG solve A x = y.
+enum class CgOp {
+    Poisson,            // L (pf: the pressure boundary)
+    Masked,             // N4: L with static obstacles, face coefficients min(mask_c, mask_nb); obstacle cells keep their value
+    Helmholtz,          // N5 diffuse.implicit: I - amount * L0 (pf carries L0: constants zeroed)
+    HelmholtzVarying,   // N6 diffuse.implicit with a varying diffusivity k: I + D0, face coefficients min(fl(ndt k))
+};
+// the operator stages one more haloed array after the CG vectors: the obstacle mask, or the diffusivity
+__host__ __device__ constexpr bool cg_op_xslot(CgOp op) { return op == CgOp::Masked || op == CgOp::HelmholtzVarying; }
+
+// The operator and its data (host side: CgLaunch; device side: the ring CG's kernel parameters, where the mask travels in CgArgs.acc).
+struct CgOperator {
+    float amount = 0.f;                  // Helmholtz
+    CgOp kind = CgOp::Poisson;
+    const float* k = nullptr;            // HelmholtzVarying: k per batch entry, or (kbcast) entry 0 for every entry
+    int kbcast = 0;
+    float ndt = 0.f;                     // -dt
+    float kclo[3] = {0.f, 0.f, 0.f}, kchi[3] = {0.f, 0.f, 0.f};   // the real boundary constants of the constant sides: coefficient
+                                                                  // ghosts and bias (pf has them zeroed for the value ghosts)
+    const float* mask = nullptr;         // Masked: accessible mask (1 = fluid, 0 = obstacle)
+};
+
 struct CgLaunch {
     DGrid g; DField pf;
     const float* rhs; float* x;
     PhiCgParams prm; PhiCgResult* result;
     void* workspace; size_t workspace_bytes;
-    const float* acc = nullptr;    // N4: accessible mask
-    bool helm = false;             // N5 diffuse.implicit: operator I - helm_amount * L instead of L (pf carries L0: constants zeroed)
-    float helm_amount = 0.f;
-    // N6 (with helm): varying diffusivity k, operator I + D0 with face coefficients min(fl(helm_ndt k)); helm_kclo / helm_kchi are
-    // the real boundary constants (coefficient ghosts; pf has them zeroed for the value ghosts)
-    const float* helm_k = nullptr;
-    bool helm_k_bcast = false;     // one k (entry 0) for every batch entry
-    float helm_ndt = 0.f;          // -dt
-    float helm_kclo[3] = {0.f, 0.f, 0.f}, helm_kchi[3] = {0.f, 0.f, 0.f};
+    CgOperator op;
 };
-size_t phi_cg_workspace_bytes(const DGrid& g);
+
+// CG workspace: r | d0 | d1 | partials[4][2][batch][CG_MAX_GRID] | d2.  d2 and partial slots 4..7 belong to the one-sweep ring CG.
+// The Helmholtz solves never run the one-sweep CG, so implicit diffusion keeps its right-hand side y' = y - bias in d2.  The vectors
+// address the first owned plane (z-slabs: after the halo planes).  base == nullptr: only `bytes` is set.
+struct CgWorkspace { float *r, *d0, *d1, *d2; double* partials; size_t bytes; };
+CgWorkspace phi_cg_workspace(const DGrid& g, void* base);
 // TMA ring fast paths (ring_kernels.cu); return -100 when the shape does not fit and the caller must fall back
 int phi_launch_laplace_ring(const DGrid& g, const DField& f, const float* x, float* y, float coeff, bool axpy, cudaStream_t s);
 #define PHI_MAX_RANKS 8
@@ -67,10 +86,8 @@ struct CommDev {                      // device view of the multi-GPU communicat
 int phi_launch_cg_ring(const CgLaunch& a, const CommDev* cm, cudaStream_t s);
 bool phi_ring_enabled();
 int phi_launch_cg(const CgLaunch& a, cudaStream_t s);
-// N5 diffuse.implicit on the ring CG (ring_kernels.cu): host-only fit test, and the solve (bias pre-pass + k_cg_ring<..., HELM>);
-// cf[c] = boundary with constants of component c (batch entry b is component b % C).  -100: the grid does not fit the ring.
-// xslot: the launch stages one more haloed array (N6: the diffusivity).
-bool phi_cg_ring_fits(const DGrid& g, bool xslot = false);
-int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField cf[3], cudaStream_t s);
-// N6 diffuse.implicit with a varying diffusivity (ring_kernels.cu): bias pre-pass + k_cg_ring<..., HELM, VARK>.  -100: no fit.
-int phi_launch_diffuse_implicit_varying(const CgLaunch& l, cudaStream_t s);
+// diffuse.implicit on the ring CG (ring_kernels.cu): host-only fit test, and the solve (bias pre-pass + k_cg_ring with the
+// Helmholtz operator l.op); cf[0 .. C-1] = boundary with constants of component c (batch entry b is component b % C; C = 1 for a varying
+// diffusivity).  -100: the grid does not fit the ring.
+bool phi_cg_ring_fits(const DGrid& g, CgOp op);
+int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField* cf, cudaStream_t s);

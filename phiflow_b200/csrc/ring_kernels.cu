@@ -283,21 +283,22 @@ __device__ __forceinline__ void groups_tile(ThreadGroups& tg, const RingCfg& cfg
 
 // ---- consumer: one plane of one tile ---------------------------------------------------------------------------------
 // sm/sc/sp: stages holding planes z-1, z, z+1 (sm/sp unused in 2-D).  Values of the differenced array are h0 (+ beta*h1).
-// MASK (N4, static obstacles): the last haloed slot of a stage holds the accessible mask; the stencil becomes
-//   q_c = sum_faces min(acc_c, acc_nb) * (v_nb - v_c) / dx^2 for fluid cells, q_c = v_c inside obstacles
-// (fluid.masked_laplace, phi/physics/fluid.py:197-202); constant (Dirichlet) ghost cells count as accessible.
-// VARK (N6, varying diffusivity): the last haloed slot holds the diffusivity k; the same face-minimum stencil runs on the
-// coefficients w = fl(epi.ndt * k) (ndt = -dt), a constant side's ghost coefficient is its boundary constant epi.kclo / epi.kchi
-// itself, and there is no obstacle override: q_c = sum_faces min(w_c, w_nb) * (v_nb - v_c) / dx^2 (phi/physics/diffuse.py:129-141).
-template <int DIM, int NH, int NE, bool MASK = false, bool VARK = false, class Epi>
+// Operators with an extra haloed slot (cg_op_xslot) run the face-minimum stencil
+//   q_c = sum_faces min(w_c, w_nb) * (v_nb - v_c) / dx^2
+// on coefficients w of the last haloed slot of a stage, which travel like the values (same staged lines):
+//   Masked (N4, static obstacles): w = the accessible mask; a constant ghost counts as accessible (w = 1); obstacle cells take
+//     q_c = v_c (fluid.masked_laplace, phi/physics/fluid.py:197-202), and the mask goes to the epilogue (set_acc);
+//   HelmholtzVarying (N6): w = fl(od->ndt * k) (ndt = -dt), rounded as the reference rounds k * (-dt); a constant side's ghost
+//     coefficient is its boundary constant od->kclo / od->kchi itself (phi/physics/diffuse.py:129-141).
+template <int DIM, int NH, int NE, CgOp OP = CgOp::Poisson, class Epi>
 __device__ __forceinline__ void ring_compute(const RingCfg& cfg, const DGrid& g, const DField& pf, const ThreadGroups& tg,
                                              const float* sm, const float* sc, const float* sp, float beta,
-                                             long long plane_off, int z, Epi& epi)
+                                             long long plane_off, int z, Epi& epi, const CgOperator* od)
 {
     const int pitch = cfg.pitch;
     const int h1 = (cfg.TY + 2) * pitch;                 // offset of the second haloed array inside a stage
-    const int aoff = NH * (cfg.TY + 2) * pitch;          // MASK: offset of the accessible mask (VARK: of the diffusivity)
-    const int e0off = (NH + ((MASK || VARK) ? 1 : 0)) * (cfg.TY + 2) * pitch;
+    const int aoff = NH * (cfg.TY + 2) * pitch;          // offset of the operator's coefficients (cg_op_xslot)
+    const int e0off = (NH + (cg_op_xslot(OP) ? 1 : 0)) * (cfg.TY + 2) * pitch;
     const int e1off = e0off + cfg.TY * pitch;
     const float ix2 = g.inv_dx2[0], iy2 = g.inv_dx2[1], iz2 = g.inv_dx2[2];
     const bool zm_const = DIM == 3 && z == 0 && pf.klo[2] == PHI_BC_CONST;
@@ -352,20 +353,24 @@ __device__ __forceinline__ void ring_compute(const RingCfg& cfg, const DGrid& g,
         }
         float4 r4 = make_float4(c.y, c.z, c.w, xr);
         if (nvalid < 4) f4_set(r4, nvalid - 1, xr);
-        if (MASK) {
-            // the mask travels like the values: same staged lines, ghost cells 1 where the value ghost is a constant
+        if constexpr (cg_op_xslot(OP)) {
             const float* am = sm + aoff; const float* ac_ = sc + aoff; const float* ap = sp + aoff;
-            const float4 ac = *reinterpret_cast<const float4*>(ac_ + rc);
+            // coefficient of a staged value, ghost coefficients of the constant sides
+            auto cw = [od](float v) { return OP == CgOp::Masked ? v : __fmul_rn(od->ndt, v); };
+            auto cw4 = [&](const float* p) { const float4 v = *reinterpret_cast<const float4*>(p); return make_float4(cw(v.x), cw(v.y), cw(v.z), cw(v.w)); };
+            auto glo = [od](int ax) { return OP == CgOp::Masked ? 1.f : od->kclo[ax]; };
+            auto ghi = [od](int ax) { return OP == CgOp::Masked ? 1.f : od->kchi[ax]; };
+            const float4 ac = cw4(ac_ + rc);
             const int row = rc - (tg.eoff[k] - tg.j[k] * pitch);
             const int nx = g.n[0];
-            float axl = (f & GF_XLO) ? (pf.klo[0] == PHI_BC_PERIODIC ? ac_[row + nx - 1] : (pf.klo[0] == PHI_BC_ZERO_GRADIENT ? ac.x : 1.f)) : ac_[rc - 1];
-            float axr = (f & GF_XHI) ? (pf.khi[0] == PHI_BC_PERIODIC ? ac_[row] : (pf.khi[0] == PHI_BC_ZERO_GRADIENT ? f4_get(ac, nvalid - 1) : 1.f)) : ac_[rc + 4];
+            float axl = (f & GF_XLO) ? (pf.klo[0] == PHI_BC_PERIODIC ? cw(ac_[row + nx - 1]) : (pf.klo[0] == PHI_BC_ZERO_GRADIENT ? ac.x : glo(0))) : cw(ac_[rc - 1]);
+            float axr = (f & GF_XHI) ? (pf.khi[0] == PHI_BC_PERIODIC ? cw(ac_[row]) : (pf.khi[0] == PHI_BC_ZERO_GRADIENT ? f4_get(ac, nvalid - 1) : ghi(0))) : cw(ac_[rc + 4]);
             const float4 al4 = make_float4(axl, ac.x, ac.y, ac.z);
             float4 ar4 = make_float4(ac.y, ac.z, ac.w, axr);
             if (nvalid < 4) f4_set(ar4, nvalid - 1, axr);
             const float4 l4 = make_float4(xl, c.x, c.y, c.z);
-            const float4 aym = (f & GF_YLOC) ? f4_splat(1.f) : *reinterpret_cast<const float4*>(ac_ + rc - pitch);
-            const float4 ayp = (f & GF_YHIC) ? f4_splat(1.f) : *reinterpret_cast<const float4*>(ac_ + rc + pitch);
+            const float4 aym = (f & GF_YLOC) ? f4_splat(glo(1)) : cw4(ac_ + rc - pitch);
+            const float4 ayp = (f & GF_YHIC) ? f4_splat(ghi(1)) : cw4(ac_ + rc + pitch);
             auto term = [](float vn, float vc, float an, float a0) { return fminf(an, a0) * (vn - vc); };
             q.x = (term(l4.x, c.x, al4.x, ac.x) + term(r4.x, c.x, ar4.x, ac.x)) * ix2 + (term(ym.x, c.x, aym.x, ac.x) + term(yp.x, c.x, ayp.x, ac.x)) * iy2;
             q.y = (term(l4.y, c.y, al4.y, ac.y) + term(r4.y, c.y, ar4.y, ac.y)) * ix2 + (term(ym.y, c.y, aym.y, ac.y) + term(yp.y, c.y, ayp.y, ac.y)) * iy2;
@@ -374,50 +379,19 @@ __device__ __forceinline__ void ring_compute(const RingCfg& cfg, const DGrid& g,
             if (DIM == 3) {
                 const float4 zm = zm_const ? f4_splat(pf.clo[2]) : val4(sm, rc);
                 const float4 zp = zp_const ? f4_splat(pf.chi[2]) : val4(sp, rc);
-                const float4 azm = zm_const ? f4_splat(1.f) : *reinterpret_cast<const float4*>(am + rc);
-                const float4 azp = zp_const ? f4_splat(1.f) : *reinterpret_cast<const float4*>(ap + rc);
+                const float4 azm = zm_const ? f4_splat(glo(2)) : cw4(am + rc);
+                const float4 azp = zp_const ? f4_splat(ghi(2)) : cw4(ap + rc);
                 q.x += (term(zm.x, c.x, azm.x, ac.x) + term(zp.x, c.x, azp.x, ac.x)) * iz2;
                 q.y += (term(zm.y, c.y, azm.y, ac.y) + term(zp.y, c.y, azp.y, ac.y)) * iz2;
                 q.z += (term(zm.z, c.z, azm.z, ac.z) + term(zp.z, c.z, azp.z, ac.z)) * iz2;
                 q.w += (term(zm.w, c.w, azm.w, ac.w) + term(zp.w, c.w, azp.w, ac.w)) * iz2;
             }
-            if (ac.x == 0.f) q.x = c.x;
-            if (ac.y == 0.f) q.y = c.y;
-            if (ac.z == 0.f) q.z = c.z;
-            if (ac.w == 0.f) q.w = c.w;
-            epi.set_acc(ac);
-        } else if constexpr (VARK) {
-            // the diffusivity travels like the mask (same slot and staged lines); each staged k becomes w = fl(ndt k), rounded as the
-            // reference rounds k * (-dt); a constant side's ghost coefficient is its boundary constant itself
-            const float* am = sm + aoff; const float* ac_ = sc + aoff; const float* ap = sp + aoff;
-            const float ndt = epi.ndt;
-            auto cw = [ndt](float v) { return __fmul_rn(ndt, v); };
-            auto cw4 = [ndt](const float4& v) { return make_float4(__fmul_rn(ndt, v.x), __fmul_rn(ndt, v.y), __fmul_rn(ndt, v.z), __fmul_rn(ndt, v.w)); };
-            const float4 ac = cw4(*reinterpret_cast<const float4*>(ac_ + rc));
-            const int row = rc - (tg.eoff[k] - tg.j[k] * pitch);
-            const int nx = g.n[0];
-            float axl = (f & GF_XLO) ? (pf.klo[0] == PHI_BC_PERIODIC ? cw(ac_[row + nx - 1]) : (pf.klo[0] == PHI_BC_ZERO_GRADIENT ? ac.x : epi.kclo[0])) : cw(ac_[rc - 1]);
-            float axr = (f & GF_XHI) ? (pf.khi[0] == PHI_BC_PERIODIC ? cw(ac_[row]) : (pf.khi[0] == PHI_BC_ZERO_GRADIENT ? f4_get(ac, nvalid - 1) : epi.kchi[0])) : cw(ac_[rc + 4]);
-            const float4 al4 = make_float4(axl, ac.x, ac.y, ac.z);
-            float4 ar4 = make_float4(ac.y, ac.z, ac.w, axr);
-            if (nvalid < 4) f4_set(ar4, nvalid - 1, axr);
-            const float4 l4 = make_float4(xl, c.x, c.y, c.z);
-            const float4 aym = (f & GF_YLOC) ? f4_splat(epi.kclo[1]) : cw4(*reinterpret_cast<const float4*>(ac_ + rc - pitch));
-            const float4 ayp = (f & GF_YHIC) ? f4_splat(epi.kchi[1]) : cw4(*reinterpret_cast<const float4*>(ac_ + rc + pitch));
-            auto term = [](float vn, float vc, float an, float a0) { return fminf(an, a0) * (vn - vc); };
-            q.x = (term(l4.x, c.x, al4.x, ac.x) + term(r4.x, c.x, ar4.x, ac.x)) * ix2 + (term(ym.x, c.x, aym.x, ac.x) + term(yp.x, c.x, ayp.x, ac.x)) * iy2;
-            q.y = (term(l4.y, c.y, al4.y, ac.y) + term(r4.y, c.y, ar4.y, ac.y)) * ix2 + (term(ym.y, c.y, aym.y, ac.y) + term(yp.y, c.y, ayp.y, ac.y)) * iy2;
-            q.z = (term(l4.z, c.z, al4.z, ac.z) + term(r4.z, c.z, ar4.z, ac.z)) * ix2 + (term(ym.z, c.z, aym.z, ac.z) + term(yp.z, c.z, ayp.z, ac.z)) * iy2;
-            q.w = (term(l4.w, c.w, al4.w, ac.w) + term(r4.w, c.w, ar4.w, ac.w)) * ix2 + (term(ym.w, c.w, aym.w, ac.w) + term(yp.w, c.w, ayp.w, ac.w)) * iy2;
-            if (DIM == 3) {
-                const float4 zm = zm_const ? f4_splat(pf.clo[2]) : val4(sm, rc);
-                const float4 zp = zp_const ? f4_splat(pf.chi[2]) : val4(sp, rc);
-                const float4 azm = zm_const ? f4_splat(epi.kclo[2]) : cw4(*reinterpret_cast<const float4*>(am + rc));
-                const float4 azp = zp_const ? f4_splat(epi.kchi[2]) : cw4(*reinterpret_cast<const float4*>(ap + rc));
-                q.x += (term(zm.x, c.x, azm.x, ac.x) + term(zp.x, c.x, azp.x, ac.x)) * iz2;
-                q.y += (term(zm.y, c.y, azm.y, ac.y) + term(zp.y, c.y, azp.y, ac.y)) * iz2;
-                q.z += (term(zm.z, c.z, azm.z, ac.z) + term(zp.z, c.z, azp.z, ac.z)) * iz2;
-                q.w += (term(zm.w, c.w, azm.w, ac.w) + term(zp.w, c.w, azp.w, ac.w)) * iz2;
+            if constexpr (OP == CgOp::Masked) {
+                if (ac.x == 0.f) q.x = c.x;
+                if (ac.y == 0.f) q.y = c.y;
+                if (ac.z == 0.f) q.z = c.z;
+                if (ac.w == 0.f) q.w = c.w;
+                epi.set_acc(ac);
             }
         } else {
         q.x = (xl + r4.x - 2.f * c.x) * ix2 + (ym.x + yp.x - 2.f * c.x) * iy2;
@@ -506,20 +480,20 @@ __device__ __forceinline__ void ring_compute_fast(const RingCfg& cfg, const DGri
     zs.have = MARCH && DIM == 3 && G <= 2;
 }
 
-template <bool GENERIC, int DIM, int NH, int NE, bool MARCH, bool MASK = false, bool VARK = false, class Epi>
+template <bool GENERIC, int DIM, int NH, int NE, bool MARCH, CgOp OP, class Epi>
 __device__ __forceinline__ void ring_compute_any(const RingCfg& cfg, const DGrid& g, const DField& pf, const ThreadGroups& tg,
                                                  bool fast, const float* sm, const float* sc, const float* sp, float beta,
-                                                 long long plane_off, int z, Epi& epi, ZMarch& zs)
+                                                 long long plane_off, int z, Epi& epi, ZMarch& zs, const CgOperator* od)
 {
     if (cfg.dbg & 4) return;
-    if (MASK || VARK) { zs.have = false; ring_compute<DIM, NH, NE, MASK, VARK>(cfg, g, pf, tg, sm, sc, sp, beta, plane_off, z, epi); return; }
+    if (cg_op_xslot(OP)) { zs.have = false; ring_compute<DIM, NH, NE, OP>(cfg, g, pf, tg, sm, sc, sp, beta, plane_off, z, epi, od); return; }
     if (!GENERIC || fast) {
         if (cfg.groups == 4) { ring_compute_fast<DIM, NH, NE, 4, MARCH>(cfg, g, tg, sm, sc, sp, beta, plane_off, epi, zs); return; }
         if (cfg.groups == 2) { ring_compute_fast<DIM, NH, NE, 2, MARCH>(cfg, g, tg, sm, sc, sp, beta, plane_off, epi, zs); return; }
         if (cfg.groups == 1) { ring_compute_fast<DIM, NH, NE, 1, MARCH>(cfg, g, tg, sm, sc, sp, beta, plane_off, epi, zs); return; }
     }
     zs.have = false;
-    if (GENERIC) ring_compute<DIM, NH, NE, false>(cfg, g, pf, tg, sm, sc, sp, beta, plane_off, z, epi);
+    if (GENERIC) ring_compute<DIM, NH, NE>(cfg, g, pf, tg, sm, sc, sp, beta, plane_off, z, epi, od);
 }
 
 // ---- one unit: producer streams its planes, consumers march through them --------------------------------------------------
@@ -558,9 +532,10 @@ __device__ __forceinline__ bool ring_next_unit(const RingCfg& cfg, const DGrid& 
 }
 
 // consumers, 3-D: march through the planes of one unit.  G > 0: every plane takes the branch-free path with G groups.
-template <bool GENERIC, int NH, int NE, bool MARCH, int G, bool MASK = false, bool VARK = false, class Epi>
+template <bool GENERIC, int NH, int NE, bool MARCH, int G, CgOp OP, class Epi>
 __device__ __forceinline__ void ring_consume_planes(Ring& rg, const RingCfg& cfg, const DGrid& g, const DField& pf, const ThreadGroups& tg,
-                                                    bool tile_fast, float beta, long long plane_off, const RingUnit& u, Epi& epi)
+                                                    bool tile_fast, float beta, long long plane_off, const RingUnit& u, Epi& epi,
+                                                    const CgOperator* od)
 {
     const int nz = u.z1 - u.z0;
     SlotIt a = rg.pos, bq = a; bq.next(cfg.R);
@@ -577,8 +552,8 @@ __device__ __forceinline__ void ring_consume_planes(Ring& rg, const RingCfg& cfg
                                                                      beta, plane_off, epi, zs);
         } else {
             const bool fast = tile_fast && !(z == 0 && pf.klo[2] == PHI_BC_CONST) && !(z == g.n[2] - 1 && pf.khi[2] == PHI_BC_CONST);
-            ring_compute_any<GENERIC, 3, NH, NE, MARCH, MASK, VARK>(cfg, g, pf, tg, fast, ring_ptr(rg, cfg, a), ring_ptr(rg, cfg, bq), ring_ptr(rg, cfg, c2),
-                                                              beta, plane_off, z, epi, zs);
+            ring_compute_any<GENERIC, 3, NH, NE, MARCH, OP>(cfg, g, pf, tg, fast, ring_ptr(rg, cfg, a), ring_ptr(rg, cfg, bq), ring_ptr(rg, cfg, c2),
+                                                            beta, plane_off, z, epi, zs, od);
         }
         ring_release(rg, a);
         a = bq; bq = c2; c2.next(cfg.R);
@@ -588,20 +563,20 @@ __device__ __forceinline__ void ring_consume_planes(Ring& rg, const RingCfg& cfg
     rg.pos = c2;
 }
 
-// MASK: hsrc[NH] is the accessible mask; it occupies the haloed slot after the NH value arrays.
-// VARK: hsrc[NH] is the diffusivity, in the same slot; it is read from batch entry kb (0 when one k serves every entry).
-template <bool GENERIC, int DIM, int NH, int NE, bool MARCH = true, bool MASK = false, bool VARK = false, class Epi>
+// cg_op_xslot(OP): hsrc[NH] holds the operator's coefficients (the obstacle mask or the diffusivity) in the haloed slot after the
+// NH value arrays; the diffusivity is read from batch entry kb (0 when one k serves every entry).  od: the operator's data.
+template <bool GENERIC, int DIM, int NH, int NE, bool MARCH = true, CgOp OP = CgOp::Poisson, class Epi>
 __device__ __forceinline__ void ring_process_unit(Ring& rg, const RingCfg& cfg, const DGrid& g, const DField& pf,
                                                   ThreadGroups& tg,
                                                   const float* const* hsrc, const float* const* esrc, float beta,
-                                                  const RingUnit& u, Epi& epi, int kb = 0)
+                                                  const RingUnit& u, Epi& epi, int kb = 0, const CgOperator* od = nullptr)
 {
-    constexpr bool XSLOT = MASK || VARK;                            // one more haloed array after the NH value arrays
+    constexpr bool XSLOT = cg_op_xslot(OP);
     const bool producer = (int)threadIdx.x >= cfg.consumers;
     if (producer) {
         const int nh = (NH == 2 && beta == 0.f) ? 1 : NH;          // first CG iteration: d' = r, old direction not read
         ProdUnit pu;
-        prod_unit_setup<DIM, VARK>(pu, cfg, g, pf, ((1u << nh) - 1u) | (XSLOT ? (1u << NH) : 0u), NH + (XSLOT ? 1 : 0), NE, hsrc, esrc, u.b, u.y0, kb);
+        prod_unit_setup<DIM, OP == CgOp::HelmholtzVarying>(pu, cfg, g, pf, ((1u << nh) - 1u) | (XSLOT ? (1u << NH) : 0u), NH + (XSLOT ? 1 : 0), NE, hsrc, esrc, u.b, u.y0, kb);
         if (DIM == 3) {
             const int nz = u.z1 - u.z0;
             for (int p = 0; p < nz + 2; ++p)
@@ -618,17 +593,17 @@ __device__ __forceinline__ void ring_process_unit(Ring& rg, const RingCfg& cfg, 
     long long plane_off = (long long)u.b * pf.sb + (long long)u.y0 * pf.sy + (DIM == 3 ? (long long)u.z0 * pf.sz : 0);
     if (DIM == 3) {
         // kernels that contain only the branch-free path pick the group count once per unit, not once per plane
-        if (!GENERIC && cfg.groups == 2) ring_consume_planes<GENERIC, NH, NE, MARCH, 2>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi);
-        else if (!GENERIC && cfg.groups == 4) ring_consume_planes<GENERIC, NH, NE, MARCH, 4>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi);
-        else if (!GENERIC) ring_consume_planes<GENERIC, NH, NE, MARCH, 1>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi);
-        else ring_consume_planes<GENERIC, NH, NE, MARCH, 0, MASK, VARK>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi);
+        if (!GENERIC && cfg.groups == 2) ring_consume_planes<GENERIC, NH, NE, MARCH, 2, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
+        else if (!GENERIC && cfg.groups == 4) ring_consume_planes<GENERIC, NH, NE, MARCH, 4, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
+        else if (!GENERIC) ring_consume_planes<GENERIC, NH, NE, MARCH, 1, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
+        else ring_consume_planes<GENERIC, NH, NE, MARCH, 0, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
     } else {
         const SlotIt a = rg.pos;
         ring_wait_full(rg, a);
         const float* sc = ring_ptr(rg, cfg, a);
         epi.set_plane(-1, 0);
         ZMarch zs; zs.have = false;
-        ring_compute_any<GENERIC, DIM, NH, NE, MARCH, MASK, VARK>(cfg, g, pf, tg, tile_fast, sc, sc, sc, beta, plane_off, 0, epi, zs);
+        ring_compute_any<GENERIC, DIM, NH, NE, MARCH, OP>(cfg, g, pf, tg, tile_fast, sc, sc, sc, beta, plane_off, 0, epi, zs, od);
         ring_release(rg, a);
         rg.pos.next(cfg.R);
     }
@@ -782,12 +757,12 @@ struct REpiHelm {
     }
 };
 
-// diffuse.implicit with a varying diffusivity (N6): the VARK consumer delivers q = D0 c, the face-minimum stencil on the
-// coefficients w = fl(ndt k) (ndt = -dt, ghosts of constant sides: kclo / kchi, which the consumer reads from here), so that
-// M c = c + q (sharpen = explicit(x, k, -dt), phi/physics/diffuse.py:90-95).  No rhs balancing: set_acc is not forwarded.
+// diffuse.implicit with a varying diffusivity (N6): the HelmholtzVarying consumer delivers q = D0 c, the face-minimum stencil on
+// the coefficients w = fl(ndt k), so that M c = c + q (sharpen = explicit(x, k, -dt), phi/physics/diffuse.py:90-95).  No rhs
+// balancing: set_acc is not forwarded.
 template <class Epi>
 struct REpiVarHelm {
-    Epi& e; float ndt; float kclo[3], kchi[3];
+    Epi& e;
     __device__ __forceinline__ void set_plane(int z, int nz) { e.set_plane(z, nz); }
     __device__ __forceinline__ void set_acc(const float4&) {}
     __device__ __forceinline__ void operator()(long long off, const float4& c, const float4& q, int nvalid, const float4& e0, const float4& e1, const float4& e2)
@@ -824,16 +799,23 @@ struct CgRingArgs {
     int comm_merge;              // multi-GPU: 1 = merged barrier + all-reduce (comm_barrier_allreduce), 0 = grid.sync + comm_allreduce
     CommDev cm;
     float* d2;                   // one-sweep CG: third direction buffer
-    float helm_a;                // HELM (diffuse.implicit): operator I - helm_a * L0
-    const float* k; int kbcast;  // VARK (varying diffusivity): k per batch entry, or (kbcast) entry 0 for all
-    float ndt;                   // VARK: -dt
-    float kclo[3], kchi[3];      // VARK: boundary constants of the constant sides (ghost coefficients; pf has them zeroed)
+    CgOperator op;               // the mask travels in a.acc
 };
 
-template <class Epi>
-__device__ __forceinline__ REpiVarHelm<Epi> var_helm(Epi& e, const CgRingArgs& A)
+// The operator's one dispatch point in the CG: picks the batch entry of the diffusivity, turns the stencil result q into M c
+// through the operator's epilogue wrapper and runs the unit.  hsrc[NH]: the obstacle mask or the diffusivity.  The Poisson sweeps
+// call ring_process_unit directly: one more inlined call level changes nvcc's register allocation of those kernels.
+template <int DIM, bool GENERIC, CgOp OP, int NH, int NE, class Epi>
+__device__ __forceinline__ void cg_op_unit(Ring& rg, const CgRingArgs& A, ThreadGroups& tg, const float* const* hsrc,
+                                           const float* const* esrc, float beta, const RingUnit& u, Epi& epi)
 {
-    return REpiVarHelm<Epi>{e, A.ndt, {A.kclo[0], A.kclo[1], A.kclo[2]}, {A.kchi[0], A.kchi[1], A.kchi[2]}};
+    if constexpr (OP == CgOp::Helmholtz) {
+        REpiHelm<Epi> he{epi, A.op.amount};
+        ring_process_unit<GENERIC, DIM, NH, NE, true, OP>(rg, A.cfg, A.a.g, A.a.pf, tg, hsrc, esrc, beta, u, he);
+    } else if constexpr (OP == CgOp::HelmholtzVarying) {
+        REpiVarHelm<Epi> he{epi};
+        ring_process_unit<GENERIC, DIM, NH, NE, true, OP>(rg, A.cfg, A.a.g, A.a.pf, tg, hsrc, esrc, beta, u, he, A.op.kbcast ? 0 : u.b, &A.op);
+    } else ring_process_unit<GENERIC, DIM, NH, NE, true, OP>(rg, A.cfg, A.a.g, A.a.pf, tg, hsrc, esrc, beta, u, epi);
 }
 
 __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p)
@@ -1232,16 +1214,19 @@ struct REpiFusedStart {
     }
 };
 
-// MASK (N4): static obstacles - a.acc is the accessible mask, staged as an extra haloed array (always the GENERIC consumer).
+// OP (cg_op_unit): Masked (N4): static obstacles - a.acc is the accessible mask, staged as an extra haloed array (always the
+// GENERIC consumer).  Helmholtz (N5, diffuse.implicit): two-sweep CG on M = I - A.op.amount * L0 (REpiHelm); every batch entry is
+// its own system.  HelmholtzVarying (N6): M = I + D0 of a varying diffusivity A.op.k (REpiVarHelm, the face-minimum consumer).
 // FUSED: the one-sweep iteration (pass F above) replaces passes A and B.
-// HELM (N5, diffuse.implicit): two-sweep CG on M = I - A.helm_a * L0 (REpiHelm); every batch entry is its own system.
-// VARK (N6, with HELM): the operator is M = I + D0 of a varying diffusivity A.k (REpiVarHelm, the VARK consumer) instead.
-template <int DIM, bool GENERIC, bool DIST, bool ADAPT, bool MASK = false, bool FUSED = false, bool HELM = false, bool VARK = false>
+template <int DIM, bool GENERIC, bool DIST, bool ADAPT, CgOp OP = CgOp::Poisson, bool FUSED = false>
 __global__ void __launch_bounds__(RING_THREADS, 1)
 k_cg_ring(CgRingArgs A)
 {
-    static_assert(!HELM || (!DIST && !ADAPT && !MASK && !FUSED), "the Helmholtz operator runs on the single-GPU two-sweep CG only");
-    static_assert(!VARK || (HELM && GENERIC), "the varying-diffusivity operator is a Helmholtz operator on the generic consumer");
+    constexpr bool MASK = OP == CgOp::Masked;
+    static_assert((OP != CgOp::Helmholtz && OP != CgOp::HelmholtzVarying) || (!DIST && !ADAPT && !FUSED),
+                  "the Helmholtz operators run on the single-GPU two-sweep CG only");
+    static_assert(!MASK || !ADAPT, "CG-adaptive has no obstacle mask");
+    static_assert(!cg_op_xslot(OP) || GENERIC, "the face-minimum stencil runs on the generic consumer");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const CgArgs& a = A.a;
     const RingCfg& cfg = A.cfg;
@@ -1322,17 +1307,12 @@ k_cg_ring(CgRingArgs A)
     }
 
     {   // r0 = y - (A + c 11^T) x0
-        const float* hsrc[2] = {a.x, MASK ? a.acc : (VARK ? A.k : nullptr)};
+        const float* hsrc[2] = {a.x, (OP == CgOp::Masked ? a.acc : (OP == CgOp::HelmholtzVarying ? A.op.k : nullptr))};
         const float* esrc[2] = {a.rhs, nullptr};
         sweep(nullptr, [&](const RingUnit& u, float& acc0, float& acc1) {
             REpiResidual0<PH> epi{a.r, sh.mean[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r), adaptive};
-            if constexpr (VARK) {
-                auto he = var_helm(epi, A);
-                ring_process_unit<GENERIC, DIM, 1, 1, true, false, true>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he, A.kbcast ? 0 : u.b);
-            } else if constexpr (HELM) {
-                REpiHelm<REpiResidual0<PH>> he{epi, A.helm_a};
-                ring_process_unit<GENERIC, DIM, 1, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he);
-            } else ring_process_unit<GENERIC, DIM, 1, 1, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
+            if constexpr (OP == CgOp::Poisson) ring_process_unit<GENERIC, DIM, 1, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
+            else cg_op_unit<DIM, GENERIC, OP, 1, 1>(rg, A, tg, hsrc, esrc, 0.f, u, epi);
             acc0 += epi.acc0; acc1 += epi.acc1;
         });
     }
@@ -1353,7 +1333,7 @@ k_cg_ring(CgRingArgs A)
     __syncthreads();
 
     if constexpr (FUSED) {
-        static_assert(DIM == 3 && !GENERIC && !DIST && !ADAPT && !MASK, "the one-sweep CG is 3-D, branch-free, single-GPU CG only");
+        static_assert(DIM == 3 && !GENERIC && !DIST && !ADAPT && OP == CgOp::Poisson, "the one-sweep CG is 3-D, branch-free, single-GPU CG only");
         // d_k lives in D[k % 3]: pass k reads d_k and d_{k-1} with halos while other CTAs write d_{k+1}.  a.r holds r_0 only.
         float* const D[3] = {a.d0, a.d1, A.d2};
         float* const tile = rg.stage0 + (size_t)cfg.R * cfg.stage_floats;
@@ -1457,17 +1437,12 @@ k_cg_ring(CgRingArgs A)
     bool x_pending = false;      // all running entries are at the same iteration, so one flag describes them all
     while (!FUSED && *sh.any_cont && comm_ok) {
         if (cfg.dbg & 1) {} else if constexpr (!ADAPT) {   // pass A
-            const float* hsrc[3] = {a.r, dold, MASK ? a.acc : (VARK ? A.k : nullptr)};
+            const float* hsrc[3] = {a.r, dold, (OP == CgOp::Masked ? a.acc : (OP == CgOp::HelmholtzVarying ? A.op.k : nullptr))};
             const float* esrc[2] = {nullptr, nullptr};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
                 REpiPassA<PH> epi{dnew, 0.f, 0.f, peer_halo(lo_dnew, hi_dnew)};
-                if constexpr (VARK) {
-                    auto he = var_helm(epi, A);
-                    ring_process_unit<GENERIC, DIM, 2, 0, true, false, true>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, he, A.kbcast ? 0 : u.b);
-                } else if constexpr (HELM) {
-                    REpiHelm<REpiPassA<PH>> he{epi, A.helm_a};
-                    ring_process_unit<GENERIC, DIM, 2, 0>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, he);
-                } else ring_process_unit<GENERIC, DIM, 2, 0, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, epi);
+                if constexpr (OP == CgOp::Poisson) ring_process_unit<GENERIC, DIM, 2, 0>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, epi);
+                else cg_op_unit<DIM, GENERIC, OP, 2, 0>(rg, A, tg, hsrc, esrc, sh.beta[u.b], u, epi);
                 acc0 += epi.acc0; acc1 += epi.acc1;
             });
         } else {                                    // pass A of CG-adaptive: additionally d'.r (r once more, element-wise)
@@ -1497,44 +1472,22 @@ k_cg_ring(CgRingArgs A)
         }
         __syncthreads();
         if (cfg.dbg & 2) {} else if (!x_pending) {   // pass B, odd iteration: r only, the x update is deferred
-            const float* hsrc[2] = {dnew, MASK ? a.acc : (VARK ? A.k : nullptr)};
+            const float* hsrc[2] = {dnew, (OP == CgOp::Masked ? a.acc : (OP == CgOp::HelmholtzVarying ? A.op.k : nullptr))};
             const float* esrc[3] = {a.r, nullptr, nullptr};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
-                if constexpr (ADAPT) {
-                    REpiPassBr<PH, true> epi{a.r, sh.alpha[u.b], 0.f, 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
-                    ring_process_unit<GENERIC, DIM, 1, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
-                    acc0 += epi.acc0; acc1 += epi.acc1;
-                } else {
-                    REpiPassBr<PH> epi{a.r, sh.alpha[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
-                    if constexpr (VARK) {
-                        auto he = var_helm(epi, A);
-                        ring_process_unit<GENERIC, DIM, 1, 1, true, false, true>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he, A.kbcast ? 0 : u.b);
-                    } else if constexpr (HELM) {
-                        REpiHelm<REpiPassBr<PH>> he{epi, A.helm_a};
-                        ring_process_unit<GENERIC, DIM, 1, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he);
-                    } else ring_process_unit<GENERIC, DIM, 1, 1, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
-                    acc0 += epi.acc0;
-                }
+                REpiPassBr<PH, ADAPT> epi{a.r, sh.alpha[u.b], ADAPT ? 0.f : sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
+                if constexpr (OP == CgOp::Poisson) ring_process_unit<GENERIC, DIM, 1, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
+                else cg_op_unit<DIM, GENERIC, OP, 1, 1>(rg, A, tg, hsrc, esrc, 0.f, u, epi);
+                acc0 += epi.acc0; if (ADAPT) acc1 += epi.acc1;
             });
         } else {            // pass B, even iteration: x += alpha_prev d_prev + alpha d
-            const float* hsrc[2] = {dnew, MASK ? a.acc : (VARK ? A.k : nullptr)};
+            const float* hsrc[2] = {dnew, (OP == CgOp::Masked ? a.acc : (OP == CgOp::HelmholtzVarying ? A.op.k : nullptr))};
             const float* esrc[3] = {a.x, a.r, dold};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
-                if constexpr (ADAPT) {
-                    REpiPassB<PH, true> epi{a.x, a.r, sh.alpha[u.b], sh.aprev[u.b], 0.f, 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
-                    ring_process_unit<GENERIC, DIM, 1, 3>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
-                    acc0 += epi.acc0; acc1 += epi.acc1;
-                } else {
-                    REpiPassB<PH> epi{a.x, a.r, sh.alpha[u.b], sh.aprev[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
-                    if constexpr (VARK) {
-                        auto he = var_helm(epi, A);
-                        ring_process_unit<GENERIC, DIM, 1, 3, true, false, true>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he, A.kbcast ? 0 : u.b);
-                    } else if constexpr (HELM) {
-                        REpiHelm<REpiPassB<PH>> he{epi, A.helm_a};
-                        ring_process_unit<GENERIC, DIM, 1, 3>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, he);
-                    } else ring_process_unit<GENERIC, DIM, 1, 3, true, MASK>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
-                    acc0 += epi.acc0;
-                }
+                REpiPassB<PH, ADAPT> epi{a.x, a.r, sh.alpha[u.b], sh.aprev[u.b], ADAPT ? 0.f : sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
+                if constexpr (OP == CgOp::Poisson) ring_process_unit<GENERIC, DIM, 1, 3>(rg, cfg, g, a.pf, tg, hsrc, esrc, 0.f, u, epi);
+                else cg_op_unit<DIM, GENERIC, OP, 1, 3>(rg, A, tg, hsrc, esrc, 0.f, u, epi);
+                acc0 += epi.acc0; if (ADAPT) acc1 += epi.acc1;
             });
         }
         x_pending = !x_pending;
@@ -1717,20 +1670,58 @@ int phi_launch_laplace_ring(const DGrid& g, const DField& f, const float* x, flo
     return (int)cudaGetLastError();
 }
 
+// ring of the two-sweep CG; lines staged per stage: pass B (even) = 1 haloed + 3 element-wise arrays = 4 TY + 2; with the
+// operator's coefficients (cg_op_xslot: the obstacle mask or the diffusivity) as an extra haloed array 5 TY + 4 (pass A: 3 haloed = 3 TY + 6)
+static bool cg_ring_config(const DGrid& g, CgOp op, int cgs, int target_units, RingCfg* c)
+{
+    const bool xslot = cg_op_xslot(op);
+    return ring_config(g, xslot ? 5 : 4, xslot ? 6 : 2, cgs, g.dim == 3 ? (xslot ? 3 : 4) : 2, RING_MAX_STAGES, target_units, c);
+}
+
+// The k_cg_ring instantiation of an operator and solver variant; nullptr: the combination has none.
+using CgRingKernel = void (*)(CgRingArgs);
+static CgRingKernel cg_ring_kernel(CgOp op, int dim, bool generic, bool dist, bool adapt, bool fused)
+{
+    constexpr CgOp P = CgOp::Poisson, M = CgOp::Masked, H = CgOp::Helmholtz, V = CgOp::HelmholtzVarying;
+    const bool d3 = dim == 3;
+    switch (op) {
+    case P:
+        if (fused)              // the one-sweep CG: 3-D, branch-free, single-GPU CG
+            return d3 && !generic && !dist && !adapt ? k_cg_ring<3, false, false, false, P, true> : nullptr;
+        if (d3) return generic ? (dist ? (adapt ? k_cg_ring<3, true, true, true> : k_cg_ring<3, true, true, false>)
+                                       : (adapt ? k_cg_ring<3, true, false, true> : k_cg_ring<3, true, false, false>))
+                               : (dist ? (adapt ? k_cg_ring<3, false, true, true> : k_cg_ring<3, false, true, false>)
+                                       : (adapt ? k_cg_ring<3, false, false, true> : k_cg_ring<3, false, false, false>));
+        return generic ? (dist ? (adapt ? k_cg_ring<2, true, true, true> : k_cg_ring<2, true, true, false>)
+                               : (adapt ? k_cg_ring<2, true, false, true> : k_cg_ring<2, true, false, false>))
+                       : (dist ? (adapt ? k_cg_ring<2, false, true, true> : k_cg_ring<2, false, true, false>)
+                               : (adapt ? k_cg_ring<2, false, false, true> : k_cg_ring<2, false, false, false>));
+    case M:                     // the generic consumer, no CG-adaptive
+        if (!generic || adapt || fused) return nullptr;
+        return d3 ? (dist ? k_cg_ring<3, true, true, false, M> : k_cg_ring<3, true, false, false, M>)
+                  : (dist ? k_cg_ring<2, true, true, false, M> : k_cg_ring<2, true, false, false, M>);
+    case H:                     // the Helmholtz operators: single-GPU two-sweep CG
+        if (dist || adapt || fused) return nullptr;
+        return d3 ? (generic ? k_cg_ring<3, true, false, false, H> : k_cg_ring<3, false, false, false, H>)
+                  : (generic ? k_cg_ring<2, true, false, false, H> : k_cg_ring<2, false, false, false, H>);
+    case V:
+        if (dist || adapt || fused || !generic) return nullptr;
+        return d3 ? k_cg_ring<3, true, false, false, V> : k_cg_ring<2, true, false, false, V>;
+    }
+    return nullptr;
+}
+
 int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
 {
     const DGrid& g = l.g;
+    const CgOp op = l.op.kind;
     if (g.batch > CG_MAX_BATCH) return -100;
-    const bool mask = l.acc != nullptr;
-    if (mask && (l.prm.method == PHI_SOLVER_CG_ADAPTIVE || l.prm.matrix_offset != 0.f)) return -100;
-    const bool vark = l.helm_k != nullptr;            // varying diffusivity: k is staged like the obstacle mask
-    const bool xslot = mask || vark;
+    if (op == CgOp::Masked && l.prm.matrix_offset != 0.f) return -100;
+    const bool xslot = cg_op_xslot(op);
     CgRingArgs A;
     const int cgs = (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128);
     const int sms = phi_sm_count();
-    // lines staged per stage: pass B (even) = 1 haloed + 3 element-wise arrays = 4 TY + 2; with the obstacle mask (or the
-    // diffusivity) as an extra haloed array 5 TY + 4 (pass A: 3 haloed = 3 TY + 6)
-    if (!ring_config(g, xslot ? 5 : 4, xslot ? 6 : 2, cgs, g.dim == 3 ? (xslot ? 3 : 4) : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
+    if (!cg_ring_config(g, op, cgs, sms, &A.cfg)) return -100;
     // pass A of CG-adaptive stages 2 haloed + 1 element-wise array = 3 TY + 4 lines: one line more than 4 TY + 2 at TY = 1
     if (l.prm.method == PHI_SOLVER_CG_ADAPTIVE && !xslot && A.cfg.TY == 1
         && !ring_config(g, 4, 3, cgs, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
@@ -1741,9 +1732,6 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     const bool generic = xslot || !ring_all_fast(g, l.pf, A.cfg);
     const bool dist = cm && cm->n > 1;
     const bool adapt = l.prm.method == PHI_SOLVER_CG_ADAPTIVE;
-    const bool helm = l.helm;                         // diffuse.implicit: single-GPU two-sweep CG on I - a L0, no obstacles
-    if (helm && (dist || adapt || mask)) return -100;
-    if (vark && !helm) return -100;
     // one-sweep CG (pass F): 3-D, branch-free tiling, periodic y and z, one GPU, plain CG without matrix offset or obstacles.
     // PHICUDA_CG_PASSES=2 forces the two-sweep kernel (A/B timing, tools/cg_passes_bench.py).
     bool fused = false;
@@ -1751,7 +1739,7 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     {
         const char* e = getenv("PHICUDA_CG_PASSES");
         const DField& pf = l.pf;
-        if (!(e && atoi(e) == 2) && g.dim == 3 && !generic && !dist && !adapt && !mask && !helm && l.prm.matrix_offset == 0.f
+        if (!(e && atoi(e) == 2) && g.dim == 3 && !generic && !dist && !adapt && op == CgOp::Poisson && l.prm.matrix_offset == 0.f
             && pf.klo[1] == PHI_BC_PERIODIC && pf.khi[1] == PHI_BC_PERIODIC && pf.klo[2] == PHI_BC_PERIODIC && pf.khi[2] == PHI_BC_PERIODIC) {
             // stage = d_k (TY+4) + d_{k-1} (TY+2) + x (TY) lines; the d_{k+1} tile is reserved at the largest TY ring_config may pick
             RingCfg fc;
@@ -1765,18 +1753,8 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
         }
     }
     const size_t smem = (size_t)cgs + 128 + (size_t)A.cfg.R * A.cfg.stage_floats * 4 + tile_bytes;
-#define CG_RING_FN2(D, GEN, DI) (adapt ? (const void*)k_cg_ring<D, GEN, DI, true> : (const void*)k_cg_ring<D, GEN, DI, false>)
-#define CG_RING_FN(D, GEN) (dist ? CG_RING_FN2(D, GEN, true) : CG_RING_FN2(D, GEN, false))
-    const void* fn = g.dim == 3 ? (generic ? CG_RING_FN(3, true) : CG_RING_FN(3, false))
-                                : (generic ? CG_RING_FN(2, true) : CG_RING_FN(2, false));
-    if (mask) fn = g.dim == 3 ? (dist ? (const void*)k_cg_ring<3, true, true, false, true> : (const void*)k_cg_ring<3, true, false, false, true>)
-                              : (dist ? (const void*)k_cg_ring<2, true, true, false, true> : (const void*)k_cg_ring<2, true, false, false, true>);
-    if (fused) fn = (const void*)k_cg_ring<3, false, false, false, false, true>;
-    if (helm) fn = g.dim == 3 ? (generic ? (const void*)k_cg_ring<3, true, false, false, false, false, true> : (const void*)k_cg_ring<3, false, false, false, false, false, true>)
-                              : (generic ? (const void*)k_cg_ring<2, true, false, false, false, false, true> : (const void*)k_cg_ring<2, false, false, false, false, false, true>);
-    if (vark) fn = g.dim == 3 ? (const void*)k_cg_ring<3, true, false, false, false, false, true, true> : (const void*)k_cg_ring<2, true, false, false, false, false, true, true>;
-#undef CG_RING_FN
-#undef CG_RING_FN2
+    const void* fn = (const void*)cg_ring_kernel(op, g.dim, generic, dist, adapt, fused);
+    if (!fn) return -100;
     e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem);
     if (e != cudaSuccess || per_sm < 1) return -100;
@@ -1806,20 +1784,13 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     }
     if (!A.cfg.split && grid > A.cfg.total_units) grid = A.cfg.total_units;
     if (grid > CG_MAX_GRID) grid = CG_MAX_GRID;
-    const size_t pf_sb = (size_t)g.cext[0] * g.cext[1] * g.cext[2];
-    const size_t arr = ((size_t)pf_sb * g.batch * sizeof(float) + 255) / 256 * 256;
-    unsigned char* ws = (unsigned char*)l.workspace;
+    const CgWorkspace w = phi_cg_workspace(g, l.workspace);
     CgArgs& a = A.a;
     a.g = g; a.pf = l.pf; a.um = UnitMap();
-    a.rhs = l.rhs; a.x = l.x; a.acc = l.acc;
-    const size_t hoff = (size_t)g.halo * g.cext[0] * g.cext[1];       // pointers address the first owned plane
-    a.r = (float*)ws + hoff; a.d0 = (float*)(ws + arr) + hoff; a.d1 = (float*)(ws + 2 * arr) + hoff;
-    a.partials = (double*)(ws + 3 * arr);
-    const size_t pbytes = ((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double) + 255) / 256 * 256;
-    A.d2 = (float*)(ws + 3 * arr + pbytes) + hoff;
-    A.helm_a = l.helm_amount;
-    A.k = l.helm_k; A.kbcast = l.helm_k_bcast ? 1 : 0; A.ndt = l.helm_ndt;
-    for (int d = 0; d < 3; ++d) { A.kclo[d] = l.helm_kclo[d]; A.kchi[d] = l.helm_kchi[d]; }
+    a.rhs = l.rhs; a.x = l.x; a.acc = l.op.mask;
+    a.r = w.r; a.d0 = w.d0; a.d1 = w.d1; a.partials = w.partials;
+    A.d2 = w.d2;
+    A.op = l.op;
     a.result = l.result; a.prm = l.prm;
     if (cm) A.cm = *cm; else { memset(&A.cm, 0, sizeof(A.cm)); A.cm.n = 1; A.cm.lower = A.cm.upper = -1; }
     // grid.sync + block-0 send is the default multi-GPU barrier; PHICUDA_COMM_MERGE=1 selects the merged barrier
@@ -1827,9 +1798,9 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     void* args[] = {&A};
     e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(threads), args, smem, s);
     if (e != cudaSuccess) { phi_set_error("cg ring: cooperative launch failed: %s", cudaGetErrorString(e)); return (int)e; }
-    note_ring_launch(PHI_KERNEL_CG_RING, A.cfg, generic, dist, adapt, grid, mask);
+    note_ring_launch(PHI_KERNEL_CG_RING, A.cfg, generic, dist, adapt, grid, op == CgOp::Masked);
     phi_note_cg_passes(fused ? 1 : 2);
-    phi_note_cg_operator(vark ? PHI_CG_OP_HELMHOLTZ_VARYING : (helm ? PHI_CG_OP_HELMHOLTZ : PHI_CG_OP_POISSON));
+    phi_note_cg_operator(op == CgOp::HelmholtzVarying ? PHI_CG_OP_HELMHOLTZ_VARYING : (op == CgOp::Helmholtz ? PHI_CG_OP_HELMHOLTZ : PHI_CG_OP_POISSON));
     return 0;
 }
 
@@ -1886,21 +1857,22 @@ __global__ void k_helm_bias_var(DGrid g, DField f, float ndt, HelmConsts hc, con
     }
 }
 
-// the grid fits the persistent ring CG (host-only test, no CUDA call); xslot: with one more haloed array (the diffusivity)
-bool phi_cg_ring_fits(const DGrid& g, bool xslot)
+// the grid fits the persistent ring CG with operator op (host-only test, no CUDA call)
+bool phi_cg_ring_fits(const DGrid& g, CgOp op)
 {
     if (g.batch > CG_MAX_BATCH || g.halo != 0) return false;
     RingCfg c;
-    const int cgs = (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128);
-    return ring_config(g, xslot ? 5 : 4, xslot ? 6 : 2, cgs, g.dim == 3 ? (xslot ? 3 : 4) : 2, RING_MAX_STAGES, 1, &c);
+    return cg_ring_config(g, op, (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128), 1, &c);
 }
 
-// l.pf: boundary kinds with zeroed constants (L0); cf[c]: the boundary with its constants of component c = entry % C (bias).  y'
-// lives in the workspace buffer of the one-sweep CG's third direction, which the two-sweep solve does not touch.  -100: the grid
-// does not fit.
-int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField cf[3], cudaStream_t s)
+// l.pf: boundary kinds with zeroed constants (the value ghosts of L0 / D0); cf[0 .. C-1]: the boundary with its constants of component
+// c = entry % C (bias; with a varying diffusivity also the coefficient ghosts l.op.kclo / kchi).  y' = y - bias goes to the
+// workspace's d2 (phi_cg_workspace).  The varying pre-pass runs whenever a constant is non-zero - also for dt = 0, where
+// f_b = min(-0, c) = c for c < 0.  -100: the grid does not fit.
+int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField* cf, cudaStream_t s)
 {
     const DGrid& g = l.g;
+    const bool varying = l.op.kind == CgOp::HelmholtzVarying;
     HelmConsts hc;
     bool bias = false;
     for (int c = 0; c < 3; ++c)
@@ -1911,44 +1883,13 @@ int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField cf[3], cu
             bias = bias || hc.clo[c][ax] != 0.f || hc.chi[c][ax] != 0.f;
         }
     CgLaunch m = l;
-    if (bias && l.helm_amount != 0.f) {
-        const size_t arr = ((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float) + 255) / 256 * 256;
-        const size_t pbytes = ((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double) + 255) / 256 * 256;
-        float* yb = (float*)((unsigned char*)l.workspace + 3 * arr + pbytes);
+    if (bias && (varying || l.op.amount != 0.f)) {
+        float* yb = phi_cg_workspace(g, l.workspace).d2;
         const long long total = (long long)g.n[0] * g.n[1] * g.n[2] * g.batch;
         const long long want = (total + 255) / 256, cap = (long long)phi_sm_count() * 8;
         const int blocks = (int)(want < cap ? want : cap);
-        k_helm_bias<<<blocks, 256, 0, s>>>(g, l.pf, C, l.helm_amount, hc, l.rhs, yb);
-        const cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return (int)e;
-        m.rhs = yb;
-    }
-    return phi_launch_cg_ring(m, nullptr, s);
-}
-
-// N6: l.pf: boundary kinds with zeroed constants (value ghosts of D0); l.helm_kclo / helm_kchi: the real constants (coefficient
-// ghosts and bias).  y' goes to the same workspace buffer as for N5.  The bias pre-pass runs whenever a constant is non-zero - also
-// for dt = 0, where f_b = min(-0, c) = c for c < 0.  -100: the grid does not fit.
-int phi_launch_diffuse_implicit_varying(const CgLaunch& l, cudaStream_t s)
-{
-    const DGrid& g = l.g;
-    HelmConsts hc;
-    memset(&hc, 0, sizeof(hc));
-    bool bias = false;
-    for (int ax = 0; ax < g.dim; ++ax) {
-        hc.clo[0][ax] = l.pf.klo[ax] == PHI_BC_CONST ? l.helm_kclo[ax] : 0.f;
-        hc.chi[0][ax] = l.pf.khi[ax] == PHI_BC_CONST ? l.helm_kchi[ax] : 0.f;
-        bias = bias || hc.clo[0][ax] != 0.f || hc.chi[0][ax] != 0.f;
-    }
-    CgLaunch m = l;
-    if (bias) {
-        const size_t arr = ((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float) + 255) / 256 * 256;
-        const size_t pbytes = ((size_t)8 * g.batch * CG_MAX_GRID * sizeof(double) + 255) / 256 * 256;
-        float* yb = (float*)((unsigned char*)l.workspace + 3 * arr + pbytes);
-        const long long total = (long long)g.n[0] * g.n[1] * g.n[2] * g.batch;
-        const long long want = (total + 255) / 256, cap = (long long)phi_sm_count() * 8;
-        const int blocks = (int)(want < cap ? want : cap);
-        k_helm_bias_var<<<blocks, 256, 0, s>>>(g, l.pf, l.helm_ndt, hc, l.helm_k, l.helm_k_bcast ? 1 : 0, l.rhs, yb);
+        if (varying) k_helm_bias_var<<<blocks, 256, 0, s>>>(g, l.pf, l.op.ndt, hc, l.op.k, l.op.kbcast, l.rhs, yb);
+        else k_helm_bias<<<blocks, 256, 0, s>>>(g, l.pf, C, l.op.amount, hc, l.rhs, yb);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return (int)e;
         m.rhs = yb;
