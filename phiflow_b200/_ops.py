@@ -309,7 +309,8 @@ def axpy_centered(dom: Domain, a: float, x, y):
 
 
 def add_buoyancy(dom: Domain, vbc, sbc, s, factor: Sequence[float], dt: float, v):
-    """v += dt * resample(s * factor, to=v) in place (phi/field/_resample.py:272-276)."""
+    """v += dt * resample(s * factor, to=v) in place (phi/field/_resample.py:272-276).  The product keeps the boundary of s
+    (phi/field/_field.py:809): faces next to a constant side c of s average c itself, unscaled, also where factor is 0."""
     require_cuda()
     b = (C.c_float * 3)(*[float(factor[i]) if i < len(factor) else 0.0 for i in range(3)])
     _lib.check(_lib.load().phicuda_add_buoyancy_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(make_bc(sbc)),

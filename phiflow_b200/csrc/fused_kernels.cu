@@ -460,7 +460,8 @@ k_advect_centered_vec(const __grid_constant__ DGrid g, const __grid_constant__ D
 }
 
 // Staggered field, all components in one launch: dst_c = interp(src_c, face_c - dt v(face_c)) [+ dt * buoyancy_c]
-//   buoyancy_c = (s * b_c)[upper cell] * 0.5 + (s * b_c)[lower cell] * 0.5      (sample_grid_at_faces)
+//   buoyancy_c = (s * b_c)[upper cell] * 0.5 + (s * b_c)[lower cell] * 0.5      (sample_grid_at_faces; a constant ghost of s
+//   stays c: the product keeps the boundary of s, phi/field/_field.py:809)
 template <int DIM, bool BUOY>
 __global__ void __launch_bounds__(FK_THREADS, 4)
 k_advect_staggered_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec vel, const __grid_constant__ DVec fld,
@@ -495,8 +496,9 @@ k_advect_staggered_vec(const __grid_constant__ DGrid g, const __grid_constant__ 
     int rS = 0, rSy = 0, rSz = 0;
     bool s_fast = true;
     if (BUOY) {
-        const int s_y = fk_res(y, sf, 1, s_fast), s_ym = b1 != 0.f ? fk_res(y - 1, sf, 1, s_fast) : 0;
-        const int s_z = DIM == 3 ? fk_res(z, sf, 2, s_fast) : 0, s_zm = (DIM == 3 && b2 != 0.f) ? fk_res(z - 1, sf, 2, s_fast) : 0;
+        // every component's lower-cell line, also for b_c = 0: a constant ghost line adds c/2 * dt even then (-> generic code)
+        const int s_y = fk_res(y, sf, 1, s_fast), s_ym = fk_res(y - 1, sf, 1, s_fast);
+        const int s_z = DIM == 3 ? fk_res(z, sf, 2, s_fast) : 0, s_zm = DIM == 3 ? fk_res(z - 1, sf, 2, s_fast) : 0;
         const int ssy = (int)sf.sy, ssz = (int)sf.sz, sbase = b * (int)sf.sb;
         rS = sbase + s_z * ssz + s_y * ssy; rSy = sbase + s_z * ssz + s_ym * ssy; rSz = sbase + s_zm * ssz + s_y * ssy;
     }
@@ -509,8 +511,9 @@ k_advect_staggered_vec(const __grid_constant__ DGrid g, const __grid_constant__ 
         const int x = xb + lane;
         const FkX X = fk_x(fx, fy, n0, xb, x);
         // a chunk that holds faces beyond the last cell (x = n0: stored upper boundary faces) is never "fast"
-        // (the lower x neighbour of the buoyancy source is wrapped / clamped below; a constant x boundary of s needs xb >= 1)
-        const bool fast = rows_ok && X.fast && xb + 32 <= n0 && (!BUOY || (s_fast && (b0 == 0.f || sf.klo[0] != PHI_BC_CONST || xb >= 1)));
+        // (the lower x neighbour of the buoyancy source is wrapped / clamped below; a constant x boundary of s needs xb >= 1 -
+        // whatever b0 is, since the constant ghost enters unscaled)
+        const bool fast = rows_ok && X.fast && xb + 32 <= n0 && (!BUOY || (s_fast && (sf.klo[0] != PHI_BC_CONST || xb >= 1)));
         float r0 = 0.f, r1 = 0.f, r2 = 0.f;
         // a fast chunk lies inside the stored x range of every component, so its store flags are warp-uniform
         const bool st0 = on0 && (fast || (x >= fld.f[0].lo[0] && x <= fld.f[0].hi[0]));
@@ -572,7 +575,7 @@ k_advect_staggered_vec(const __grid_constant__ DGrid g, const __grid_constant__ 
                 if (st1) r1 = fk_interp<DIM>(fld.p[1], g, fld.f[1], b, K1);
                 if (DIM == 3 && st2) r2 = fk_interp<DIM>(fld.p[2], g, fld.f[2], b, K2);
             }
-            if (BUOY) {
+            if (BUOY) {                                            // no constant ghost of s on a fast chunk: b_c = 0 adds 0
                 if (b0 != 0.f) r0 = r0 + ((sc * b0) * 0.5f + (scm * b0) * 0.5f) * dt;
                 if (b1 != 0.f) r1 = r1 + ((sc * b1) * 0.5f + (sy_ * b1) * 0.5f) * dt;
                 if (DIM == 3 && b2 != 0.f) r2 = r2 + ((sc * b2) * 0.5f + (sz_ * b2) * 0.5f) * dt;
@@ -585,9 +588,9 @@ k_advect_staggered_vec(const __grid_constant__ DGrid g, const __grid_constant__ 
                 if (!st) continue;
                 float r = fk_generic_sample<DIM>(&g, &vel, &fld.f[c], fld.p[c], c, b, x, y, z, dt);
                 const float bc = c == 0 ? b0 : (c == 1 ? b1 : b2);
-                if (BUOY && bc != 0.f) {
-                    const float up = phi_fetch<DIM>(s, g, sf, b, x, y, z) * bc;
-                    const float lw = phi_fetch<DIM>(s, g, sf, b, x - (c == 0), y - (c == 1), z - (c == 2)) * bc;
+                if (BUOY) {                                        // a constant ghost of s enters unscaled (phi_fetch_scaled)
+                    const float up = phi_fetch_scaled<DIM>(s, g, sf, b, x, y, z, bc);
+                    const float lw = phi_fetch_scaled<DIM>(s, g, sf, b, x - (c == 0), y - (c == 1), z - (c == 2), bc);
                     r = r + (up * 0.5f + lw * 0.5f) * dt;
                 }
                 if (c == 0) r0 = r; else if (c == 1) r1 = r; else r2 = r;
@@ -623,8 +626,11 @@ int phi_launch_advect_staggered_vec(const DGrid& g, const DVec& vel, const DVec&
                                     const DField* sf, const float* sarr, const float bu[3], cudaStream_t s)
 {
     if (!fits_int32(g)) return -100;
-    const bool buoy = sarr != nullptr && bu && (bu[0] != 0.f || bu[1] != 0.f || (g.dim == 3 && bu[2] != 0.f));
     const DField sfv = sf ? *sf : fld.f[0];
+    bool const_side = false;                 // resample(s * b, to=v) is c/2 * dt next to a constant side c != 0 of s, even for b = 0
+    for (int a = 0; a < g.dim; ++a)
+        const_side = const_side || (sfv.klo[a] == PHI_BC_CONST && sfv.clo[a] != 0.f) || (sfv.khi[a] == PHI_BC_CONST && sfv.chi[a] != 0.f);
+    const bool buoy = sarr != nullptr && bu && (bu[0] != 0.f || bu[1] != 0.f || (g.dim == 3 && bu[2] != 0.f) || const_side);
     const float b0 = buoy ? bu[0] : 0.f, b1 = buoy ? bu[1] : 0.f, b2 = (buoy && g.dim == 3) ? bu[2] : 0.f;
     if (g.dim == 3) {
         if (buoy) k_advect_staggered_vec<3, true><<<adv_grid(g), FK_THREADS, 0, s>>>(g, vel, fld, dst, dt, sfv, sarr, b0, b1, b2);

@@ -73,6 +73,19 @@ __device__ __forceinline__ float phi_fetch(const float* __restrict__ a, const DG
     return __ldg(a + (long long)b * f.sb + (long long)z * f.sz + (long long)y * f.sy + x);
 }
 
+// value of the product s * k at (x, y, z): s * k on stored cells and across periodic / zero-gradient sides, but a constant side
+// keeps its own value c, unscaled - multiplying a field by a constant leaves its boundary unchanged (phi/field/_field.py:809),
+// so resample(s * (0, 0.1), to=v) averages c, not c * 0.1, into the faces next to a constant side of s
+template <int DIM>
+__device__ __forceinline__ float phi_fetch_scaled(const float* __restrict__ a, const DGrid& g, const DField& f, int b, int x, int y, int z, float k)
+{
+    float c = 0.f;
+    if (DIM == 3) { if (!phi_resolve(z, f, 2, c)) return c; } else z = 0;
+    if (!phi_resolve(y, f, 1, c)) return c;
+    if (!phi_resolve(x, f, 0, c)) return c;
+    return __ldg(a + (long long)b * f.sb + (long long)z * f.sz + (long long)y * f.sy + x) * k;
+}
+
 // a / b with a precomputed correctly rounded reciprocal inv_b = RN(1 / b) (DGrid.inv_dx, computed on the host): Markstein's
 // correction q = RN(a * inv_b); r = a - q * b (exact in the FMA); q' = RN(q + r * inv_b) gives the correctly rounded quotient -
 // the value the reference's `/ dx` produces (spatial_gradient, PhiML/phiml/math/_nd.py:813-815) - in 3 instructions instead of

@@ -123,7 +123,8 @@ k_grad_sub(DGrid g, DVec vin, DVecOut v, DField pf, const float* __restrict__ p,
     }
 }
 
-// N2: v_c[face] += ((s*b_c)[upper]*0.5 + (s*b_c)[lower]*0.5) * dt on the stored faces
+// N2: v_c[face] += ((s*b_c)[upper]*0.5 + (s*b_c)[lower]*0.5) * dt on the stored faces; a constant ghost of s stays c (not c * b_c,
+// phi_fetch_scaled), so a face next to a constant side gets c/2 * dt even for b_c = 0
 template <int DIM>
 __global__ void __launch_bounds__(128)
 k_buoyancy(DGrid g, DVec vin, DVecOut v, DField sf, const float* __restrict__ s, float b0, float b1, float b2, float dt)
@@ -134,11 +135,9 @@ k_buoyancy(DGrid g, DVec vin, DVecOut v, DField sf, const float* __restrict__ s,
 #pragma unroll
     for (int c = 0; c < DIM; ++c) {
         const float bc = c == 0 ? b0 : (c == 1 ? b1 : b2);
-        if (bc == 0.f) continue;
         if (!phi_in_range(vin.f[c], DIM, i.x, i.y, i.z)) continue;
-        // the outside value of (s * b_c) is (outside value of s) * b_c for all three boundary kinds
-        const float up = phi_fetch<DIM>(s, g, sf, i.b, i.x, i.y, i.z) * bc;
-        const float lw = phi_fetch<DIM>(s, g, sf, i.b, i.x - (c == 0), i.y - (c == 1), i.z - (c == 2)) * bc;
+        const float up = phi_fetch_scaled<DIM>(s, g, sf, i.b, i.x, i.y, i.z, bc);
+        const float lw = phi_fetch_scaled<DIM>(s, g, sf, i.b, i.x - (c == 0), i.y - (c == 1), i.z - (c == 2), bc);
         v.p[c][off] = vin.p[c][off] + (up * 0.5f + lw * 0.5f) * dt;
     }
 }
