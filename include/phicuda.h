@@ -82,7 +82,8 @@ typedef struct PhiCgParams {
     int32_t method;          /* PHI_SOLVER_CG: Shewchuk CG (_linalg.py:52-90);  PHI_SOLVER_CG_ADAPTIVE: the Hestenes-Stiefel
                                 variant behind Solve('CG-adaptive') and, in PhiML 1.7, Solve('auto') (_linalg.py:93-128,
                                 _backend.py:1446): step (d.r)/(d.Ad), direction r - ((r.Ad)/(d.Ad)) d, tolerance relative
-                                to |y|^2.  Requires matrix_offset == 0. */
+                                to |y|^2 (with balance_rhs: the balanced y').  Requires matrix_offset == 0 and the TMA ring
+                                kernel, with or without obstacles (single GPU); elsewhere PHI_ERR_UNSUPPORTED. */
 } PhiCgParams;
 #define PHI_SOLVER_CG 0
 #define PHI_SOLVER_CG_ADAPTIVE 1
@@ -267,7 +268,8 @@ int phicuda_make_incompressible_centered_host_f32(const PhiGrid* g, const PhiVBC
  * obstacle cells are identity rows), v -= hard_bcs * grad p.  The caller applies apply_boundary_conditions first
  * (v *= 1 - obstacle mask at faces: phicuda_mul_faces_f32).  The solve runs on the TMA-ring kernel with the mask staged as an
  * extra haloed array (k_cg_ring<..., CgOp::Masked>; 5 lines per tile line and stage instead of 4); grids whose lines do not fit the
- * ring fall back to the register-marching kernel. */
+ * ring fall back to the register-marching kernel with PHI_SOLVER_CG, and return PHI_ERR_UNSUPPORTED with PHI_SOLVER_CG_ADAPTIVE
+ * (CG-adaptive runs on the ring only; the z-slab entry phicuda_cg_poisson_dist_masked_f32 takes PHI_SOLVER_CG only). */
 int phicuda_mul_faces_f32(const PhiGrid* g, const PhiVBC* vbc, float* const v[3], const float* const mask[3], void* stream);
 /* the two stencil pieces of the masked projection on their own (z-slab runs exchange halo planes between them):
  * div = divergence(v) * accessible;   v -= hard_bcs * grad p, hard_bcs = min of the two adjacent cells' accessibility */

@@ -328,7 +328,12 @@ int phi_launch_cg(const CgLaunch& l, cudaStream_t s)
         const int e = phi_launch_cg_ring(l, nullptr, s);
         if (e != -100) return e;
     }
-    if (adaptive) { phi_set_error("cg: CG-adaptive runs on the TMA ring kernel only (no obstacles, grid lines must fit the ring)"); return PHI_ERR_UNSUPPORTED; }
+    if (adaptive) {
+        if (!phi_ring_enabled()) phi_set_error("cg: CG-adaptive runs on the TMA ring kernel only, which PHICUDA_NO_RING switches off");
+        else phi_set_error("cg: CG-adaptive runs on the TMA ring kernel only; grid lines of %d cells do not fit it (%d-D%s, batch %d: at most %d cells)",
+                           g.n[0], g.dim, mask ? " with obstacles" : "", g.batch, phi_cg_ring_max_width(g, l.op.kind, true));
+        return PHI_ERR_UNSUPPORTED;
+    }
     if (mask && l.prm.matrix_offset != 0.f) { phi_set_error("cg: matrix_offset is not supported together with obstacles"); return PHI_ERR_UNSUPPORTED; }
     int per_sm = 0;
     int grid = cg_grid_size(g.dim, g.batch, mask, &per_sm);

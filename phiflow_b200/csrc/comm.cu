@@ -90,6 +90,7 @@ int phicuda_cg_poisson_dist_masked_f32(const PhiGrid* g, const PhiVBC* vbc, cons
                                        const PhiCgParams* prm, PhiCgResult* result, PhiComm* c, void* stream)
 {
     if (!accessible) { phi_set_error("cg_dist_masked: accessible is NULL"); return PHI_ERR_INVALID; }
+    if (prm && prm->method == PHI_SOLVER_CG_ADAPTIVE) { phi_set_error("cg_dist_masked: CG-adaptive with obstacles runs on one GPU only"); return PHI_ERR_UNSUPPORTED; }
     return cg_dist(g, vbc, rhs, x, accessible, prm, result, c, stream);
 }
 

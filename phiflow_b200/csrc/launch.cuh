@@ -90,4 +90,6 @@ int phi_launch_cg(const CgLaunch& a, cudaStream_t s);
 // Helmholtz operator l.op); cf[0 .. C-1] = boundary with constants of component c (batch entry b is component b % C; C = 1 for a varying
 // diffusivity).  -100: the grid does not fit the ring.
 bool phi_cg_ring_fits(const DGrid& g, CgOp op);
+// widest grid line the ring CG takes for g's other extents and batch (host-only; error messages of refused solves)
+int phi_cg_ring_max_width(const DGrid& g, CgOp op, bool adapt);
 int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField* cf, cudaStream_t s);

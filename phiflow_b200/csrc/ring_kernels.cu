@@ -1225,7 +1225,7 @@ k_cg_ring(CgRingArgs A)
     constexpr bool MASK = OP == CgOp::Masked;
     static_assert((OP != CgOp::Helmholtz && OP != CgOp::HelmholtzVarying) || (!DIST && !ADAPT && !FUSED),
                   "the Helmholtz operators run on the single-GPU two-sweep CG only");
-    static_assert(!MASK || !ADAPT, "CG-adaptive has no obstacle mask");
+    static_assert(!MASK || !ADAPT || (!DIST && !FUSED), "CG-adaptive with obstacles runs on the single-GPU two-sweep CG only");
     static_assert(!cg_op_xslot(OP) || GENERIC, "the face-minimum stencil runs on the generic consumer");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const CgArgs& a = A.a;
@@ -1445,12 +1445,20 @@ k_cg_ring(CgRingArgs A)
                 else cg_op_unit<DIM, GENERIC, OP, 2, 0>(rg, A, tg, hsrc, esrc, sh.beta[u.b], u, epi);
                 acc0 += epi.acc0; acc1 += epi.acc1;
             });
-        } else {                                    // pass A of CG-adaptive: additionally d'.r (r once more, element-wise)
+        } else if constexpr (OP == CgOp::Poisson) { // pass A of CG-adaptive: additionally d'.r (r once more, element-wise)
             const float* hsrc[2] = {a.r, dold};
             const float* esrc[2] = {a.r, nullptr};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
                 REpiPassAAdapt<PH> epi{dnew, 0.f, 0.f, peer_halo(lo_dnew, hi_dnew)};
                 ring_process_unit<GENERIC, DIM, 2, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, epi);
+                acc0 += epi.acc0; acc1 += epi.acc1;
+            });
+        } else {                                    // the same with obstacles: the mask in the haloed slot after r and dold
+            const float* hsrc[3] = {a.r, dold, a.acc};
+            const float* esrc[2] = {a.r, nullptr};
+            sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
+                REpiPassAAdapt<PH> epi{dnew, 0.f, 0.f, peer_halo(lo_dnew, hi_dnew)};
+                cg_op_unit<DIM, GENERIC, OP, 2, 1>(rg, A, tg, hsrc, esrc, sh.beta[u.b], u, epi);
                 acc0 += epi.acc0; acc1 += epi.acc1;
             });
         }
@@ -1671,7 +1679,8 @@ int phi_launch_laplace_ring(const DGrid& g, const DField& f, const float* x, flo
 }
 
 // ring of the two-sweep CG; lines staged per stage: pass B (even) = 1 haloed + 3 element-wise arrays = 4 TY + 2; with the
-// operator's coefficients (cg_op_xslot: the obstacle mask or the diffusivity) as an extra haloed array 5 TY + 4 (pass A: 3 haloed = 3 TY + 6)
+// operator's coefficients (cg_op_xslot: the obstacle mask or the diffusivity) as an extra haloed array 5 TY + 4 (pass A: 3 haloed = 3 TY + 6;
+// pass A of CG-adaptive with obstacles: r, d, mask haloed + r element-wise = 4 TY + 6), reserved as 5 TY + 6
 static bool cg_ring_config(const DGrid& g, CgOp op, int cgs, int target_units, RingCfg* c)
 {
     const bool xslot = cg_op_xslot(op);
@@ -1696,8 +1705,9 @@ static CgRingKernel cg_ring_kernel(CgOp op, int dim, bool generic, bool dist, bo
                                : (adapt ? k_cg_ring<2, true, false, true> : k_cg_ring<2, true, false, false>))
                        : (dist ? (adapt ? k_cg_ring<2, false, true, true> : k_cg_ring<2, false, true, false>)
                                : (adapt ? k_cg_ring<2, false, false, true> : k_cg_ring<2, false, false, false>));
-    case M:                     // the generic consumer, no CG-adaptive
-        if (!generic || adapt || fused) return nullptr;
+    case M:                     // the generic consumer; CG-adaptive on one GPU only
+        if (!generic || fused || (adapt && dist)) return nullptr;
+        if (adapt) return d3 ? k_cg_ring<3, true, false, true, M> : k_cg_ring<2, true, false, true, M>;
         return d3 ? (dist ? k_cg_ring<3, true, true, false, M> : k_cg_ring<3, true, false, false, M>)
                   : (dist ? k_cg_ring<2, true, true, false, M> : k_cg_ring<2, true, false, false, M>);
     case H:                     // the Helmholtz operators: single-GPU two-sweep CG
@@ -1722,7 +1732,8 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     const int cgs = (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128);
     const int sms = phi_sm_count();
     if (!cg_ring_config(g, op, cgs, sms, &A.cfg)) return -100;
-    // pass A of CG-adaptive stages 2 haloed + 1 element-wise array = 3 TY + 4 lines: one line more than 4 TY + 2 at TY = 1
+    // pass A of CG-adaptive stages 2 haloed + 1 element-wise array = 3 TY + 4 lines: one line more than 4 TY + 2 at TY = 1 (with
+    // obstacles 4 TY + 6 lines, inside the 5 TY + 6 of cg_ring_config)
     if (l.prm.method == PHI_SOLVER_CG_ADAPTIVE && !xslot && A.cfg.TY == 1
         && !ring_config(g, 4, 3, cgs, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
     const int threads = RING_THREADS;
@@ -1863,6 +1874,22 @@ bool phi_cg_ring_fits(const DGrid& g, CgOp op)
     if (g.batch > CG_MAX_BATCH || g.halo != 0) return false;
     RingCfg c;
     return cg_ring_config(g, op, (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128), 1, &c);
+}
+
+// the widest grid line (cells, a multiple of 4) that phi_launch_cg_ring takes for g's other extents and batch with operator op and
+// solver method adapt; 0: none (host-only, no CUDA call; for the error message of a refused solve)
+int phi_cg_ring_max_width(const DGrid& g, CgOp op, bool adapt)
+{
+    if (g.batch > CG_MAX_BATCH || g.halo != 0) return 0;
+    const int cgs = (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128);
+    for (int w = g.cext[0] < 4096 ? g.cext[0] / 4 * 4 : 4096; w >= 4; w -= 4) {       // ty * nx4 <= RING_G * 256: no line beyond 4096
+        DGrid h = g; h.n[0] = w; h.cext[0] = w;
+        RingCfg c;
+        if (!cg_ring_config(h, op, cgs, 1, &c)) continue;
+        if (adapt && !cg_op_xslot(op) && c.TY == 1 && !ring_config(h, 4, 3, cgs, h.dim == 3 ? 4 : 2, RING_MAX_STAGES, 1, &c)) continue;
+        return w;
+    }
+    return 0;
 }
 
 // l.pf: boundary kinds with zeroed constants (the value ghosts of L0 / D0); cf[0 .. C-1]: the boundary with its constants of component

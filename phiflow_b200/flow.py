@@ -3,7 +3,7 @@
 (the surface `from phi.flow import *` gives a grid-fluid notebook: phi/flow.py:13-28), backed by the CUDA kernels.
 
 Mirrored (same names, argument meaning and error behaviour; reference file:line in each docstring):
-    Box, Sphere, union, CenteredGrid, StaggeredGrid, extrapolation (ZERO, ONE, PERIODIC, ZERO_GRADIENT, BOUNDARY, combine_sides),
+    Box, Sphere, union, geom.infinite_cylinder, CenteredGrid, StaggeredGrid, extrapolation (ZERO, ONE, PERIODIC, ZERO_GRADIENT, BOUNDARY, combine_sides),
     Solve, SolveTape, NotConverged, Diverged, field.{divergence, laplace, spatial_gradient}, resample,
     advect.{semi_lagrangian, mac_cormack, advect}, diffuse.{explicit, implicit}, fluid.{make_incompressible, incompressible_step},
     write / read (field.write / field.read: the reference's .npz field files, see field_io.py).
@@ -23,7 +23,7 @@ from . import _ops as ops
 from . import field_io
 from . import scene as _scene
 
-__all__ = ['Scene', 'vec', 'batch', 'iterate', 'jit_compile', 'Box', 'Sphere', 'union', 'CenteredGrid', 'StaggeredGrid', 'extrapolation', 'ZERO', 'ONE', 'PERIODIC', 'ZERO_GRADIENT',
+__all__ = ['Scene', 'vec', 'batch', 'iterate', 'jit_compile', 'Box', 'Sphere', 'union', 'geom', 'CenteredGrid', 'StaggeredGrid', 'extrapolation', 'ZERO', 'ONE', 'PERIODIC', 'ZERO_GRADIENT',
            'BOUNDARY', 'combine_sides', 'Solve', 'SolveTape', 'NotConverged', 'Diverged', 'ConvergenceException', 'field',
            'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read']
 
@@ -168,6 +168,31 @@ class Sphere:
         return np.clip(np.float32(0.5) - (d - np.float32(self.radius)) / np.float32(cell_radius), 0, 1).astype(np.float32)
 
 
+class InfiniteCylinder:
+    """geom.infinite_cylinder(x=20, y=50, radius=10, inf_dim='z')  (phi/geom/_embed.py:139-158): a Sphere over the named axes,
+    embedded along `inf_dim`.  Points are projected onto the sphere's axes (_EmbeddedGeometry._down_project, _embed.py:41-47)."""
+
+    def __init__(self, sphere: Sphere, inf_dim: str):
+        self.sphere, self.inf_dim = sphere, inf_dim
+
+    def _down_project(self, pts):
+        return pts[..., [AXES.index(n) for n in self.sphere.names]]
+
+    def lies_inside(self, pts):
+        return self.sphere.lies_inside(self._down_project(pts))
+
+    def signed_distance(self, pts):
+        return self.sphere.signed_distance(self._down_project(pts))
+
+
+def infinite_cylinder(center=None, radius=None, inf_dim: str = None, **center_):
+    """geom.infinite_cylinder (phi/geom/_embed.py:139-158) with the centre as keyword arguments over the other axes."""
+    _require(center is None and isinstance(inf_dim, str) and inf_dim in AXES and inf_dim not in center_ and radius is not None,
+             "infinite_cylinder other than infinite_cylinder(x=..., y=..., radius=..., inf_dim='z')")
+    _require(all(n in AXES for n in center_), f"cylinder axes {tuple(center_)}")
+    return InfiniteCylinder(Sphere(radius, **center_), inf_dim)
+
+
 class Union:
     """union(Box(...), Box(...))  (phi/geom/_geom_ops.py:297-320): a point lies inside when it lies inside any member."""
 
@@ -189,6 +214,9 @@ def union(*geometries):
         _require(isinstance(g, (Box, Sphere, Union)), f"union of {type(g).__name__}")
         flat += list(g.geometries) if isinstance(g, Union) else [g]
     return Union(*flat)
+
+
+geom = SimpleNamespace(Box=Box, Sphere=Sphere, union=union, infinite_cylinder=infinite_cylinder)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -722,13 +750,13 @@ diffuse = SimpleNamespace(explicit=explicit, implicit=implicit)
 # ----------------------------------------------------------------------------------------------------------------------
 # fluid  (phi/physics/fluid.py)
 # ----------------------------------------------------------------------------------------------------------------------
-def _cg_params(v: StaggeredGrid, solve: Solve, masked=False):
+def _cg_params(v: StaggeredGrid, solve: Solve):
     # Solver policy = the reference's: 'CG' is Shewchuk CG (the north-star solver); 'auto' (the default Solve()) and
     # 'CG-adaptive' run the Hestenes-Stiefel variant exactly as the vendored PhiML maps them (backend/_backend.py:1446-1447,
-    # _linalg.py:93-128), tolerance relative to |rhs|^2.  Exception: with obstacle masks the adaptive variant is not
-    # available (it lives on the TMA ring kernel only), so 'auto' runs plain CG there and an explicit 'CG-adaptive' raises.
+    # _linalg.py:93-128), tolerance relative to |rhs|^2, with and without obstacle masks.  CG-adaptive lives on the TMA ring
+    # kernel only: on grids whose lines do not fit it, 'auto' and 'CG-adaptive' raise Unsupported.
     _require(solve.method in ('CG', 'auto', 'CG-adaptive'), f"solver '{solve.method}'")
-    adaptive = solve.method == 'CG-adaptive' or (solve.method == 'auto' and not masked)
+    adaptive = solve.method in ('CG-adaptive', 'auto')
     return ops.cg_params(v.vspec, rtol=solve.rel_tol, atol=solve.abs_tol, max_iter=solve.max_iterations,
                          matrix_offset=0.0 if adaptive else solve.matrix_offset, method='CG-adaptive' if adaptive else 'CG')
 
@@ -748,7 +776,8 @@ def _obstacle_masks(velocity: StaggeredGrid, obstacles):
     """Static obstacles (phi/physics/fluid.py:130-137, 212-240): returns (accessible centred mask, per-component face factors
     1 - resample(geometry, velocity, soft=True, balance=1)).  Geometry sampling is set-up work done on the host."""
     geoms = list(obstacles) if isinstance(obstacles, (tuple, list)) else [obstacles]
-    _require(all(isinstance(o, (Box, Sphere)) for o in geoms), "obstacles other than stationary Box / Sphere geometries")
+    _require(all(isinstance(o, (Box, Sphere, InfiniteCylinder)) for o in geoms),
+             "obstacles other than stationary Box / Sphere / infinite_cylinder geometries")
     centred = CenteredGrid(0, ZERO, velocity.bounds, velocity.batch, **dict(zip(velocity.axes, velocity.res)))
     pts = centred.points()
     inside = np.zeros(pts.shape[:-1], bool)
@@ -768,7 +797,7 @@ def _obstacle_masks(velocity: StaggeredGrid, obstacles):
 
 def make_incompressible(velocity: StaggeredGrid, obstacles=(), solve: Solve = None, active=None, order=2):
     """fluid.make_incompressible (phi/physics/fluid.py:94-162): returns (divergence-free velocity, pressure).
-    obstacles: stationary Box / Sphere geometries (row N4)."""
+    obstacles: stationary Box / Sphere / infinite_cylinder geometries (row N4)."""
     solve = solve or Solve()
     _require(isinstance(velocity, StaggeredGrid), "CenteredGrid velocities")
     _require(active is None and order == 2, "active masks / higher order")
@@ -780,7 +809,7 @@ def make_incompressible(velocity: StaggeredGrid, obstacles=(), solve: Solve = No
         p_data = solve.x0.data.clone() if solve.x0 is not None else velocity.dom.alloc_centered()
         v_data = [c.clone() for c in velocity.data]
         ops.mul_faces(velocity.dom, velocity.vspec, v_data, factors)             # apply_boundary_conditions
-        ops.make_incompressible(velocity.dom, velocity.vspec, v_data, p_data, _cg_params(velocity, solve, masked=True), accessible=accessible)
+        ops.make_incompressible(velocity.dom, velocity.vspec, v_data, p_data, _cg_params(velocity, solve), accessible=accessible)
         _finish_solve(velocity.dom, solve)
         pressure = CenteredGrid(boundary=_pressure_boundary(velocity.boundary), bounds=velocity.bounds, batch=velocity.batch, _data=p_data, **res)
         return velocity.with_values(v_data), pressure
