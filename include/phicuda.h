@@ -303,6 +303,18 @@ size_t phicuda_plume_scratch_bytes(const PhiGrid* g);
 int phicuda_plume_step_f32(const PhiGrid* g, const PhiVBC* vbc, const PhiBC* sbc, float* const v[3], float* s, float* p,
                            const float* inflow, const PhiPlumeParams* sp, const PhiCgParams* prm, PhiCgResult* result,
                            float* scratch, void* workspace, size_t workspace_bytes, void* stream);
+/* The same step with static obstacles (N4; Batched_Smoke, Fluid_Logo): the smoke is advected as above, then
+ * v* = (semi_lagrangian(v, v, dt) + dt * buoyancy(s')) * face_factors   (apply_boundary_conditions, one advection launch) and
+ * v', p' = make_incompressible(v*, obstacles, Solve(x0 = p)) as phicuda_make_incompressible_masked_f32 computes it.
+ * accessible: centred mask (1 fluid, 0 obstacle); face_factors[c]: 1 - resample(geometry, v, soft=True, balance=1) on the stored
+ * faces of component c (fext layout).  Both carry the full batch: every batch entry may have its own obstacle.  The result is bit for
+ * bit that of phicuda_plume_step_f32's advection, phicuda_mul_faces_f32 and phicuda_make_incompressible_masked_f32 in sequence.
+ * prm->method: PHI_SOLVER_CG or PHI_SOLVER_CG_ADAPTIVE (ring-only, as phicuda_cg_poisson_masked_f32), matrix_offset 0.
+ * Single GPU: z-slab grids (halo > 0) return PHI_ERR_UNSUPPORTED.  Every argument check runs before the first CUDA call. */
+int phicuda_plume_step_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const PhiBC* sbc, float* const v[3], float* s, float* p,
+                                  const float* inflow, const float* accessible, const float* const face_factors[3],
+                                  const PhiPlumeParams* sp, const PhiCgParams* prm, PhiCgResult* result,
+                                  float* scratch, void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

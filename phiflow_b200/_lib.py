@@ -105,6 +105,9 @@ PROTOTYPES = {
     'phicuda_plume_step_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiBC), F3, C.c_void_p, C.c_void_p, C.c_void_p,
                                          _P(PhiPlumeParams), _P(PhiCgParams), C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_size_t, C.c_void_p]),
+    'phicuda_plume_step_masked_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiBC), F3, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, F3, _P(PhiPlumeParams), _P(PhiCgParams), C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 

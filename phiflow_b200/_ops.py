@@ -512,12 +512,16 @@ def make_incompressible_centered(dom: Domain, vbc, v: List[torch.Tensor], p: tor
 
 
 def plume_step(dom: Domain, vbc, sbc, v, s, p, inflow, dt, inflow_rate, buoyancy, prm: PhiCgParams, mac_cormack=False, cg_events=None,
-               static_scalar=False):
+               static_scalar=False, accessible=None, factors=None):
     """incompressible_step: the notebook step (examples/grids/Smoke_Plume.ipynb:58-68) as one C-ABI call; state updated in place.
     cg_events: optional pair of torch.cuda.Event(enable_timing=True) that the library records around the pressure solve.
-    static_scalar: `s` is a stationary forcing field (v* = advect(v) + dt * resample(s * buoyancy, to=v)), not advected smoke."""
+    static_scalar: `s` is a stationary forcing field (v* = advect(v) + dt * resample(s * buoyancy, to=v)), not advected smoke.
+    accessible, factors: static obstacles (Batched_Smoke, Fluid_Logo) - the centred accessible mask and the per-component face factors
+    of apply_boundary_conditions (flow._obstacle_masks), both with the full batch (one obstacle per entry); v* is multiplied by the
+    factors and projected with the masked operator (phicuda_plume_step_masked_f32)."""
     require_cuda()
     assert dom.halo == 0, "plume_step is the single-GPU fused call; z-slab runs sequence the step in phiflow_b200.dist"
+    assert (accessible is None) == (factors is None), "obstacles need both the accessible mask and the face factors"
     ws, res = dom.workspace()
     sp = PhiPlumeParams()
     sp.dt, sp.inflow_rate, sp.mac_cormack, sp.static_scalar = dt, inflow_rate, int(mac_cormack), int(static_scalar)
@@ -528,6 +532,12 @@ def plume_step(dom: Domain, vbc, sbc, v, s, p, inflow, dt, inflow_rate, buoyancy
             if not ev.cuda_event:                   # torch creates the cudaEvent_t lazily at the first record
                 ev.record()
         sp.cg_start_event, sp.cg_stop_event = cg_events[0].cuda_event, cg_events[1].cuda_event
+    if accessible is not None:
+        _lib.check(_lib.load().phicuda_plume_step_masked_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(make_bc(sbc)), _f3(v),
+                                                             _ptr(s), _ptr(p), _ptr(inflow), _ptr(accessible), _f3(factors), C.byref(sp),
+                                                             C.byref(prm), _ptr(res), _ptr(dom.scratch()), _ptr(ws), C.c_size_t(ws.numel()),
+                                                             _stream()))
+        return v, s, p
     _lib.check(_lib.load().phicuda_plume_step_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(make_bc(sbc)), _f3(v),
                                                   _ptr(s), _ptr(p), _ptr(inflow), C.byref(sp), C.byref(prm), _ptr(res),
                                                   _ptr(dom.scratch()), _ptr(ws), C.c_size_t(ws.numel()), _stream()))

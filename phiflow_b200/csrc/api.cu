@@ -5,6 +5,7 @@
 #include <cstdlib>
 #include <cstring>
 #include "phi_internal.cuh"
+#include "cg_common.cuh"
 #include "launch.cuh"
 
 // ---- error state -----------------------------------------------------------------------------------------------
@@ -240,7 +241,7 @@ int phicuda_divergence_f32(const PhiGrid* g, const PhiVBC* vbc, const float* con
     DGrid dg; DVec dv; DField cf; PhiBC none; memset(&none, 0, sizeof(none));
     CHECK(phi_make_dgrid(g, &dg)); CHECK(make_vec(g, vbc, v, &dv)); CHECK(phi_make_centered(g, &none, &cf));
     if (!div) { phi_set_error("divergence: div is NULL"); return PHI_ERR_INVALID; }
-    if (!phi_scalar_kernels()) return cuda_fail(phi_launch_divergence_vec(dg, dv, cf, div, (cudaStream_t)stream), "divergence");
+    if (!phi_scalar_kernels()) return cuda_fail(phi_launch_divergence_vec(dg, dv, cf, div, nullptr, (cudaStream_t)stream), "divergence");
     return cuda_fail(phi_launch_divergence(dg, dv, cf, div, nullptr, (cudaStream_t)stream), "divergence");
 }
 
@@ -251,7 +252,7 @@ int phicuda_grad_sub_f32(const PhiGrid* g, const PhiVBC* vbc, float* const v[3],
     CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &pf));
     if (!p) { phi_set_error("grad_sub: p is NULL"); return PHI_ERR_INVALID; }
     for (int c = 0; c < 3; ++c) out.p[c] = c < g->dim ? v[c] : nullptr;
-    if (!phi_scalar_kernels()) return cuda_fail(phi_launch_grad_sub_vec(dg, dv, out, pf, p, (cudaStream_t)stream), "grad_sub");
+    if (!phi_scalar_kernels()) return cuda_fail(phi_launch_grad_sub_vec(dg, dv, out, pf, p, nullptr, nullptr, (cudaStream_t)stream), "grad_sub");
     return cuda_fail(phi_launch_grad_sub(dg, dv, out, pf, p, nullptr, nullptr, (cudaStream_t)stream), "grad_sub");
 }
 
@@ -279,7 +280,7 @@ int phicuda_advect_staggered_f32(const PhiGrid* g, const PhiVBC* vbc, const floa
     }
     if (!phi_scalar_kernels()) {      // all components in one launch: the velocity lines are loaded once and shared
         DVecOut out; for (int c = 0; c < 3; ++c) out.p[c] = c < g->dim ? dst[c] : nullptr;
-        const int e = phi_launch_advect_staggered_vec(dg, dv, df, out, dt, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+        const int e = phi_launch_advect_staggered_vec(dg, dv, df, out, dt, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
         if (e != -100) return cuda_fail(e, "advect_staggered");
     }
     for (int c = 0; c < g->dim; ++c)
@@ -350,6 +351,7 @@ int phicuda_divergence_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const flo
     DGrid dg; DVec dv; DField cf; PhiBC none; memset(&none, 0, sizeof(none));
     CHECK(phi_make_dgrid(g, &dg)); CHECK(make_vec(g, vbc, v, &dv)); CHECK(phi_make_centered(g, &none, &cf));
     if (!div || !accessible) { phi_set_error("divergence_masked: NULL argument"); return PHI_ERR_INVALID; }
+    if (!phi_scalar_kernels()) return cuda_fail(phi_launch_divergence_vec(dg, dv, cf, div, accessible, (cudaStream_t)stream), "divergence_masked");
     return cuda_fail(phi_launch_divergence(dg, dv, cf, div, accessible, (cudaStream_t)stream), "divergence_masked");
 }
 
@@ -360,6 +362,7 @@ int phicuda_grad_sub_masked_f32(const PhiGrid* g, const PhiVBC* vbc, float* cons
     CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &pf)); CHECK(accessible_field(g, vbc, &af));
     if (!p || !accessible) { phi_set_error("grad_sub_masked: NULL argument"); return PHI_ERR_INVALID; }
     for (int c = 0; c < 3; ++c) out.p[c] = c < g->dim ? v[c] : nullptr;
+    if (!phi_scalar_kernels()) return cuda_fail(phi_launch_grad_sub_vec(dg, dv, out, pf, p, &af, accessible, (cudaStream_t)stream), "grad_sub_masked");
     return cuda_fail(phi_launch_grad_sub(dg, dv, out, pf, p, &af, accessible, (cudaStream_t)stream), "grad_sub_masked");
 }
 
@@ -384,19 +387,16 @@ int phicuda_cg_poisson_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const flo
     return phi_launch_cg(l, (cudaStream_t)stream);
 }
 
+static int project(const PhiGrid* g, const PhiVBC* vbc, const float* const vin[3], float* const vout[3], float* p, float* div,
+                   const float* accessible, const PhiCgParams* prm, PhiCgResult* result, void* workspace, size_t workspace_bytes,
+                   void* ev0, void* ev1, void* stream);
+
 int phicuda_make_incompressible_masked_f32(const PhiGrid* g, const PhiVBC* vbc, float* const v[3], float* p, float* div,
                                            const float* accessible, const PhiCgParams* prm, PhiCgResult* result,
                                            void* workspace, size_t workspace_bytes, void* stream)
 {
-    DGrid dg; DVec dv; DVecOut out; DField cf, af, pf; PhiBC none, pbc; memset(&none, 0, sizeof(none));
-    CHECK(phi_make_dgrid(g, &dg)); CHECK(make_vec(g, vbc, v, &dv)); CHECK(phi_make_centered(g, &none, &cf));
     if (!accessible || !p || !div) { phi_set_error("make_incompressible_masked: NULL argument"); return PHI_ERR_INVALID; }
-    CHECK(accessible_field(g, vbc, &af));
-    CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &pf));
-    for (int c = 0; c < 3; ++c) out.p[c] = c < g->dim ? v[c] : nullptr;
-    CHECK(cuda_fail(phi_launch_divergence(dg, dv, cf, div, accessible, (cudaStream_t)stream), "divergence"));       // div *= active
-    CHECK(phicuda_cg_poisson_masked_f32(g, vbc, div, p, accessible, prm, result, workspace, workspace_bytes, stream));
-    return cuda_fail(phi_launch_grad_sub(dg, dv, out, pf, p, &af, accessible, (cudaStream_t)stream), "grad_sub");   // grad *= hard_bcs
+    return project(g, vbc, v, v, p, div, accessible, prm, result, workspace, workspace_bytes, nullptr, nullptr, stream);
 }
 
 size_t phicuda_cg_workspace_bytes(const PhiGrid* g)
@@ -497,12 +497,16 @@ int phicuda_diffuse_implicit_varying_f32(const PhiGrid* g, const PhiBC* bc, cons
 }
 
 // div -> CG -> v = vin - grad p.  vin/vout may be the same arrays (make_incompressible) or scratch -> state (fused step).
+// accessible != nullptr: the obstacle projection (N4), div *= accessible, masked CG, grad p *= hard_bcs.  The stencils take the float4
+// kernels unless PHICUDA_SCALAR_KERNELS=1, with and without the mask.
 static int project(const PhiGrid* g, const PhiVBC* vbc, const float* const vin[3], float* const vout[3], float* p, float* div,
-                   const PhiCgParams* prm, PhiCgResult* result, void* workspace, size_t workspace_bytes, void* ev0, void* ev1, void* stream)
+                   const float* accessible, const PhiCgParams* prm, PhiCgResult* result, void* workspace, size_t workspace_bytes,
+                   void* ev0, void* ev1, void* stream)
 {
-    DGrid dg; DVec dv; DVecOut out; DField cf, pf; PhiBC none, pbc; memset(&none, 0, sizeof(none));
+    DGrid dg; DVec dv; DVecOut out; DField cf, pf, af; PhiBC none, pbc; memset(&none, 0, sizeof(none));
     CHECK(phi_make_dgrid(g, &dg)); CHECK(make_vec(g, vbc, vin, &dv)); CHECK(phi_make_centered(g, &none, &cf));
     CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &pf));
+    if (accessible) CHECK(accessible_field(g, vbc, &af));
     if (!p || !div || !vout) { phi_set_error("make_incompressible: NULL argument"); return PHI_ERR_INVALID; }
     for (int c = 0; c < 3; ++c) {
         out.p[c] = c < g->dim ? vout[c] : nullptr;
@@ -510,18 +514,20 @@ static int project(const PhiGrid* g, const PhiVBC* vbc, const float* const vin[3
     }
     cudaStream_t st = (cudaStream_t)stream;
     const bool scalar = phi_scalar_kernels();
-    CHECK(cuda_fail(scalar ? phi_launch_divergence(dg, dv, cf, div, nullptr, st) : phi_launch_divergence_vec(dg, dv, cf, div, st), "divergence"));
+    const DField* afp = accessible ? &af : nullptr;
+    CHECK(cuda_fail(scalar ? phi_launch_divergence(dg, dv, cf, div, accessible, st) : phi_launch_divergence_vec(dg, dv, cf, div, accessible, st), "divergence"));
     if (ev0) CHECK(cuda_fail(cudaEventRecord((cudaEvent_t)ev0, st), "cudaEventRecord"));
-    CHECK(phicuda_cg_poisson_f32(g, vbc, div, p, prm, result, workspace, workspace_bytes, stream));
+    if (accessible) CHECK(phicuda_cg_poisson_masked_f32(g, vbc, div, p, accessible, prm, result, workspace, workspace_bytes, stream));
+    else            CHECK(phicuda_cg_poisson_f32(g, vbc, div, p, prm, result, workspace, workspace_bytes, stream));
     if (ev1) CHECK(cuda_fail(cudaEventRecord((cudaEvent_t)ev1, st), "cudaEventRecord"));
-    return cuda_fail(scalar ? phi_launch_grad_sub(dg, dv, out, pf, p, nullptr, nullptr, st) : phi_launch_grad_sub_vec(dg, dv, out, pf, p, st), "grad_sub");
+    return cuda_fail(scalar ? phi_launch_grad_sub(dg, dv, out, pf, p, afp, accessible, st) : phi_launch_grad_sub_vec(dg, dv, out, pf, p, afp, accessible, st), "grad_sub");
 }
 
 int phicuda_make_incompressible_f32(const PhiGrid* g, const PhiVBC* vbc, float* const v[3], float* p, float* div,
                                     const PhiCgParams* prm, PhiCgResult* result, void* workspace,
                                     size_t workspace_bytes, void* stream)
 {
-    return project(g, vbc, v, v, p, div, prm, result, workspace, workspace_bytes, nullptr, nullptr, stream);
+    return project(g, vbc, v, v, p, div, nullptr, prm, result, workspace, workspace_bytes, nullptr, nullptr, stream);
 }
 
 // ---- CenteredGrid velocities (wide stencil) -------------------------------------------------------------------------------
@@ -578,13 +584,15 @@ size_t phicuda_plume_scratch_bytes(const PhiGrid* g)
     return g ? (2 * centred_elems(g) + (size_t)g->dim * face_elems(g)) * sizeof(float) : 0;
 }
 
-int phicuda_plume_step_f32(const PhiGrid* g, const PhiVBC* vbc, const PhiBC* sbc, float* const v[3], float* s, float* p,
-                           const float* inflow, const PhiPlumeParams* sp, const PhiCgParams* prm, PhiCgResult* result,
-                           float* scratch, void* workspace, size_t workspace_bytes, void* stream)
+// The step without the argument checks of its entry point.  faces / accessible: static obstacles (N4), nullptr = none.
+static int plume_step(const PhiGrid* g, const PhiVBC* vbc, const PhiBC* sbc, float* const v[3], float* s, float* p,
+                      const float* inflow, const float* accessible, const float* const* faces, const PhiPlumeParams* sp,
+                      const PhiCgParams* prm, PhiCgResult* result, float* scratch, void* workspace, size_t workspace_bytes, void* stream)
 {
     // Launch sequence (5 kernels + 1 device copy; round 1: 9 kernels + 4 copies):
     //   1. s_new = interp(s, x - dt v) + rate * inflow                      advection with the inflow as epilogue
-    //   2. v*    = interp(v, faces - dt v) + dt * buoyancy(s_new)           all components in one launch, buoyancy as epilogue
+    //   2. v*    = (interp(v, faces - dt v) + dt * buoyancy(s_new)) [* f]   all components in one launch, buoyancy and the
+    //                                                                        obstacle face factors as epilogues
     //   3. s     <- s_new                                                    (the only copy: s cannot be advected in place)
     //   4. div   = divergence(v*)     5. p = CG(div, x0 = p)                 6. v = v* - grad p   (written into the caller's v)
     DGrid dg; DVec dv; DField sf;
@@ -599,22 +607,24 @@ int phicuda_plume_step_f32(const PhiGrid* g, const PhiVBC* vbc, const PhiBC* sbc
     for (int c = 0; c < 3; ++c) { vn[c] = c < g->dim ? scratch + 2 * carr + c * farr : nullptr; out.p[c] = vn[c]; }
     cudaStream_t st = (cudaStream_t)stream;
     const bool has_inflow = inflow && sp->inflow_rate != 0.f;
+    const bool big = (long long)farr > (1ll << 31) - (1ll << 20);     // beyond 32-bit element offsets: 64-bit scalar kernels
     if (sp->static_scalar) {                // forced step: s is a stationary source field
-        if (phi_scalar_kernels() || (long long)farr > (1ll << 31) - (1ll << 20)) {
+        if (phi_scalar_kernels() || big) {
             CHECK(phicuda_advect_staggered_f32(g, vbc, v, vbc, v, vn, sp->dt, stream));
             CHECK(phicuda_add_buoyancy_f32(g, vbc, sbc, s, sp->buoyancy, sp->dt, vn, stream));
+            if (faces) CHECK(phicuda_mul_faces_f32(g, vbc, vn, faces, stream));
         } else {
-            CHECK(cuda_fail(phi_launch_advect_staggered_vec(dg, dv, dv, out, sp->dt, &sf, s, sp->buoyancy, st), "advect_staggered"));
+            CHECK(cuda_fail(phi_launch_advect_staggered_vec(dg, dv, dv, out, sp->dt, &sf, s, sp->buoyancy, faces, st), "advect_staggered"));
         }
-        return project(g, vbc, vn, v, p, tmp, prm, result, workspace, workspace_bytes, sp->cg_start_event, sp->cg_stop_event, stream);
+        return project(g, vbc, vn, v, p, tmp, accessible, prm, result, workspace, workspace_bytes, sp->cg_start_event, sp->cg_stop_event, stream);
     }
-    const bool big = (long long)farr > (1ll << 31) - (1ll << 20);     // beyond 32-bit element offsets: 64-bit scalar kernels
     if (phi_scalar_kernels() || big) {      // round-1 sequence, kept for A/B comparisons
         if (sp->mac_cormack) CHECK(phicuda_mac_cormack_centered_f32(g, vbc, v, sbc, s, s_new, tmp, sp->dt, 1.0f, stream));
         else                 CHECK(phicuda_advect_centered_f32(g, vbc, v, sbc, s, s_new, sp->dt, stream));
         if (has_inflow) CHECK(phicuda_axpy_centered_f32(g, sp->inflow_rate, inflow, s_new, stream));
         CHECK(phicuda_advect_staggered_f32(g, vbc, v, vbc, v, vn, sp->dt, stream));
         CHECK(phicuda_add_buoyancy_f32(g, vbc, sbc, s_new, sp->buoyancy, sp->dt, vn, stream));
+        if (faces) CHECK(phicuda_mul_faces_f32(g, vbc, vn, faces, stream));
     } else {
         if (sp->mac_cormack) {
             CHECK(cuda_fail(phi_launch_mac_cormack(dg, dv, sf, s, s_new, tmp, sp->dt, 1.0f, st), "mac_cormack"));
@@ -622,11 +632,51 @@ int phicuda_plume_step_f32(const PhiGrid* g, const PhiVBC* vbc, const PhiBC* sbc
         } else {
             CHECK(cuda_fail(phi_launch_advect_centered_vec(dg, dv, sf, s, s_new, sp->dt, has_inflow ? inflow : nullptr, sp->inflow_rate, st), "advect_centered"));
         }
-        CHECK(cuda_fail(phi_launch_advect_staggered_vec(dg, dv, dv, out, sp->dt, &sf, s_new, sp->buoyancy, st), "advect_staggered"));
+        CHECK(cuda_fail(phi_launch_advect_staggered_vec(dg, dv, dv, out, sp->dt, &sf, s_new, sp->buoyancy, faces, st), "advect_staggered"));
     }
     cudaError_t e = cudaMemcpyAsync(s, s_new, carr * sizeof(float), cudaMemcpyDeviceToDevice, st);
     if (e) return cuda_fail(e, "plume_step copy s");
-    return project(g, vbc, vn, v, p, tmp, prm, result, workspace, workspace_bytes, sp->cg_start_event, sp->cg_stop_event, stream);
+    return project(g, vbc, vn, v, p, tmp, accessible, prm, result, workspace, workspace_bytes, sp->cg_start_event, sp->cg_stop_event, stream);
+}
+
+int phicuda_plume_step_f32(const PhiGrid* g, const PhiVBC* vbc, const PhiBC* sbc, float* const v[3], float* s, float* p,
+                           const float* inflow, const PhiPlumeParams* sp, const PhiCgParams* prm, PhiCgResult* result,
+                           float* scratch, void* workspace, size_t workspace_bytes, void* stream)
+{
+    return plume_step(g, vbc, sbc, v, s, p, inflow, nullptr, nullptr, sp, prm, result, scratch, workspace, workspace_bytes, stream);
+}
+
+int phicuda_plume_step_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const PhiBC* sbc, float* const v[3], float* s, float* p,
+                                  const float* inflow, const float* accessible, const float* const face_factors[3],
+                                  const PhiPlumeParams* sp, const PhiCgParams* prm, PhiCgResult* result,
+                                  float* scratch, void* workspace, size_t workspace_bytes, void* stream)
+{
+    // every check of the step, its projection and its solve runs before the first CUDA call: a refused step leaves the state untouched
+    DGrid dg; DVec dv; DField sf, cf, pf, af; PhiBC none, pbc; memset(&none, 0, sizeof(none));
+    CHECK(phi_make_dgrid(g, &dg));
+    if (!sp || !scratch || !s || !p || !v || !prm || !result || !workspace) { phi_set_error("plume_step_masked: NULL argument"); return PHI_ERR_INVALID; }
+    if (!accessible || !face_factors) { phi_set_error("plume_step_masked: accessible / face_factors is NULL"); return PHI_ERR_INVALID; }
+    for (int c = 0; c < g->dim; ++c)
+        if (!face_factors[c]) { phi_set_error("plume_step_masked: face_factors[%d] is NULL", c); return PHI_ERR_INVALID; }
+    if (g->halo != 0) { phi_set_error("plume_step_masked: z-slab grids are not supported (slab runs sequence the step in dist.py)"); return PHI_ERR_UNSUPPORTED; }
+    CHECK(make_vec(g, vbc, v, &dv)); CHECK(phi_make_centered(g, sbc, &sf)); CHECK(phi_make_centered(g, &none, &cf));
+    CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &pf)); CHECK(accessible_field(g, vbc, &af));
+    if (g->batch > CG_MAX_BATCH) { phi_set_error("cg: batch %d exceeds %d (split the batch)", g->batch, CG_MAX_BATCH); return PHI_ERR_UNSUPPORTED; }
+    const size_t ws_need = phi_cg_workspace(dg, nullptr).bytes;
+    if (workspace_bytes < ws_need) { phi_set_error("cg: workspace %zu < %zu bytes", workspace_bytes, ws_need); return PHI_ERR_WORKSPACE; }
+    const bool adaptive = prm->method == PHI_SOLVER_CG_ADAPTIVE;
+    if (prm->method != PHI_SOLVER_CG && !adaptive) { phi_set_error("cg: unknown solver method %d", prm->method); return PHI_ERR_INVALID; }
+    if (prm->matrix_offset != 0.f) {
+        phi_set_error(adaptive ? "cg: CG-adaptive does not take a matrix_offset" : "cg: matrix_offset is not supported together with obstacles");
+        return PHI_ERR_UNSUPPORTED;
+    }
+    if (adaptive && (!phi_ring_enabled() || !phi_cg_ring_fits(dg, CgOp::Masked))) {     // the message of phi_launch_cg
+        if (!phi_ring_enabled()) phi_set_error("cg: CG-adaptive runs on the TMA ring kernel only, which PHICUDA_NO_RING switches off");
+        else phi_set_error("cg: CG-adaptive runs on the TMA ring kernel only; grid lines of %d cells do not fit it (%d-D%s, batch %d: at most %d cells)",
+                           g->n[0], g->dim, " with obstacles", g->batch, phi_cg_ring_max_width(dg, CgOp::Masked, true));
+        return PHI_ERR_UNSUPPORTED;
+    }
+    return plume_step(g, vbc, sbc, v, s, p, inflow, accessible, face_factors, sp, prm, result, scratch, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -1,6 +1,6 @@
-// Vectorised projection stencils (A5 divergence, A6 gradient subtraction) and the one-launch semi-Lagrangian advection
-// (A9-A11) of the incompressible step, replacing the one-thread-per-sample kernels of round 1 (stencil_kernels.cu /
-// advect_kernels.cu keep those as the obstacle-mask variants and as the arithmetic these kernels must reproduce).
+// Vectorised projection stencils (A5 divergence, A6 gradient subtraction, with or without static obstacle masks) and the
+// one-launch semi-Lagrangian advection (A9-A11) of the incompressible step, replacing the one-thread-per-sample kernels of
+// round 1 (stencil_kernels.cu / advect_kernels.cu keep those as the arithmetic these kernels must reproduce).
 //
 // Design (SURVEY.md section 8d byte table; profiles/r2_ncu_summary.md has the measurements behind each choice):
 //   * a warp owns one grid line (y, z) and walks a 128-cell x segment; which neighbouring lines a stencil reads, and whether
@@ -75,10 +75,12 @@ __device__ __forceinline__ FkLine fk_line4(const DGrid& g)
 
 // ---------------------------------------------------------------------------------------------------------
 // A5  divergence:  div = sum_d (v_d[i + e_d] - v_d[i]) / dx_d      16 B/cell (3-D), 12 (2-D)
+// MASK (N4): div *= accessible, one more float4 per group (20 / 16 B/cell); the product of k_divergence with a mask
 // ---------------------------------------------------------------------------------------------------------
-template <int DIM>
+template <int DIM, bool MASK>
 __global__ void __launch_bounds__(FK_THREADS)
-k_div_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec v, const __grid_constant__ DField cf, float* __restrict__ div)
+k_div_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec v, const __grid_constant__ DField cf, float* __restrict__ div,
+          const float* __restrict__ accm)
 {
     const FkLine L = fk_line4<DIM>(g);
     if (!L.ok || L.y >= g.n[1] || L.z < 0 || L.z >= g.n[2]) return;          // whole warp leaves together
@@ -120,28 +122,40 @@ k_div_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec v, const
         o.x += phi_div(az1.x - az0.x, dz, iz); o.y += phi_div(az1.y - az0.y, dz, iz);
         o.z += phi_div(az1.z - az0.z, dz, iz); o.w += phi_div(az1.w - az0.w, dz, iz);
     }
-    float* dst = div + (long long)L.b * cf.sb + (long long)L.z * cf.sz + (long long)L.y * cf.sy + x0;
+    const long long coff = (long long)L.b * cf.sb + (long long)L.z * cf.sz + (long long)L.y * cf.sy + x0;
+    if (MASK) {                                                             // cext[0] % 4 == 0: the float4 stays in the row
+        const float4 m = __ldg(reinterpret_cast<const float4*>(accm + coff));
+        o.x = o.x * m.x; o.y = o.y * m.y; o.z = o.z * m.z; o.w = o.w * m.w;
+    }
+    float* dst = div + coff;
     const int nvalid = g.n[0] - x0;
     if (nvalid >= 4) *reinterpret_cast<float4*>(dst) = o;
     else for (int j = 0; j < nvalid; ++j) dst[j] = f4_get(o, j);
 }
 
-int phi_launch_divergence_vec(const DGrid& g, const DVec& v, const DField& cf, float* div, cudaStream_t s)
+int phi_launch_divergence_vec(const DGrid& g, const DVec& v, const DField& cf, float* div, const float* acc, cudaStream_t s)
 {
     dim3 grid((g.fext[0] / 4 + 31) / 32, (g.fext[1] + FK_WARPS - 1) / FK_WARPS, g.fext[2] * g.batch);
-    if (g.dim == 3) k_div_vec<3><<<grid, FK_THREADS, 0, s>>>(g, v, cf, div);
-    else            k_div_vec<2><<<grid, FK_THREADS, 0, s>>>(g, v, cf, div);
+    if (g.dim == 3) {
+        if (acc) k_div_vec<3, true><<<grid, FK_THREADS, 0, s>>>(g, v, cf, div, acc);
+        else     k_div_vec<3, false><<<grid, FK_THREADS, 0, s>>>(g, v, cf, div, nullptr);
+    } else {
+        if (acc) k_div_vec<2, true><<<grid, FK_THREADS, 0, s>>>(g, v, cf, div, acc);
+        else     k_div_vec<2, false><<<grid, FK_THREADS, 0, s>>>(g, v, cf, div, nullptr);
+    }
     return (int)cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------------------
 // A6  v_d[f] = vin_d[f] - (p[upper(f)] - p[lower(f)]) / dx_d on the stored faces       28 B/cell (3-D), 20 (2-D)
 // Out of place (vout may equal vin): the fused step writes the projected velocity straight back into the caller's arrays.
+// MASK (N4): the gradient is scaled by hard_bcs = min(acc[upper cell], acc[lower cell]) as k_grad_sub does with a mask, the
+// accessibility ghosts from af (fluid._accessible_extrapolation); the acc lines are resolved and loaded like the p lines.
 // ---------------------------------------------------------------------------------------------------------
-template <int DIM>
+template <int DIM, bool MASK>
 __global__ void __launch_bounds__(FK_THREADS)
 k_gradsub_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec vin, const __grid_constant__ DVecOut vout,
-              const __grid_constant__ DField pf, const float* __restrict__ p)
+              const __grid_constant__ DField pf, const float* __restrict__ p, const __grid_constant__ DField af, const float* __restrict__ accm)
 {
     const FkLine L = fk_line4<DIM>(g);
     if (!L.ok || (DIM == 3 && (L.z < 0 || L.z >= g.fext[2] - 2 * g.halo))) return;
@@ -157,6 +171,16 @@ k_gradsub_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec vin,
     if (in_line) pc = fk_ld4(p, r0, pf, x0);
     float pl = __shfl_up_sync(0xffffffffu, pc.w, 1);                         // p[x0 - 1]
     if (in_line && (lane == 0 || x0 == 0)) pl = fk_ldx(p, r0, pf, x0 - 1);
+    // MASK: the same for the accessibility (centred like p: an interior line has p's offset)
+    RowRef<3> ra0 = r0;
+    float4 ac = f4_splat(1.f);
+    float al = 1.f;
+    if (MASK) {
+        if (!interior) ra0 = fk_row<DIM>(g, af, L.b, L.y, L.z);
+        if (in_line) ac = fk_ld4(accm, ra0, af, x0);
+        al = __shfl_up_sync(0xffffffffu, ac.w, 1);
+        if (in_line && (lane == 0 || x0 == 0)) al = fk_ldx(accm, ra0, af, x0 - 1);
+    }
     if (!in_line) return;
     const long long off = (long long)L.b * vin.f[0].sb + (long long)L.z * vin.f[0].sz + (long long)L.y * vin.f[0].sy + x0;
     const float dx = g.dx[0], dy = g.dx[1], dz = g.dx[2], ix = g.inv_dx[0], iy = g.inv_dx[1], iz = g.inv_dx[2];
@@ -165,8 +189,13 @@ k_gradsub_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec vin,
         const DField& f = vin.f[0];
         if (yz_c && x0 <= f.hi[0] && x0 + 3 >= f.lo[0]) {
             float4 a = *reinterpret_cast<const float4*>(vin.p[0] + off);
-            a.x -= phi_div(pc.x - pl, dx, ix); a.y -= phi_div(pc.y - pc.x, dx, ix);
-            a.z -= phi_div(pc.z - pc.y, dx, ix); a.w -= phi_div(pc.w - pc.z, dx, ix);
+            if (MASK) {     // separate multiply and subtract, as k_grad_sub rounds them
+                a.x -= __fmul_rn(phi_div(pc.x - pl, dx, ix), fminf(ac.x, al)); a.y -= __fmul_rn(phi_div(pc.y - pc.x, dx, ix), fminf(ac.y, ac.x));
+                a.z -= __fmul_rn(phi_div(pc.z - pc.y, dx, ix), fminf(ac.z, ac.y)); a.w -= __fmul_rn(phi_div(pc.w - pc.z, dx, ix), fminf(ac.w, ac.z));
+            } else {
+                a.x -= phi_div(pc.x - pl, dx, ix); a.y -= phi_div(pc.y - pc.x, dx, ix);
+                a.z -= phi_div(pc.z - pc.y, dx, ix); a.w -= phi_div(pc.w - pc.z, dx, ix);
+            }
             if (x0 >= f.lo[0] && x0 + 3 <= f.hi[0]) *reinterpret_cast<float4*>(vout.p[0] + off) = a;
             else for (int j = 0; j < 4; ++j) if (x0 + j >= f.lo[0] && x0 + j <= f.hi[0]) vout.p[0][off + j] = f4_get(a, j);
         }
@@ -180,8 +209,16 @@ k_gradsub_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec vin,
             if (interior) rm.off = r0.off - pf.sy; else rm = fk_row<DIM>(g, pf, L.b, L.y - 1, L.z);
             const float4 pm = fk_ld4(p, rm, pf, x0);
             float4 a = *reinterpret_cast<const float4*>(vin.p[1] + off);
-            a.x -= phi_div(pc.x - pm.x, dy, iy); a.y -= phi_div(pc.y - pm.y, dy, iy);
-            a.z -= phi_div(pc.z - pm.z, dy, iy); a.w -= phi_div(pc.w - pm.w, dy, iy);
+            if (MASK) {
+                RowRef<3> ram = ra0;
+                if (interior) ram.off = ra0.off - af.sy; else ram = fk_row<DIM>(g, af, L.b, L.y - 1, L.z);
+                const float4 am = fk_ld4(accm, ram, af, x0);
+                a.x -= __fmul_rn(phi_div(pc.x - pm.x, dy, iy), fminf(ac.x, am.x)); a.y -= __fmul_rn(phi_div(pc.y - pm.y, dy, iy), fminf(ac.y, am.y));
+                a.z -= __fmul_rn(phi_div(pc.z - pm.z, dy, iy), fminf(ac.z, am.z)); a.w -= __fmul_rn(phi_div(pc.w - pm.w, dy, iy), fminf(ac.w, am.w));
+            } else {
+                a.x -= phi_div(pc.x - pm.x, dy, iy); a.y -= phi_div(pc.y - pm.y, dy, iy);
+                a.z -= phi_div(pc.z - pm.z, dy, iy); a.w -= phi_div(pc.w - pm.w, dy, iy);
+            }
             if (nvx >= 4) *reinterpret_cast<float4*>(vout.p[1] + off) = a;
             else for (int j = 0; j < nvx; ++j) vout.p[1][off + j] = f4_get(a, j);
         }
@@ -193,19 +230,34 @@ k_gradsub_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec vin,
             if (interior) rm.off = r0.off - pf.sz; else rm = fk_row<DIM>(g, pf, L.b, L.y, L.z - 1);
             const float4 pm = fk_ld4(p, rm, pf, x0);
             float4 a = *reinterpret_cast<const float4*>(vin.p[2] + off);
-            a.x -= phi_div(pc.x - pm.x, dz, iz); a.y -= phi_div(pc.y - pm.y, dz, iz);
-            a.z -= phi_div(pc.z - pm.z, dz, iz); a.w -= phi_div(pc.w - pm.w, dz, iz);
+            if (MASK) {
+                RowRef<3> ram = ra0;
+                if (interior) ram.off = ra0.off - af.sz; else ram = fk_row<DIM>(g, af, L.b, L.y, L.z - 1);
+                const float4 am = fk_ld4(accm, ram, af, x0);
+                a.x -= __fmul_rn(phi_div(pc.x - pm.x, dz, iz), fminf(ac.x, am.x)); a.y -= __fmul_rn(phi_div(pc.y - pm.y, dz, iz), fminf(ac.y, am.y));
+                a.z -= __fmul_rn(phi_div(pc.z - pm.z, dz, iz), fminf(ac.z, am.z)); a.w -= __fmul_rn(phi_div(pc.w - pm.w, dz, iz), fminf(ac.w, am.w));
+            } else {
+                a.x -= phi_div(pc.x - pm.x, dz, iz); a.y -= phi_div(pc.y - pm.y, dz, iz);
+                a.z -= phi_div(pc.z - pm.z, dz, iz); a.w -= phi_div(pc.w - pm.w, dz, iz);
+            }
             if (nvx >= 4) *reinterpret_cast<float4*>(vout.p[2] + off) = a;
             else for (int j = 0; j < nvx; ++j) vout.p[2][off + j] = f4_get(a, j);
         }
     }
 }
 
-int phi_launch_grad_sub_vec(const DGrid& g, const DVec& vin, const DVecOut& vout, const DField& pf, const float* p, cudaStream_t s)
+int phi_launch_grad_sub_vec(const DGrid& g, const DVec& vin, const DVecOut& vout, const DField& pf, const float* p,
+                            const DField* af, const float* acc, cudaStream_t s)
 {
     dim3 grid((g.fext[0] / 4 + 31) / 32, (g.fext[1] + FK_WARPS - 1) / FK_WARPS, g.fext[2] * g.batch);
-    if (g.dim == 3) k_gradsub_vec<3><<<grid, FK_THREADS, 0, s>>>(g, vin, vout, pf, p);
-    else            k_gradsub_vec<2><<<grid, FK_THREADS, 0, s>>>(g, vin, vout, pf, p);
+    const DField a = af ? *af : pf;
+    if (g.dim == 3) {
+        if (acc) k_gradsub_vec<3, true><<<grid, FK_THREADS, 0, s>>>(g, vin, vout, pf, p, a, acc);
+        else     k_gradsub_vec<3, false><<<grid, FK_THREADS, 0, s>>>(g, vin, vout, pf, p, a, nullptr);
+    } else {
+        if (acc) k_gradsub_vec<2, true><<<grid, FK_THREADS, 0, s>>>(g, vin, vout, pf, p, a, acc);
+        else     k_gradsub_vec<2, false><<<grid, FK_THREADS, 0, s>>>(g, vin, vout, pf, p, a, nullptr);
+    }
     return (int)cudaGetLastError();
 }
 
@@ -459,14 +511,16 @@ k_advect_centered_vec(const __grid_constant__ DGrid g, const __grid_constant__ D
     }
 }
 
-// Staggered field, all components in one launch: dst_c = interp(src_c, face_c - dt v(face_c)) [+ dt * buoyancy_c]
+// Staggered field, all components in one launch: dst_c = interp(src_c, face_c - dt v(face_c)) [+ dt * buoyancy_c] [* f_c]
 //   buoyancy_c = (s * b_c)[upper cell] * 0.5 + (s * b_c)[lower cell] * 0.5      (sample_grid_at_faces; a constant ghost of s
 //   stays c: the product keeps the boundary of s, phi/field/_field.py:809)
-template <int DIM, bool BUOY>
+//   f_c (FACES, N4): face factors of stationary obstacles, 1 - resample(geometry, v, soft=True, balance=1) = apply_boundary_conditions
+//   (phi/physics/fluid.py:212-240).  A separate rounded product after the stored-value arithmetic, as k_mul_faces forms it.
+template <int DIM, bool BUOY, bool FACES>
 __global__ void __launch_bounds__(FK_THREADS, 4)
 k_advect_staggered_vec(const __grid_constant__ DGrid g, const __grid_constant__ DVec vel, const __grid_constant__ DVec fld,
                        const __grid_constant__ DVecOut dst, float dt, const __grid_constant__ DField sf, const float* __restrict__ s,
-                       float b0, float b1, float b2)
+                       float b0, float b1, float b2, const float* __restrict__ f0, const float* __restrict__ f1, const float* __restrict__ f2)
 {
     const FkAdvLine L = fk_adv_line<DIM>(g);
     if (!L.ok) return;
@@ -596,6 +650,11 @@ k_advect_staggered_vec(const __grid_constant__ DGrid g, const __grid_constant__ 
                 if (c == 0) r0 = r; else if (c == 1) r1 = r; else r2 = r;
             }
         }
+        if (FACES) {
+            if (st0) r0 = __fmul_rn(r0, __ldg(f0 + line + x));
+            if (st1) r1 = __fmul_rn(r1, __ldg(f1 + line + x));
+            if (DIM == 3 && st2) r2 = __fmul_rn(r2, __ldg(f2 + line + x));
+        }
         if (st0) dst.p[0][line + x] = r0;
         if (st1) dst.p[1][line + x] = r1;
         if (DIM == 3 && st2) dst.p[2][line + x] = r2;
@@ -623,7 +682,7 @@ int phi_launch_advect_centered_vec(const DGrid& g, const DVec& vel, const DField
 }
 
 int phi_launch_advect_staggered_vec(const DGrid& g, const DVec& vel, const DVec& fld, const DVecOut& dst, float dt,
-                                    const DField* sf, const float* sarr, const float bu[3], cudaStream_t s)
+                                    const DField* sf, const float* sarr, const float bu[3], const float* const* faces, cudaStream_t s)
 {
     if (!fits_int32(g)) return -100;
     const DField sfv = sf ? *sf : fld.f[0];
@@ -632,13 +691,18 @@ int phi_launch_advect_staggered_vec(const DGrid& g, const DVec& vel, const DVec&
         const_side = const_side || (sfv.klo[a] == PHI_BC_CONST && sfv.clo[a] != 0.f) || (sfv.khi[a] == PHI_BC_CONST && sfv.chi[a] != 0.f);
     const bool buoy = sarr != nullptr && bu && (bu[0] != 0.f || bu[1] != 0.f || (g.dim == 3 && bu[2] != 0.f) || const_side);
     const float b0 = buoy ? bu[0] : 0.f, b1 = buoy ? bu[1] : 0.f, b2 = (buoy && g.dim == 3) ? bu[2] : 0.f;
+    const float* f0 = faces ? faces[0] : nullptr;
+    const float* f1 = faces ? faces[1] : nullptr;
+    const float* f2 = faces && g.dim == 3 ? faces[2] : nullptr;
+#define FK_ADV_STAG(D, B, F) k_advect_staggered_vec<D, B, F><<<adv_grid(g), FK_THREADS, 0, s>>>(g, vel, fld, dst, dt, sfv, sarr, b0, b1, b2, f0, f1, f2)
     if (g.dim == 3) {
-        if (buoy) k_advect_staggered_vec<3, true><<<adv_grid(g), FK_THREADS, 0, s>>>(g, vel, fld, dst, dt, sfv, sarr, b0, b1, b2);
-        else      k_advect_staggered_vec<3, false><<<adv_grid(g), FK_THREADS, 0, s>>>(g, vel, fld, dst, dt, sfv, sarr, b0, b1, b2);
+        if (faces) { if (buoy) FK_ADV_STAG(3, true, true); else FK_ADV_STAG(3, false, true); }
+        else       { if (buoy) FK_ADV_STAG(3, true, false); else FK_ADV_STAG(3, false, false); }
     } else {
-        if (buoy) k_advect_staggered_vec<2, true><<<adv_grid(g), FK_THREADS, 0, s>>>(g, vel, fld, dst, dt, sfv, sarr, b0, b1, b2);
-        else      k_advect_staggered_vec<2, false><<<adv_grid(g), FK_THREADS, 0, s>>>(g, vel, fld, dst, dt, sfv, sarr, b0, b1, b2);
+        if (faces) { if (buoy) FK_ADV_STAG(2, true, true); else FK_ADV_STAG(2, false, true); }
+        else       { if (buoy) FK_ADV_STAG(2, true, false); else FK_ADV_STAG(2, false, false); }
     }
+#undef FK_ADV_STAG
     return (int)cudaGetLastError();
 }
 

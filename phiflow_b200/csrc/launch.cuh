@@ -18,13 +18,14 @@ int phi_launch_advect(const DGrid& g, const DVec& vel, const DField& ff, int tar
 int phi_launch_mac_cormack(const DGrid& g, const DVec& vel, const DField& ff, const float* src, float* dst, float* tmp,
                            float dt, float strength, cudaStream_t s);
 
-// vectorised / fused variants (fused_kernels.cu); no obstacle masks
-int phi_launch_divergence_vec(const DGrid& g, const DVec& v, const DField& cf, float* div, cudaStream_t s);
-int phi_launch_grad_sub_vec(const DGrid& g, const DVec& vin, const DVecOut& vout, const DField& pf, const float* p, cudaStream_t s);
+// vectorised / fused variants (fused_kernels.cu); acc / af / faces: static obstacle masks (N4), nullptr = none
+int phi_launch_divergence_vec(const DGrid& g, const DVec& v, const DField& cf, float* div, const float* acc, cudaStream_t s);
+int phi_launch_grad_sub_vec(const DGrid& g, const DVec& vin, const DVecOut& vout, const DField& pf, const float* p,
+                            const DField* af, const float* acc, cudaStream_t s);
 int phi_launch_advect_centered_vec(const DGrid& g, const DVec& vel, const DField& ff, const float* src, float* dst, float dt,
                                    const float* add, float add_scale, cudaStream_t s);
 int phi_launch_advect_staggered_vec(const DGrid& g, const DVec& vel, const DVec& fld, const DVecOut& dst, float dt,
-                                    const DField* sf, const float* sarr, const float bu[3], cudaStream_t s);
+                                    const DField* sf, const float* sarr, const float bu[3], const float* const* faces, cudaStream_t s);
 int phi_launch_grid_sample(const DGrid& g, const DField& f, const float* grid, const float* coords, long long npoints, float* out, cudaStream_t s);
 // CenteredGrid (collocated) velocities, wide stencil (collocated_kernels.cu)
 size_t phi_collocated_workspace_bytes(const DGrid& g);

@@ -205,6 +205,11 @@ class Union:
             ok |= g.lies_inside(pts)
         return ok
 
+    def signed_distance(self, pts):
+        """Union.approximate_signed_distance (phi/geom/_geom_ops.py:100-102): the minimum over the members, so a union obstacle's face
+        factors are 1 - max of the members' fractions (Fluid_Logo.ipynb's eight touching boxes), not the product of separate obstacles."""
+        return np.minimum.reduce([g.signed_distance(pts) for g in self.geometries]).astype(np.float32)
+
 
 def union(*geometries):
     """geom.union (phi/geom/_geom_ops.py:297-320): union(Box(x=(0, 10), y=(2, 3)), Box(x=(4.5, 5.5), y=(1, 4))) as Heat_Flow.ipynb builds its
@@ -776,8 +781,8 @@ def _obstacle_masks(velocity: StaggeredGrid, obstacles):
     """Static obstacles (phi/physics/fluid.py:130-137, 212-240): returns (accessible centred mask, per-component face factors
     1 - resample(geometry, velocity, soft=True, balance=1)).  Geometry sampling is set-up work done on the host."""
     geoms = list(obstacles) if isinstance(obstacles, (tuple, list)) else [obstacles]
-    _require(all(isinstance(o, (Box, Sphere, InfiniteCylinder)) for o in geoms),
-             "obstacles other than stationary Box / Sphere / infinite_cylinder geometries")
+    _require(all(isinstance(o, (Box, Sphere, InfiniteCylinder, Union)) for o in geoms),
+             "obstacles other than stationary Box / Sphere / infinite_cylinder / union geometries")
     centred = CenteredGrid(0, ZERO, velocity.bounds, velocity.batch, **dict(zip(velocity.axes, velocity.res)))
     pts = centred.points()
     inside = np.zeros(pts.shape[:-1], bool)
@@ -795,6 +800,36 @@ def _obstacle_masks(velocity: StaggeredGrid, obstacles):
     return accessible, velocity.dom.faces_from_numpy(factors, velocity.vspec)
 
 
+def _geometry_key(o):
+    """The parameters that decide a stationary geometry's masks (hashable)."""
+    if isinstance(o, Box):
+        return ('box', o.names, tuple(o.lower[k] for k in o.names), tuple(o.upper[k] for k in o.names))
+    if isinstance(o, Sphere):
+        return ('sphere', o.names, o.center, o.radius)
+    if isinstance(o, InfiniteCylinder):
+        return ('cylinder', _geometry_key(o.sphere), o.inf_dim)
+    if isinstance(o, Union):
+        return ('union',) + tuple(_geometry_key(g) for g in o.geometries)
+    _require(False, "obstacles other than stationary Box / Sphere / infinite_cylinder / union geometries")
+
+
+_MASKS = {}
+_MASKS_KEPT = 8
+
+
+def _obstacle_masks_cached(velocity: StaggeredGrid, obstacles):
+    """_obstacle_masks memoised on the geometry parameters and the grid (resolution, bounds, batch, boundary, device): a step loop and
+    make_incompressible with the same stationary obstacle rasterise it on the host once.  The masks are read-only device tensors."""
+    geoms = list(obstacles) if isinstance(obstacles, (tuple, list)) else [obstacles]
+    key = (tuple(_geometry_key(o) for o in geoms), velocity.res, velocity.lower, velocity.upper, velocity.batch, velocity.boundary,
+           str(velocity.dom.device))
+    if key not in _MASKS:
+        if len(_MASKS) >= _MASKS_KEPT:
+            del _MASKS[next(iter(_MASKS))]
+        _MASKS[key] = _obstacle_masks(velocity, obstacles)
+    return _MASKS[key]
+
+
 def make_incompressible(velocity: StaggeredGrid, obstacles=(), solve: Solve = None, active=None, order=2):
     """fluid.make_incompressible (phi/physics/fluid.py:94-162): returns (divergence-free velocity, pressure).
     obstacles: stationary Box / Sphere / infinite_cylinder geometries (row N4)."""
@@ -804,7 +839,7 @@ def make_incompressible(velocity: StaggeredGrid, obstacles=(), solve: Solve = No
     if solve.x0 is not None:
         _require(isinstance(solve.x0, CenteredGrid) and solve.x0.res == velocity.res and solve.x0.batch == velocity.batch, "x0 on a different grid")
     if obstacles:
-        accessible, factors = _obstacle_masks(velocity, obstacles)
+        accessible, factors = _obstacle_masks_cached(velocity, obstacles)
         res = dict(zip(velocity.axes, velocity.res))
         p_data = solve.x0.data.clone() if solve.x0 is not None else velocity.dom.alloc_centered()
         v_data = [c.clone() for c in velocity.data]
@@ -826,19 +861,25 @@ def make_incompressible(velocity: StaggeredGrid, obstacles=(), solve: Solve = No
 
 
 def incompressible_step(v: StaggeredGrid, s: CenteredGrid, p, dt: float, inflow: CenteredGrid = None, inflow_rate: float = 0.0,
-                        buoyancy=(0, 0.1), solve: Solve = None, smoke_advection='semi_lagrangian'):
+                        buoyancy=(0, 0.1), solve: Solve = None, smoke_advection='semi_lagrangian', obstacles=()):
     """The notebook step (examples/grids/Smoke_Plume.ipynb:58-68) as ONE library call:
         s = advect(s, v, dt) + inflow_rate * inflow ;  v = semi_lagrangian(v, v, dt) + resample(s * buoyancy, to=v) * dt ;
-        v, p = make_incompressible(v, (), Solve('CG', ..., x0=p))
+        v, p = make_incompressible(v, obstacles, Solve('CG', ..., x0=p))
+    obstacles: the stationary geometries make_incompressible takes (Box, Sphere, infinite_cylinder, union; Batched_Smoke.ipynb,
+    Fluid_Logo.ipynb); their masks are rasterised once per geometry and grid.
     Returns new (v, s, p); inputs are not modified."""
     solve = solve or Solve('CG', 1e-3)
     _check_velocity(s, v)
+    kw = {}
+    if obstacles:
+        kw['accessible'], kw['factors'] = _obstacle_masks_cached(v, obstacles)
+    prm = _cg_params(v, solve)
     v_data = [c.clone() for c in v.data]
     s_data = s.data.clone()
     p_data = p.data.clone() if p is not None else v.dom.alloc_centered()
     infl = inflow.data if inflow is not None else None
     ops.plume_step(v.dom, v.vspec, s.spec, v_data, s_data, p_data, infl, float(dt), float(inflow_rate), tuple(buoyancy),
-                   _cg_params(v, solve), mac_cormack=(smoke_advection == 'mac_cormack'))
+                   prm, mac_cormack=(smoke_advection == 'mac_cormack'), **kw)
     _finish_solve(v.dom, solve)
     pressure = CenteredGrid(boundary=_pressure_boundary(v.boundary), bounds=v.bounds, batch=v.batch, _data=p_data, **dict(zip(v.axes, v.res)))
     return v.with_values(v_data), s.with_values(s_data), pressure
