@@ -951,72 +951,85 @@ __device__ __forceinline__ void ring_unit_cells(const RingCfg& cfg, const DGrid&
 // iteration: d_k, d_{k-1} read, d_{k+1} written (12 B/cell) + x += alpha_{k-1} d_{k-1} + alpha_k d_k every second iteration, with
 // d_{k-1} already staged (8 B/cell) = 16 B/cell, against 30 for the two sweeps of k_cg_ring.
 // Stage layout: d_k (TY+4 lines: halo 2 in y, because d_{k+1} is needed on the halo lines), d_{k-1} (TY+2 lines, not fetched in
-// iteration 0), x (TY lines, fetched on x-update iterations only).  d_{k+1} of each plane goes to a triple-buffered shared tile
-// (TY+2 lines) from which the q_{k+1} stencil takes its y and warp-edge x neighbours; consumers sync on a named barrier once per plane.
+// iteration 0).  x has no halo and is read only on owned cells of every second iteration, so it does not travel through the ring:
+// consumers load it from global memory one plane ahead.  d_{k+1} of each plane goes to a triple-buffered shared tile (TY+2 lines)
+// from which the q_{k+1} stencil takes its y and warp-edge x neighbours; consumers sync on a named barrier once per plane.
 // Only for 3-D, the branch-free tiling, periodic y and z, one GPU, CG without matrix offset or obstacles (phi_launch_cg_ring).
-#define RING_GF 3                // consumer groups per thread on the haloed (TY+2)-line region: (TY + 2) * nx4 <= RING_GF * 256
+#define FUSED_GI 2               // owned groups per consumer thread: TY * nx4 <= FUSED_GI * consumers
+#define FUSED_GH 2               // groups per consumer thread on the two halo lines: 2 * nx4 <= FUSED_GH * consumers
 #define FUSED_TILE_BUFS 3
 
+// A thread's groups come in two kinds with fixed register slots: owned groups (lines 1 .. TY of the d_{k+1} tile) carry d_k, d_{k+1}
+// and r_{k+1} from plane to plane, halo groups (lines 0 and TY+1) only d_k.  Group k of a kind is group threadIdx.x + k * consumers
+// of that kind's lines; with nx4 % 32 == 0 (shfl_ok) every warp's 32 groups lie on one line, so validity is warp-uniform, and
+// lane 0 / lane 31 are the only lanes whose x-1 / x+4 neighbour is not a shuffle away.
 struct FusedGroups {
-    int t[RING_GF];             // (jj * pitch + x0): offset in the d_{k+1} tile of line jj = j + 1 (j = -1 .. TY); in the d stage + pitch
-    int tl[RING_GF], tr[RING_GF];   // tile offsets of the x-1 / x+4 neighbours of the groups that cannot take them from a shuffle
-    int goff[RING_GF];          // (jj - 1) * sy + x0: element offset of an owned (inner) group relative to (y0, x = 0) of the plane
-    unsigned valid, inner, needl, needr;    // bit k; valid and inner are warp-uniform
+    int ti[FUSED_GI], th[FUSED_GH];   // jj * pitch + x0: offset in the d_{k+1} tile (line jj); in the d stage + pitch
+    int ei[FUSED_GI], eh[FUSED_GH];   // tile offset of the x neighbour lane 0 (x-1) or lane 31 (x+4) reads; other lanes 0 (broadcast)
+    int gi[FUSED_GI];                       // (jj - 1) * sy + x0: element offset of an owned group relative to (y0, x = 0) of the plane
+    unsigned vi, vh;                  // bit k: owned / halo group k exists (warp-uniform)
 };
 
 __device__ __forceinline__ void fused_groups_init(FusedGroups& fg, const RingCfg& cfg, const DGrid& g, const DField& pf)
 {
-    const int lane = threadIdx.x & 31, nx = g.n[0], pitch = cfg.pitch;
-    fg.valid = fg.inner = fg.needl = fg.needr = 0;
-#pragma unroll
-    for (int k = 0; k < RING_GF; ++k) {
-        const int ge = threadIdx.x + k * cfg.consumers;
-        const int jj = ge / cfg.nx4, x0 = (ge - jj * cfg.nx4) * 4;
+    const int lane = threadIdx.x & 31, nx = g.n[0], pitch = cfg.pitch, nx4 = cfg.nx4;
+    // tile offset of the x neighbour this lane reads for the group at line jj, x0 (lane 0: x-1, lane 31: x+4, ghosts resolved)
+    auto edge = [&](int jj, int x0) -> int {
         const int row = jj * pitch;
-        if (jj < cfg.TY + 2) fg.valid |= 1u << k;
-        if (jj >= 1 && jj <= cfg.TY) fg.inner |= 1u << k;
-        fg.t[k] = row + x0;
-        fg.goff[k] = (jj - 1) * (int)pf.sy + x0;
-        fg.tl[k] = row + x0 - 1; fg.tr[k] = row + x0 + 4;
-        if (lane == 0) fg.needl |= 1u << k;
-        if (lane == 31) fg.needr |= 1u << k;
-        if (x0 == 0) { fg.needl |= 1u << k; fg.tl[k] = pf.klo[0] == PHI_BC_PERIODIC ? row + nx - 1 : row; }
-        if (x0 + 4 >= nx) { fg.needr |= 1u << k; fg.tr[k] = pf.khi[0] == PHI_BC_PERIODIC ? row : row + nx - 1; }
-        if (!(fg.needl & (1u << k))) fg.tl[k] = 0;          // broadcast address: every lane loads, the shuffled value wins
-        if (!(fg.needr & (1u << k))) fg.tr[k] = 0;
+        if (lane == 0) return x0 == 0 ? (pf.klo[0] == PHI_BC_PERIODIC ? row + nx - 1 : row) : row + x0 - 1;
+        if (lane == 31) return x0 + 4 >= nx ? (pf.khi[0] == PHI_BC_PERIODIC ? row : row + nx - 1) : row + x0 + 4;
+        return 0;
+    };
+    fg.vi = fg.vh = 0;
+#pragma unroll
+    for (int k = 0; k < FUSED_GI; ++k) {
+        const int ge = threadIdx.x + k * cfg.consumers;
+        const int j = ge / nx4, x0 = (ge - j * nx4) * 4;
+        if (j < cfg.TY) fg.vi |= 1u << k;
+        fg.ti[k] = (j + 1) * pitch + x0;
+        fg.ei[k] = edge(j + 1, x0);
+        fg.gi[k] = j * (int)pf.sy + x0;
+    }
+#pragma unroll
+    for (int k = 0; k < FUSED_GH; ++k) {
+        const int ge = threadIdx.x + k * cfg.consumers;
+        const int h = ge / nx4, x0 = (ge - h * nx4) * 4;
+        const int jj = h == 0 ? 0 : cfg.TY + 1;
+        if (h < 2) fg.vh |= 1u << k;
+        fg.th[k] = jj * pitch + x0;
+        fg.eh[k] = edge(jj, x0);
     }
 }
 
-// Producer of pass F.  Staged line slots: d_k (TY+4 lines from y0-2), d_{k-1} (TY+2 from y0-1), x (TY).  Category 0 (d_k) is fetched
-// on every plane of the unit, 1 (d_{k-1}) on planes z0-1 .. z1, 2 (x) on the owned planes of x-update iterations.  A null source
-// (d_{k-1} in iteration 0, x on other iterations) is not fetched.
+// Producer of pass F.  Staged line slots: d_k (TY+4 lines from y0-2), d_{k-1} (TY+2 from y0-1).  Category 0 (d_k) is fetched on every
+// plane of the unit, 1 (d_{k-1}) on planes z0-1 .. z1.  A null source (d_{k-1} in iteration 0) is not fetched.
 struct ProdUnitF {
     long long yoff[4];
     const float* base[4];
     uint32_t dsto[4];
     uint32_t nbytes[4];
-    unsigned m[3];
-    int tot[3];
+    unsigned m[2];
+    int tot[2];
 };
 
 __device__ __forceinline__ void prod_fused_setup(ProdUnitF& pu, const RingCfg& cfg, const DGrid& g, const DField& pf,
-                                                 const float* d, const float* dprev, const float* x, int b, int y0)
+                                                 const float* d, const float* dprev, int b, int y0)
 {
     const int lane = threadIdx.x & 31, TY = cfg.TY;
     const uint32_t row_bytes = (uint32_t)cfg.pitch * 4u;
     const bool mergeable = cfg.merge && pf.sy == cfg.pitch;
-    const int rows[3] = {TY + 4, TY + 2, TY};
-    const int ylo[3] = {y0 - 2, y0 - 1, y0};
-    const float* src[3] = {d, dprev, x};
-    int cnt[3] = {0, 0, 0};
-    pu.m[0] = pu.m[1] = pu.m[2] = 0;
+    const int rows[2] = {TY + 4, TY + 2};
+    const int ylo[2] = {y0 - 2, y0 - 1};
+    const float* src[2] = {d, dprev};
+    int cnt[2] = {0, 0};
+    pu.m[0] = pu.m[1] = 0;
 #pragma unroll
     for (int it = 0; it < 4; ++it) {
         const int line = lane + 32 * it;
         pu.yoff[it] = 0; pu.base[it] = nullptr; pu.dsto[it] = 0; pu.nbytes[it] = row_bytes;
         int key = -1, yv = 0, first = 0;
 #pragma unroll
-        for (int arr = 0; arr < 3; ++arr) {
+        for (int arr = 0; arr < 2; ++arr) {
             if (key < 0 && line >= first && line < first + rows[arr] && src[arr]) {
                 int yy = ylo[arr] + (line - first); float cv;
                 phi_resolve(yy, pf, 1, cv);                         // periodic in y: always a stored line
@@ -1027,25 +1040,25 @@ __device__ __forceinline__ void prod_fused_setup(ProdUnitF& pu, const RingCfg& c
             }
             first += rows[arr];
         }
-        cnt[0] += key == 0; cnt[1] += key == 1; cnt[2] += key == 2;       // categories: d_k, d_{k-1}, x
+        cnt[0] += key == 0; cnt[1] += key == 1;                     // categories: d_k, d_{k-1}
         const int pkey = __shfl_up_sync(0xffffffffu, key, 1), pyv = __shfl_up_sync(0xffffffffu, yv, 1);
         const bool cont = mergeable && key >= 0 && lane > 0 && pkey == key && pyv + 1 == yv;
         const unsigned cm = __ballot_sync(0xffffffffu, cont);
         if (key >= 0 && !cont) {
             const unsigned follow = lane == 31 ? 0u : (cm >> (lane + 1));
             pu.nbytes[it] = (uint32_t)__ffs(~follow) * row_bytes;
-            if (key == 0) pu.m[0] |= 1u << it; else if (key == 1) pu.m[1] |= 1u << it; else pu.m[2] |= 1u << it;
+            pu.m[key] |= 1u << it;
         }
     }
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
+    for (int c = 0; c < 2; ++c) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) cnt[c] += __shfl_xor_sync(0xffffffffu, cnt[c], o);
         pu.tot[c] = cnt[c];
     }
 }
 
-__device__ __forceinline__ void ring_produce_fused(Ring& rg, const RingCfg& cfg, const DField& pf, const ProdUnitF& pu, int z, bool pplane, bool eplane)
+__device__ __forceinline__ void ring_produce_fused(Ring& rg, const RingCfg& cfg, const DField& pf, const ProdUnitF& pu, int z, bool pplane)
 {
     const int lane = threadIdx.x & 31;
     const int slot = rg.pos.slot;
@@ -1054,8 +1067,8 @@ __device__ __forceinline__ void ring_produce_fused(Ring& rg, const RingCfg& cfg,
     float cv;
     phi_resolve(z, pf, 2, cv);                                      // periodic in z
     const long long zoff = (long long)z * pf.sz;
-    const unsigned mask = pu.m[0] | (pplane ? pu.m[1] : 0u) | (eplane ? pu.m[2] : 0u);
-    const int cnt = pu.tot[0] + (pplane ? pu.tot[1] : 0) + (eplane ? pu.tot[2] : 0);
+    const unsigned mask = pu.m[0] | (pplane ? pu.m[1] : 0u);
+    const int cnt = pu.tot[0] + (pplane ? pu.tot[1] : 0);
     if (lane == 0) {
         mbar_wait(rg.empty0 + 8 * slot, rg.pos.par ^ 1u);
         mbar_expect_tx(full, (uint32_t)cnt * (uint32_t)cfg.pitch * 4u);
@@ -1100,33 +1113,59 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
     const int nz = u.z1 - u.z0;
     if ((int)threadIdx.x >= cfg.consumers) {
         ProdUnitF pu;
-        prod_fused_setup(pu, cfg, g, pf, P.d, P.dprev, P.x, u.b, u.y0);
+        prod_fused_setup(pu, cfg, g, pf, P.d, P.dprev, u.b, u.y0);
         for (int p = 0; p < nz + 4; ++p)
-            ring_produce_fused(rg, cfg, pf, pu, u.z0 - 2 + p, p >= 1 && p <= nz + 2, P.x && p >= 2 && p <= nz + 1);
+            ring_produce_fused(rg, cfg, pf, pu, u.z0 - 2 + p, p >= 1 && p <= nz + 2);
         return;
     }
     const int pitch = cfg.pitch, TY = cfg.TY;
-    const int pb = (TY + 4) * pitch, xb = (2 * TY + 6) * pitch - pitch;
+    const int pb = (TY + 4) * pitch;
     const int tsz = (TY + 2) * pitch;
+    const int lane = threadIdx.x & 31;
     const float ix2 = g.inv_dx2[0], iy2 = g.inv_dx2[1], iz2 = g.inv_dx2[2];
     const float cc = 2.f * (ix2 + iy2 + iz2);
     const float alpha = P.alpha, aprev = P.aprev, beta = P.beta, bprev = P.bprev;
     const bool has_prev = P.dprev != nullptr;
     long long plane_off = (long long)u.b * pf.sb + (long long)u.y0 * pf.sy + (long long)u.z0 * pf.sz - pf.sz;   // plane z0 - 1
 
-    float4 dm[RING_GF], dc[RING_GF];             // d_k on planes p-1, p (own cells of the haloed region)
-    float4 n2[RING_GF], n1[RING_GF];             // d_{k+1} on planes p-2, p-1
-    float4 r1[RING_GF];                          // r_{k+1} on plane p-1
+    // d_{k+1} of the group at stage offset o (= pitch + tile offset) of plane p; c = d_k on p, zm = d_k on p-1, e = tile offset of
+    // this lane's x neighbour.  rv: r_{k+1}, dp: d_{k-1}.
+    auto dnew = [&](const float* sc, const float* sn, int o, int e, const float4& c, const float4& zm, float4& rv, float4& dp, float4& zp) {
+        const float4 ym = lds4(sc, o - pitch), yp = lds4(sc, o + pitch);
+        zp = lds4(sn, o);
+        float xl = __shfl_up_sync(0xffffffffu, c.w, 1), xr = __shfl_down_sync(0xffffffffu, c.x, 1);
+        const float ev = sc[pitch + e];
+        if (lane == 0) xl = ev;
+        if (lane == 31) xr = ev;
+        const float4 q = stencil7(c, xl, xr, ym, yp, zm, zp, ix2, iy2, iz2, cc);
+        rv = c; dp = f4_splat(0.f);                          // r_k = d_k - beta_k d_{k-1}; r_0 = d_0 (d_{k-1} slot not staged)
+        if (has_prev) {
+            dp = lds4(sc, pb + o - pitch);
+            rv = make_float4(fmaf(-bprev, dp.x, c.x), fmaf(-bprev, dp.y, c.y), fmaf(-bprev, dp.z, c.z), fmaf(-bprev, dp.w, c.w));
+        }
+        rv.x = fmaf(-alpha, q.x, rv.x); rv.y = fmaf(-alpha, q.y, rv.y); rv.z = fmaf(-alpha, q.z, rv.z); rv.w = fmaf(-alpha, q.w, rv.w);
+        return make_float4(fmaf(beta, c.x, rv.x), fmaf(beta, c.y, rv.y), fmaf(beta, c.z, rv.z), fmaf(beta, c.w, rv.w));
+    };
+
+    float4 dm[FUSED_GI], dc[FUSED_GI];           // d_k on planes p-1, p (owned groups)
+    float4 hm[FUSED_GH], hc[FUSED_GH];           // the same on the halo groups
+    float4 n2[FUSED_GI], n1[FUSED_GI];           // d_{k+1} on planes p-2, p-1
+    float4 r1[FUSED_GI];                         // r_{k+1} on plane p-1
+    float4 xv[FUSED_GI];                         // x on plane p (x-update iterations), loaded during plane p-1
     SlotIt cur = rg.pos, nxt = cur; nxt.next(cfg.R);
     ring_wait_full(rg, cur); ring_wait_full(rg, nxt);
     {
         const float* s0 = ring_ptr(rg, cfg, cur);
         const float* s1 = ring_ptr(rg, cfg, nxt);
 #pragma unroll
-        for (int k = 0; k < RING_GF; ++k) {
-            dm[k] = f4_splat(0.f); dc[k] = f4_splat(0.f);
-            if (fg.valid & (1u << k)) { dm[k] = lds4(s0, pitch + fg.t[k]); dc[k] = lds4(s1, pitch + fg.t[k]); }
-            n2[k] = n1[k] = r1[k] = f4_splat(0.f);
+        for (int k = 0; k < FUSED_GI; ++k) {
+            dm[k] = dc[k] = n2[k] = n1[k] = r1[k] = xv[k] = f4_splat(0.f);
+            if (fg.vi & (1u << k)) { dm[k] = lds4(s0, pitch + fg.ti[k]); dc[k] = lds4(s1, pitch + fg.ti[k]); }
+        }
+#pragma unroll
+        for (int k = 0; k < FUSED_GH; ++k) {
+            hm[k] = hc[k] = f4_splat(0.f);
+            if (fg.vh & (1u << k)) { hm[k] = lds4(s0, pitch + fg.th[k]); hc[k] = lds4(s1, pitch + fg.th[k]); }
         }
     }
     ring_release(rg, cur);
@@ -1137,54 +1176,56 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
         const float* sc = ring_ptr(rg, cfg, cur);
         const float* sn = ring_ptr(rg, cfg, nxt);
         float* tw = tile + (i % FUSED_TILE_BUFS) * tsz;
-        float4 n0[RING_GF], r0[RING_GF];
 #pragma unroll
-        for (int k = 0; k < RING_GF; ++k) {
+        for (int k = 0; k < FUSED_GH; ++k) {
+            if (!(fg.vh & (1u << k))) continue;
+            float4 rv, dp, zp;
+            const float4 dv = dnew(sc, sn, pitch + fg.th[k], fg.eh[k], hc[k], hm[k], rv, dp, zp);
+            *reinterpret_cast<float4*>(tw + fg.th[k]) = dv;
+            hm[k] = hc[k]; hc[k] = zp;
+        }
+        float4 n0[FUSED_GI], r0[FUSED_GI];
+        float* const dnp = P.dn + plane_off;
+        float* const xp = P.x ? P.x + plane_off : nullptr;
+#pragma unroll
+        for (int k = 0; k < FUSED_GI; ++k) {
             n0[k] = r0[k] = f4_splat(0.f);
-            if (!(fg.valid & (1u << k))) continue;
-            const int o = pitch + fg.t[k];
+            if (!(fg.vi & (1u << k))) continue;
             const float4 c = dc[k];
-            const float4 ym = lds4(sc, o - pitch), yp = lds4(sc, o + pitch), zp = lds4(sn, o);
-            float xl = __shfl_up_sync(0xffffffffu, c.w, 1), xr = __shfl_down_sync(0xffffffffu, c.x, 1);
-            const float el = sc[pitch + fg.tl[k]], er = sc[pitch + fg.tr[k]];
-            xl = (fg.needl & (1u << k)) ? el : xl;
-            xr = (fg.needr & (1u << k)) ? er : xr;
-            const float4 q = stencil7(c, xl, xr, ym, yp, dm[k], zp, ix2, iy2, iz2, cc);
-            float4 rv = c, dp = f4_splat(0.f);                 // r_k = d_k - beta_k d_{k-1}; r_0 = d_0 (d_{k-1} slot not staged)
-            if (has_prev) {
-                dp = lds4(sc, pb + fg.t[k]);
-                rv = make_float4(fmaf(-bprev, dp.x, c.x), fmaf(-bprev, dp.y, c.y), fmaf(-bprev, dp.z, c.z), fmaf(-bprev, dp.w, c.w));
-            }
-            rv.x = fmaf(-alpha, q.x, rv.x); rv.y = fmaf(-alpha, q.y, rv.y); rv.z = fmaf(-alpha, q.z, rv.z); rv.w = fmaf(-alpha, q.w, rv.w);
-            const float4 dv = make_float4(fmaf(beta, c.x, rv.x), fmaf(beta, c.y, rv.y), fmaf(beta, c.z, rv.z), fmaf(beta, c.w, rv.w));
-            *reinterpret_cast<float4*>(tw + fg.t[k]) = dv;
-            if (own && (fg.inner & (1u << k))) {
-                const long long off = plane_off + fg.goff[k];
-                *reinterpret_cast<float4*>(P.dn + off) = dv;
+            float4 rv, dp, zp;
+            const float4 dv = dnew(sc, sn, pitch + fg.ti[k], fg.ei[k], c, dm[k], rv, dp, zp);
+            *reinterpret_cast<float4*>(tw + fg.ti[k]) = dv;
+            if (own) {
+                *reinterpret_cast<float4*>(dnp + fg.gi[k]) = dv;
                 acc[1] += dot4(rv, rv);
-                if (P.x) {                                   // odd k: d_{k-1} is staged
-                    float4 xv = lds4(sc, xb + fg.t[k]);
-                    xv.x += aprev * dp.x; xv.y += aprev * dp.y; xv.z += aprev * dp.z; xv.w += aprev * dp.w;
-                    xv.x += alpha * c.x; xv.y += alpha * c.y; xv.z += alpha * c.z; xv.w += alpha * c.w;
-                    *reinterpret_cast<float4*>(P.x + off) = xv;
+                if (xp) {                                    // odd k: d_{k-1} is staged
+                    float4 x4 = xv[k];
+                    x4.x += aprev * dp.x; x4.y += aprev * dp.y; x4.z += aprev * dp.z; x4.w += aprev * dp.w;
+                    x4.x += alpha * c.x; x4.y += alpha * c.y; x4.z += alpha * c.z; x4.w += alpha * c.w;
+                    *reinterpret_cast<float4*>(xp + fg.gi[k]) = x4;
                 }
             }
             n0[k] = dv; r0[k] = rv;
             dm[k] = c; dc[k] = zp;
         }
         ring_release(rg, cur);
+        if (xp && i < nz) {                          // x of the next owned plane, in flight while q_{k+1} is formed
+#pragma unroll
+            for (int k = 0; k < FUSED_GI; ++k)
+                if (fg.vi & (1u << k)) xv[k] = __ldcs(reinterpret_cast<const float4*>(xp + pf.sz + fg.gi[k]));
+        }
         asm volatile("bar.sync 1, %0;" ::"r"(cfg.consumers) : "memory");      // the tile of plane p is complete
         if (i >= 2) {                                // q_{k+1} on plane p - 1 (owned: i - 1 in 1 .. nz)
             const float* tp = tile + ((i - 1) % FUSED_TILE_BUFS) * tsz;
 #pragma unroll
-            for (int k = 0; k < RING_GF; ++k) {
-                if (!(fg.inner & (1u << k))) continue;
+            for (int k = 0; k < FUSED_GI; ++k) {
+                if (!(fg.vi & (1u << k))) continue;
                 const float4 c = n1[k];
-                const float4 ym = lds4(tp, fg.t[k] - pitch), yp = lds4(tp, fg.t[k] + pitch);
+                const float4 ym = lds4(tp, fg.ti[k] - pitch), yp = lds4(tp, fg.ti[k] + pitch);
                 float xl = __shfl_up_sync(0xffffffffu, c.w, 1), xr = __shfl_down_sync(0xffffffffu, c.x, 1);
-                const float el = tp[fg.tl[k]], er = tp[fg.tr[k]];
-                xl = (fg.needl & (1u << k)) ? el : xl;
-                xr = (fg.needr & (1u << k)) ? er : xr;
+                const float ev = tp[fg.ei[k]];
+                if (lane == 0) xl = ev;
+                if (lane == 31) xr = ev;
                 const float4 q = stencil7(c, xl, xr, ym, yp, n2[k], n0[k], ix2, iy2, iz2, cc);
                 acc[0] += dot4(c, q);
                 acc[2] += dot4(r1[k], q);
@@ -1192,7 +1233,7 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
             }
         }
 #pragma unroll
-        for (int k = 0; k < RING_GF; ++k) { n2[k] = n1[k]; n1[k] = n0[k]; r1[k] = r0[k]; }
+        for (int k = 0; k < FUSED_GI; ++k) { n2[k] = n1[k]; n1[k] = n0[k]; r1[k] = r0[k]; }
         cur = nxt; nxt.next(cfg.R);
         plane_off += pf.sz;
     }
@@ -1736,7 +1777,6 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     // obstacles 4 TY + 6 lines, inside the 5 TY + 6 of cg_ring_config)
     if (l.prm.method == PHI_SOLVER_CG_ADAPTIVE && !xslot && A.cfg.TY == 1
         && !ring_config(g, 4, 3, cgs, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, sms, &A.cfg)) return -100;
-    const int threads = RING_THREADS;
     A.ring_smem_offset = cgs;
     int per_sm = 0;
     cudaError_t e;
@@ -1752,17 +1792,20 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
         const DField& pf = l.pf;
         if (!(e && atoi(e) == 2) && g.dim == 3 && !generic && !dist && !adapt && op == CgOp::Poisson && l.prm.matrix_offset == 0.f
             && pf.klo[1] == PHI_BC_PERIODIC && pf.khi[1] == PHI_BC_PERIODIC && pf.klo[2] == PHI_BC_PERIODIC && pf.khi[2] == PHI_BC_PERIODIC) {
-            // stage = d_k (TY+4) + d_{k-1} (TY+2) + x (TY) lines; the d_{k+1} tile is reserved at the largest TY ring_config may pick
+            // stage = d_k (TY+4) + d_{k-1} (TY+2) lines; the tile is chosen with TY more lines per stage (3 TY + 6), which keeps the
+            // tiling pass F had while it staged x (lines up to 1024 cells at TY 1).  The d_{k+1} tile is reserved at the largest TY
+            // ring_config may pick.
             RingCfg fc;
             if (ring_config(g, 3, 6, cgs, 4, RING_MAX_STAGES, sms, &fc, RING_CONSUMERS, 4)
                 && ring_config(g, 3, 6, cgs + FUSED_TILE_BUFS * (fc.TY + 2) * fc.pitch * 4, 4, RING_MAX_STAGES, sms, &fc, RING_CONSUMERS, 4)
-                && ring_all_fast(g, pf, fc) && (fc.TY + 2) * fc.nx4 <= RING_GF * fc.consumers) {
+                && ring_all_fast(g, pf, fc) && fc.TY * fc.nx4 <= FUSED_GI * fc.consumers && 2 * fc.nx4 <= FUSED_GH * fc.consumers) {
                 fused = true;
                 A.cfg = fc;
                 tile_bytes = (size_t)FUSED_TILE_BUFS * (fc.TY + 2) * fc.pitch * 4;
             }
         }
     }
+    const int threads = RING_THREADS;
     const size_t smem = (size_t)cgs + 128 + (size_t)A.cfg.R * A.cfg.stage_floats * 4 + tile_bytes;
     const void* fn = (const void*)cg_ring_kernel(op, g.dim, generic, dist, adapt, fused);
     if (!fn) return -100;
