@@ -108,3 +108,75 @@ __device__ __forceinline__ void reduce_partials(const CgShared& sh, const double
     __syncthreads();
 }
 
+// ---- per-entry bookkeeping of a solve (the caller runs these in its `for (b = threadIdx.x; ...)` loops) -----------------------
+
+// Setup sums sum0 = sum y, sum1 = sum of the accessible mask (MASK) or of x0 -> balanced right-hand side y - mean (* mask,
+// fluid.py:205-209) and the offset c * sum x0 of the rank-1 matrix offset.  cells: the global cell count.
+template <bool MASK>
+__device__ __forceinline__ void cg_balance(const CgShared& sh, const PhiCgParams& prm, int b, double cells)
+{
+    if (MASK) { sh.mean[b] = (prm.balance_rhs && sh.sum1[b] > 0.0) ? (float)(sh.sum0[b] / sh.sum1[b]) : 0.f; sh.offs[b] = 0.f; }
+    else { sh.mean[b] = prm.balance_rhs ? (float)(sh.sum0[b] / cells) : 0.f; sh.offs[b] = prm.matrix_offset * (float)sh.sum1[b]; }
+}
+
+// Sums of the zero-mean projection, sum0 = sum x (* mask), sum1 = sum of the mask (MASK) -> the mean to remove.
+template <bool MASK>
+__device__ __forceinline__ float cg_projection_mean(const CgShared& sh, int b, double cells)
+{
+    return MASK ? (sh.sum1[b] > 0.0 ? (float)(sh.sum0[b] / sh.sum1[b]) : 0.f) : (float)(sh.sum0[b] / cells);
+}
+
+// End of an iteration of entry b with the new |r|^2 (the caller has formed its step sizes): iteration count and the stopping
+// rule of stop_on_l2 (_linalg.py:29-36).  Returns whether the entry continues.
+__device__ __forceinline__ bool cg_iteration_done(const CgShared& sh, const PhiCgParams& prm, int b, double rsq_new)
+{
+    sh.delta[b] = rsq_new;
+    const int it = ++sh.iters[b];
+    const float rsq = fabsf((float)rsq_new);
+    const bool conv = rsq <= sh.tol_sq[b];
+    const bool divg = !isfinite(rsq) || (rsq / sh.rsq0[b] > 1e5f && it >= 8);
+    const bool cont = !conv && !divg && it < prm.max_iter;
+    sh.conv[b] = conv; sh.divg[b] = divg; sh.cont[b] = cont ? 1 : 0;
+    return cont;
+}
+
+// ---- whole-CTA steps ----------------------------------------------------------------------------------------------------------
+
+// *any_cont = whether any entry still runs.  Every CTA computes it from its own copy of the flags, so all take the same branch.
+__device__ __forceinline__ void cg_count_running(const CgShared& sh, int batch)
+{
+    __syncthreads();
+    if (threadIdx.x == 0) { int any = 0; for (int b = 0; b < batch; ++b) any |= sh.cont[b]; *sh.any_cont = any; }
+    __syncthreads();
+}
+
+// Start of the solve from the r0 sums: sum0 = |r0|^2, sum1 = the tolerance reference (|r0| without the matrix offset, or |y|^2
+// for CG-adaptive; _linalg.py:61-67).  An entry that already meets the tolerance does not iterate.
+__device__ __forceinline__ void cg_start(const CgShared& sh, const PhiCgParams& prm, int batch)
+{
+    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+        const double d0 = sh.sum0[b], d0tol = sh.sum1[b];
+        sh.delta[b] = d0;
+        const float tol = fmaxf(prm.rtol * prm.rtol * (float)d0tol, prm.atol * prm.atol);
+        sh.tol_sq[b] = tol; sh.rsq0[b] = (float)d0;
+        const bool conv = (float)d0 <= tol;
+        const bool divg = !isfinite((float)d0);
+        sh.conv[b] = conv; sh.divg[b] = divg; sh.iters[b] = 0;
+        sh.cont[b] = (!conv && !divg && prm.max_iter > 0) ? 1 : 0;
+        sh.beta[b] = 0.f; sh.alpha[b] = 0.f; sh.aprev[b] = 0.f;
+    }
+    cg_count_running(sh, batch);
+}
+
+// Block 0 writes the PhiCgResult of every entry.  comm_ok false (a multi-GPU all-reduce timed out): diverged = -1.
+__device__ __forceinline__ void cg_write_result(const CgShared& sh, PhiCgResult* result, int batch, bool comm_ok)
+{
+    if (blockIdx.x != 0) return;
+    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+        PhiCgResult res;
+        res.iterations = sh.iters[b]; res.converged = sh.conv[b]; res.diverged = comm_ok ? sh.divg[b] : -1;
+        res.residual_sq = fabsf((float)sh.delta[b]); res.tol_sq = sh.tol_sq[b]; res.initial_residual_sq = sh.rsq0[b];
+        result[b] = res;
+    }
+}
+

@@ -171,10 +171,7 @@ k_cg_poisson(CgArgs a)
             });
         });
         barrier_and_reduce(nullptr);
-        for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-            if (MASK) { sh.mean[b] = (a.prm.balance_rhs && sh.sum1[b] > 0.0) ? (float)(sh.sum0[b] / sh.sum1[b]) : 0.f; sh.offs[b] = 0.f; }
-            else { sh.mean[b] = a.prm.balance_rhs ? (float)(sh.sum0[b] / cells) : 0.f; sh.offs[b] = coffs * (float)sh.sum1[b]; }
-        }
+        for (int b = threadIdx.x; b < batch; b += blockDim.x) cg_balance<MASK>(sh, a.prm, b, cells);
         __syncthreads();
     }
 
@@ -187,20 +184,7 @@ k_cg_poisson(CgArgs a)
         acc0 += epi.acc0; acc1 += epi.acc1;
     });
     barrier_and_reduce(nullptr);
-    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-        const double d0 = sh.sum0[b], d0tol = sh.sum1[b];
-        sh.delta[b] = d0;
-        const float tol = fmaxf(a.prm.rtol * a.prm.rtol * (float)d0tol, a.prm.atol * a.prm.atol);
-        sh.tol_sq[b] = tol; sh.rsq0[b] = (float)d0;
-        const bool conv = (float)d0 <= tol;
-        const bool divg = !isfinite((float)d0);
-        sh.conv[b] = conv; sh.divg[b] = divg; sh.iters[b] = 0;
-        sh.cont[b] = (!conv && !divg && a.prm.max_iter > 0) ? 1 : 0;
-        sh.beta[b] = 0.f; sh.alpha[b] = 0.f;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) { int any = 0; for (int b = 0; b < batch; ++b) any |= sh.cont[b]; *sh.any_cont = any; }
-    __syncthreads();
+    cg_start(sh, a.prm, batch);
 
     float* dold = a.d0; float* dnew = a.d1;
     while (*sh.any_cont) {
@@ -235,17 +219,9 @@ k_cg_poisson(CgArgs a)
             const double dn = sh.sum0[b];
             const double dold_ = sh.delta[b];
             sh.beta[b] = (dold_ != 0.0) ? (float)(dn / dold_) : 0.f;
-            sh.delta[b] = dn;
-            const int it = ++sh.iters[b];
-            const float rsq = fabsf((float)dn);
-            const bool conv = rsq <= sh.tol_sq[b];
-            bool divg = !isfinite(rsq) || (rsq / sh.rsq0[b] > 1e5f && it >= 8);   // stop_on_l2 (_linalg.py:29-36)
-            sh.conv[b] = conv; sh.divg[b] = divg;
-            sh.cont[b] = (!conv && !divg && it < a.prm.max_iter) ? 1 : 0;
+            cg_iteration_done(sh, a.prm, b, dn);
         }
-        __syncthreads();
-        if (threadIdx.x == 0) { int any = 0; for (int b = 0; b < batch; ++b) any |= sh.cont[b]; *sh.any_cont = any; }
-        __syncthreads();
+        cg_count_running(sh, batch);
         float* t = dold; dold = dnew; dnew = t;
     }
 
@@ -260,21 +236,14 @@ k_cg_poisson(CgArgs a)
         for (int unit = blockIdx.x; unit < um.total_units; unit += gridDim.x) {
             const WarpUnit w = phi_warp_unit<DIM>(g, um, unit, warp);
             if (!w.valid) continue;
-            const float m = MASK ? (sh.sum1[w.b] > 0.0 ? (float)(sh.sum0[w.b] / sh.sum1[w.b]) : 0.f) : (float)(sh.sum0[w.b] / cells);
+            const float m = cg_projection_mean<MASK>(sh, w.b, cells);
             for_unit_cells<DIM>(g, a.pf, w, [&](long long off, int nvalid) {
                 for (int j = 0; j < nvalid; ++j) a.x[off + j] -= MASK ? m * a.acc[off + j] : m;
             });
         }
     }
 
-    if (blockIdx.x == 0) {
-        for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-            PhiCgResult res;
-            res.iterations = sh.iters[b]; res.converged = sh.conv[b]; res.diverged = sh.divg[b];
-            res.residual_sq = fabsf((float)sh.delta[b]); res.tol_sq = sh.tol_sq[b]; res.initial_residual_sq = sh.rsq0[b];
-            a.result[b] = res;
-        }
-    }
+    cg_write_result(sh, a.result, batch, true);
 }
 
 // ---- host side --------------------------------------------------------------------------------------------------

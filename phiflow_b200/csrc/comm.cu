@@ -119,8 +119,6 @@ static int cg_dist(const PhiGrid* g, const PhiVBC* vbc, const float* rhs, float*
         cm.flag[q] = (unsigned long long*)(c->peer[q] + c->off_flags);
     }
     cm.seq = (unsigned long long*)(c->local + c->off_seq);
-    cm.arrive = (unsigned*)(c->local + c->off_seq + 64);
-    { cudaError_t ce = cudaMemsetAsync(cm.arrive, 0, sizeof(unsigned), (cudaStream_t)stream); if (ce != cudaSuccess) { phi_set_error("cg_dist: memset failed: %s", cudaGetErrorString(ce)); return (int)ce; } }
     if (cm.lower >= 0) { const CgWorkspace w = phi_cg_workspace(l.g, c->peer[cm.lower] + c->off_ws); cm.lo_r = w.r; cm.lo_d0 = w.d0; cm.lo_d1 = w.d1; }
     if (cm.upper >= 0) { const CgWorkspace w = phi_cg_workspace(l.g, c->peer[cm.upper] + c->off_ws); cm.hi_r = w.r; cm.hi_d0 = w.d0; cm.hi_d1 = w.d1; }
     if (c->n > 1 && (cm.lower < 0 && cm.upper < 0)) { phi_set_error("cg_dist: %d ranks but no PHI_BC_HALO side on the z axis", c->n); return PHI_ERR_INVALID; }

@@ -80,7 +80,6 @@ struct CommDev {                      // device view of the multi-GPU communicat
     double* mbox[PHI_MAX_RANKS];      // mailbox of every rank ([rank] = local), [2 parity][PHI_MAX_RANKS][2*CG_MAX_BATCH]
     unsigned long long* flag[PHI_MAX_RANKS];   // [2 parity][PHI_MAX_RANKS] event numbers
     unsigned long long* seq;          // local persistent event counter
-    unsigned* arrive;                 // local arrival counter of the merged barrier (zeroed by the launcher)
     float *lo_r, *lo_d0, *lo_d1;      // lower neighbour's CG vectors (first owned plane)
     float *hi_r, *hi_d0, *hi_d1;      // upper neighbour's
 };

@@ -37,9 +37,6 @@ struct RingCfg {
     int consumers;             // consumer threads per CTA (256 or 512); the producer warp follows them
     int groups;                // ceil(TY * nx4 / consumers)
     int shfl_ok;               // lanes of a warp own consecutive groups of one line -> x neighbours via shuffles
-    int hint;                  // 1: element-wise lines are fetched with an L2 evict-first policy
-    int merge;                 // 1: lines that are contiguous in memory travel in one bulk copy
-    int dbg;                   // profiling only (PHICUDA_RING_DEBUG): 1 skip CG pass A, 2 skip pass B, 4 consumers skip the arithmetic
     // "tail split" decomposition of the CG kernel (3-D, batch 1, fewer y tiles than persistent CTAs): CTA c < nyt marches tile c
     // over planes [0, Zm); the remaining CTAs share the tails [Zm, nz) of all tiles, split_t tiles each.  Keeps every SM busy
     // when the tile count does not divide the CTA count (128 tiles on 132 SMs for 512-wide slabs).
@@ -70,15 +67,6 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-// same copy with an L2 evict-first policy: element-wise streams (x, r, rhs) are read once per pass, so they should not push the
-// halo lines that neighbouring CTAs still need out of L2
-__device__ __forceinline__ void bulk_g2s_stream(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar)
-{
-    uint64_t pol;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
@@ -126,6 +114,20 @@ struct ProdUnit {
     int tot_h, tot_e;           // warp totals of active lines
 };
 
+// A line that continues the one held by the previous lane (same key = array, next source row yv) rides on that lane's copy.
+// key < 0: the lane holds no line.  Returns whether this lane issues a copy; if so, nbytes covers its line and the ones that follow.
+__device__ __forceinline__ bool prod_merge_lines(int key, int yv, bool mergeable, uint32_t row_bytes, uint32_t& nbytes)
+{
+    const int lane = threadIdx.x & 31;
+    const int pkey = __shfl_up_sync(0xffffffffu, key, 1), pyv = __shfl_up_sync(0xffffffffu, yv, 1);
+    const bool cont = mergeable && key >= 0 && lane > 0 && pkey == key && pyv + 1 == yv;
+    const unsigned cm = __ballot_sync(0xffffffffu, cont);
+    if (key < 0 || cont) return false;
+    const unsigned follow = lane == 31 ? 0u : (cm >> (lane + 1));
+    nbytes = (uint32_t)__ffs(~follow) * row_bytes;          // 1 + number of lines that continue this one
+    return true;
+}
+
 // hactive: bit k set = haloed slot k is fetched (slot 1 idles in the first CG iteration; with obstacles the last slot is the mask)
 // KSLOT (varying diffusivity): the last haloed slot is read from batch entry kb instead of b (kb = 0 broadcasts one k to all entries)
 template <int DIM, bool KSLOT = false>
@@ -135,7 +137,7 @@ __device__ __forceinline__ void prod_unit_setup(ProdUnit& pu, const RingCfg& cfg
 {
     const int lane = threadIdx.x & 31, hrows = cfg.TY + 2;
     const uint32_t row_bytes = (uint32_t)cfg.pitch * 4u;
-    const bool mergeable = cfg.merge && pf.sy == cfg.pitch;      // neighbouring lines are contiguous in memory and in the stage
+    const bool mergeable = pf.sy == cfg.pitch;      // neighbouring lines are contiguous in memory and in the stage
     pu.hmask = pu.emask = 0;
     int ch = 0, ce = 0;
 #pragma unroll
@@ -163,13 +165,7 @@ __device__ __forceinline__ void prod_unit_setup(ProdUnit& pu, const RingCfg& cfg
                 key = 8 + arr; yv = yy; ce++;
             }
         }
-        // a line that continues the one held by the previous lane (same array, next row) rides on that lane's copy
-        const int pkey = __shfl_up_sync(0xffffffffu, key, 1), pyv = __shfl_up_sync(0xffffffffu, yv, 1);
-        const bool cont = mergeable && key >= 0 && lane > 0 && pkey == key && pyv + 1 == yv;
-        const unsigned cm = __ballot_sync(0xffffffffu, cont);
-        if (key >= 0 && !cont) {
-            const unsigned follow = lane == 31 ? 0u : (cm >> (lane + 1));
-            pu.nbytes[it] = (uint32_t)__ffs(~follow) * row_bytes;          // 1 + number of lines that continue this one
+        if (prod_merge_lines(key, yv, mergeable, row_bytes, pu.nbytes[it])) {
             if (halo_line) pu.hmask |= 1u << it; else pu.emask |= 1u << it;
         }
     }
@@ -199,10 +195,7 @@ __device__ __forceinline__ void ring_produce(Ring& rg, const RingCfg& cfg, const
     __syncwarp();
 #pragma unroll
     for (int it = 0; it < 4; ++it)
-        if (mask & (1u << it)) {
-            if (cfg.hint && (pu.emask & (1u << it))) bulk_g2s_stream(sbase + pu.dsto[it], pu.base[it] + pu.yoff[it] + zoff, pu.nbytes[it], full);
-            else bulk_g2s(sbase + pu.dsto[it], pu.base[it] + pu.yoff[it] + zoff, pu.nbytes[it], full);
-        }
+        if (mask & (1u << it)) bulk_g2s(sbase + pu.dsto[it], pu.base[it] + pu.yoff[it] + zoff, pu.nbytes[it], full);
     rg.pos.next(cfg.R);
 }
 
@@ -485,7 +478,6 @@ __device__ __forceinline__ void ring_compute_any(const RingCfg& cfg, const DGrid
                                                  bool fast, const float* sm, const float* sc, const float* sp, float beta,
                                                  long long plane_off, int z, Epi& epi, ZMarch& zs, const CgOperator* od)
 {
-    if (cfg.dbg & 4) return;
     if (cg_op_xslot(OP)) { zs.have = false; ring_compute<DIM, NH, NE, OP>(cfg, g, pf, tg, sm, sc, sp, beta, plane_off, z, epi, od); return; }
     if (!GENERIC || fast) {
         if (cfg.groups == 4) { ring_compute_fast<DIM, NH, NE, 4, MARCH>(cfg, g, tg, sm, sc, sp, beta, plane_off, epi, zs); return; }
@@ -547,9 +539,8 @@ __device__ __forceinline__ void ring_consume_planes(Ring& rg, const RingCfg& cfg
         ring_wait_full(rg, c2);
         epi.set_plane(z, g.n[2]);
         if (G > 0) {
-            if (!(cfg.dbg & 4))
-                ring_compute_fast<3, NH, NE, (G > 0 ? G : 1), MARCH>(cfg, g, tg, ring_ptr(rg, cfg, a), ring_ptr(rg, cfg, bq), ring_ptr(rg, cfg, c2),
-                                                                     beta, plane_off, epi, zs);
+            ring_compute_fast<3, NH, NE, (G > 0 ? G : 1), MARCH>(cfg, g, tg, ring_ptr(rg, cfg, a), ring_ptr(rg, cfg, bq), ring_ptr(rg, cfg, c2),
+                                                                 beta, plane_off, epi, zs);
         } else {
             const bool fast = tile_fast && !(z == 0 && pf.klo[2] == PHI_BC_CONST) && !(z == g.n[2] - 1 && pf.khi[2] == PHI_BC_CONST);
             ring_compute_any<GENERIC, 3, NH, NE, MARCH, OP>(cfg, g, pf, tg, fast, ring_ptr(rg, cfg, a), ring_ptr(rg, cfg, bq), ring_ptr(rg, cfg, c2),
@@ -669,25 +660,9 @@ struct REpiResidual0 {          // e0 = rhs
     }
 };
 
-template <class PH>
+// pass A: stores d', sums d'.Ad' and sum d'; ADAPT (CG-adaptive): the second sum is d'.r (e0 = r, element-wise), _linalg.py:113
+template <class PH, bool ADAPT>
 struct REpiPassA {
-    __device__ __forceinline__ void set_acc(const float4&) {}
-    float* dnew; float acc0, acc1; PH ph;
-    __device__ __forceinline__ void set_plane(int z, int nz) { ph.set_plane(z, nz); }
-    __device__ __forceinline__ void operator()(long long off, const float4& c, const float4& q, int nvalid, const float4&, const float4&, const float4&)
-    {
-        if (nvalid == 4) {
-            *reinterpret_cast<float4*>(dnew + off) = c;
-            if (ph.zf) ph.put4(off, c);
-            acc0 += c.x * q.x + c.y * q.y + c.z * q.z + c.w * q.w;
-            acc1 += (c.x + c.y) + (c.z + c.w);
-        } else for (int j = 0; j < nvalid; ++j) { const float v = f4_get(c, j); dnew[off + j] = v; if (ph.zf) ph.put1(off + j, v); acc0 += v * f4_get(q, j); acc1 += v; }
-    }
-};
-
-// CG-adaptive pass A: the second sum is d'.r (e0 = r, element-wise), _linalg.py:113
-template <class PH>
-struct REpiPassAAdapt {
     __device__ __forceinline__ void set_acc(const float4&) {}
     float* dnew; float acc0, acc1; PH ph;
     __device__ __forceinline__ void set_plane(int z, int nz) { ph.set_plane(z, nz); }
@@ -697,8 +672,12 @@ struct REpiPassAAdapt {
             *reinterpret_cast<float4*>(dnew + off) = c;
             if (ph.zf) ph.put4(off, c);
             acc0 += c.x * q.x + c.y * q.y + c.z * q.z + c.w * q.w;
-            acc1 += c.x * re.x + c.y * re.y + c.z * re.z + c.w * re.w;
-        } else for (int j = 0; j < nvalid; ++j) { const float v = f4_get(c, j); dnew[off + j] = v; if (ph.zf) ph.put1(off + j, v); acc0 += v * f4_get(q, j); acc1 += v * f4_get(re, j); }
+            if (ADAPT) acc1 += c.x * re.x + c.y * re.y + c.z * re.z + c.w * re.w;
+            else acc1 += (c.x + c.y) + (c.z + c.w);
+        } else for (int j = 0; j < nvalid; ++j) {
+            const float v = f4_get(c, j); dnew[off + j] = v; if (ph.zf) ph.put1(off + j, v); acc0 += v * f4_get(q, j);
+            if (ADAPT) acc1 += v * f4_get(re, j); else acc1 += v;
+        }
     }
 };
 
@@ -796,7 +775,6 @@ struct CgRingArgs {
     CgArgs a;
     RingCfg cfg;
     int ring_smem_offset;        // byte offset of the ring inside dynamic shared memory (after the CgShared block)
-    int comm_merge;              // multi-GPU: 1 = merged barrier + all-reduce (comm_barrier_allreduce), 0 = grid.sync + comm_allreduce
     CommDev cm;
     float* d2;                   // one-sweep CG: third direction buffer
     CgOperator op;               // the mask travels in a.acc
@@ -838,59 +816,6 @@ __device__ __forceinline__ bool comm_allreduce(const CommDev& cm, const CgShared
     const int par = (int)(seq & 1ull);
     const size_t stride = 2 * (size_t)CG_MAX_BATCH;
     if (blockIdx.x == 0) {
-        for (int q = 0; q < cm.n; ++q) {
-            double* dst = cm.mbox[q] + ((size_t)par * PHI_MAX_RANKS + cm.rank) * stride;
-            for (int b = threadIdx.x; b < batch; b += blockDim.x) { dst[b] = sh.sum0[b]; dst[CG_MAX_BATCH + b] = sh.sum1[b]; }
-        }
-        __threadfence_system();
-        __syncthreads();
-        if ((int)threadIdx.x < cm.n) st_release_sys(cm.flag[threadIdx.x] + par * PHI_MAX_RANKS + cm.rank, seq);
-    }
-    bool ok = true;
-    if ((int)threadIdx.x < cm.n) {
-        const unsigned long long* f = cm.flag[cm.rank] + par * PHI_MAX_RANKS + threadIdx.x;
-        const long long t0 = clock64();
-        while (ld_acquire_sys(f) < seq) {
-            if (clock64() - t0 > 40000000000ll) { ok = false; break; }        // ~20 s: a peer died; do not hang the GPU
-        }
-    }
-    ok = __syncthreads_and(ok);
-    const double* src = cm.mbox[cm.rank] + (size_t)par * PHI_MAX_RANKS * stride;
-    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-        double s0 = 0, s1 = 0;
-        for (int q = 0; q < cm.n; ++q) {
-            s0 += *(volatile const double*)(src + q * stride + b);
-            s1 += *(volatile const double*)(src + q * stride + CG_MAX_BATCH + b);
-        }
-        sh.sum0[b] = s0; sh.sum1[b] = s1;
-    }
-    __syncthreads();
-    return ok;
-}
-
-// Merged barrier + all-reduce of the multi-GPU kernels - an experiment, opt-in with PHICUDA_COMM_MERGE=1 (default: grid.sync +
-// comm_allreduce; the two measure the same, see phi_launch_cg_ring).
-// Every CTA makes its stores visible system-wide (partial sums, halo planes stored into the neighbours' memory) and arrives on a
-// local counter; the LAST CTA to arrive sums the per-CTA partials in a fixed order and sends the result with a release flag to
-// every rank (itself included); every CTA of every rank then waits for the n flags in its own mailbox and adds the n entries in
-// rank order.  One arrival + one flag hop instead of a full grid barrier followed by block 0's send: the local release of the
-// grid barrier, the redundant partial reduction in all CTAs and block 0's serial send are gone.  The own rank's flag is only
-// written after all local CTAs arrived, so passing the wait still implies "every local CTA finished the pass".
-__device__ __forceinline__ bool comm_barrier_allreduce(const CommDev& cm, const CgShared& sh, const double* partials, int region, int batch,
-                                                       int units_per_batch, const unsigned char* active, unsigned long long seq)
-{
-    const int par = (int)(seq & 1ull);
-    const size_t stride = 2 * (size_t)CG_MAX_BATCH;
-    __threadfence_system();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        const unsigned prev = atomicAdd(cm.arrive, 1u);
-        sh.any_cont[1] = ((prev + 1u) % gridDim.x == 0u) ? 1 : 0;
-    }
-    __syncthreads();
-    if (sh.any_cont[1]) {                                    // CTA-uniform: the last arriver
-        __threadfence();
-        reduce_partials(sh, partials, region, batch, units_per_batch, active);
         for (int q = 0; q < cm.n; ++q) {
             double* dst = cm.mbox[q] + ((size_t)par * PHI_MAX_RANKS + cm.rank) * stride;
             for (int b = threadIdx.x; b < batch; b += blockDim.x) { dst[b] = sh.sum0[b]; dst[CG_MAX_BATCH + b] = sh.sum1[b]; }
@@ -1001,28 +926,20 @@ __device__ __forceinline__ void fused_groups_init(FusedGroups& fg, const RingCfg
     }
 }
 
-// Producer of pass F.  Staged line slots: d_k (TY+4 lines from y0-2), d_{k-1} (TY+2 from y0-1).  Category 0 (d_k) is fetched on every
-// plane of the unit, 1 (d_{k-1}) on planes z0-1 .. z1.  A null source (d_{k-1} in iteration 0) is not fetched.
-struct ProdUnitF {
-    long long yoff[4];
-    const float* base[4];
-    uint32_t dsto[4];
-    uint32_t nbytes[4];
-    unsigned m[2];
-    int tot[2];
-};
-
-__device__ __forceinline__ void prod_fused_setup(ProdUnitF& pu, const RingCfg& cfg, const DGrid& g, const DField& pf,
-                                                 const float* d, const float* dprev, int b, int y0)
+// Producer of pass F: the haloed lines (hmask, tot_h) are d_k (TY+4 lines from y0-2), fetched on every plane of the unit; the
+// element-wise ones (emask, tot_e) are d_{k-1} (TY+2 lines from y0-1), fetched on planes z0-1 .. z1.  A null source (d_{k-1} in
+// iteration 0) is not fetched.  y and z are periodic, so every line and plane is a stored one and ring_produce<3> streams them.
+__device__ __forceinline__ void prod_fused_setup(ProdUnit& pu, const RingCfg& cfg, const DField& pf, const float* d, const float* dprev,
+                                                 int b, int y0)
 {
     const int lane = threadIdx.x & 31, TY = cfg.TY;
     const uint32_t row_bytes = (uint32_t)cfg.pitch * 4u;
-    const bool mergeable = cfg.merge && pf.sy == cfg.pitch;
+    const bool mergeable = pf.sy == cfg.pitch;
     const int rows[2] = {TY + 4, TY + 2};
     const int ylo[2] = {y0 - 2, y0 - 1};
     const float* src[2] = {d, dprev};
     int cnt[2] = {0, 0};
-    pu.m[0] = pu.m[1] = 0;
+    pu.hmask = pu.emask = 0;
 #pragma unroll
     for (int it = 0; it < 4; ++it) {
         const int line = lane + 32 * it;
@@ -1040,44 +957,16 @@ __device__ __forceinline__ void prod_fused_setup(ProdUnitF& pu, const RingCfg& c
             }
             first += rows[arr];
         }
-        cnt[0] += key == 0; cnt[1] += key == 1;                     // categories: d_k, d_{k-1}
-        const int pkey = __shfl_up_sync(0xffffffffu, key, 1), pyv = __shfl_up_sync(0xffffffffu, yv, 1);
-        const bool cont = mergeable && key >= 0 && lane > 0 && pkey == key && pyv + 1 == yv;
-        const unsigned cm = __ballot_sync(0xffffffffu, cont);
-        if (key >= 0 && !cont) {
-            const unsigned follow = lane == 31 ? 0u : (cm >> (lane + 1));
-            pu.nbytes[it] = (uint32_t)__ffs(~follow) * row_bytes;
-            pu.m[key] |= 1u << it;
+        cnt[0] += key == 0; cnt[1] += key == 1;
+        if (prod_merge_lines(key, yv, mergeable, row_bytes, pu.nbytes[it])) {
+            if (key == 0) pu.hmask |= 1u << it; else pu.emask |= 1u << it;
         }
     }
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
+    for (int c = 0; c < 2; ++c)
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) cnt[c] += __shfl_xor_sync(0xffffffffu, cnt[c], o);
-        pu.tot[c] = cnt[c];
-    }
-}
-
-__device__ __forceinline__ void ring_produce_fused(Ring& rg, const RingCfg& cfg, const DField& pf, const ProdUnitF& pu, int z, bool pplane)
-{
-    const int lane = threadIdx.x & 31;
-    const int slot = rg.pos.slot;
-    const uint32_t full = rg.full0 + 8 * slot;
-    const uint32_t sbase = rg.stage0_s + 4u * (uint32_t)(slot * cfg.stage_floats);
-    float cv;
-    phi_resolve(z, pf, 2, cv);                                      // periodic in z
-    const long long zoff = (long long)z * pf.sz;
-    const unsigned mask = pu.m[0] | (pplane ? pu.m[1] : 0u);
-    const int cnt = pu.tot[0] + (pplane ? pu.tot[1] : 0);
-    if (lane == 0) {
-        mbar_wait(rg.empty0 + 8 * slot, rg.pos.par ^ 1u);
-        mbar_expect_tx(full, (uint32_t)cnt * (uint32_t)cfg.pitch * 4u);
-    }
-    __syncwarp();
-#pragma unroll
-    for (int it = 0; it < 4; ++it)
-        if (mask & (1u << it)) bulk_g2s(sbase + pu.dsto[it], pu.base[it] + pu.yoff[it] + zoff, pu.nbytes[it], full);
-    rg.pos.next(cfg.R);
+    pu.tot_h = cnt[0]; pu.tot_e = cnt[1];
 }
 
 __device__ __forceinline__ float4 lds4(const float* s, int off) { return *reinterpret_cast<const float4*>(s + off); }
@@ -1112,10 +1001,10 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
 {
     const int nz = u.z1 - u.z0;
     if ((int)threadIdx.x >= cfg.consumers) {
-        ProdUnitF pu;
-        prod_fused_setup(pu, cfg, g, pf, P.d, P.dprev, u.b, u.y0);
+        ProdUnit pu;
+        prod_fused_setup(pu, cfg, pf, P.d, P.dprev, u.b, u.y0);
         for (int p = 0; p < nz + 4; ++p)
-            ring_produce_fused(rg, cfg, pf, pu, u.z0 - 2 + p, p >= 1 && p <= nz + 2);
+            ring_produce<3>(rg, cfg, pf, pu, u.z0 - 2 + p, p >= 1 && p <= nz + 2);
         return;
     }
     const int pitch = cfg.pitch, TY = cfg.TY;
@@ -1283,6 +1172,8 @@ k_cg_ring(CgRingArgs A)
     int region = 0;
     ThreadGroups tg;
     groups_init(tg, cfg, g, a.pf);
+    // the operator's haloed array after the CG vectors (cg_op_xslot): the obstacle mask or the diffusivity
+    const float* const xsrc = OP == CgOp::Masked ? a.acc : (OP == CgOp::HelmholtzVarying ? A.op.k : nullptr);
 
     auto sweep = [&](const unsigned char* active, auto&& body) {
         int cur_b = cfg.split ? 0 : -1; float acc0 = 0.f, acc1 = 0.f;      // split mode: every CTA reports for the one batch entry
@@ -1302,12 +1193,6 @@ k_cg_ring(CgRingArgs A)
     bool comm_ok = true;
     auto barrier_and_reduce = [&](const unsigned char* active) {
         fence_proxy_async();                       // generic-proxy stores of this pass -> later TMA (async proxy) loads
-        if (DIST && cm.n > 1 && A.comm_merge) {    // merged barrier + all-reduce
-            comm_ok = comm_barrier_allreduce(cm, sh, a.partials, region, batch, cfg.split ? (int)gridDim.x : cfg.units_per_batch, active, ++seq) && comm_ok;
-            region ^= 1;
-            fence_proxy_async();
-            return;
-        }
         if (cm.n > 1) __threadfence_system();      // halo planes stored into the neighbours' memory
         grid.sync();
         fence_proxy_async();
@@ -1340,15 +1225,12 @@ k_cg_ring(CgRingArgs A)
             });
         });
         barrier_and_reduce(nullptr);
-        for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-            if (MASK) { sh.mean[b] = (a.prm.balance_rhs && sh.sum1[b] > 0.0) ? (float)(sh.sum0[b] / sh.sum1[b]) : 0.f; sh.offs[b] = 0.f; }
-            else { sh.mean[b] = a.prm.balance_rhs ? (float)(sh.sum0[b] / cells) : 0.f; sh.offs[b] = coffs * (float)sh.sum1[b]; }
-        }
+        for (int b = threadIdx.x; b < batch; b += blockDim.x) cg_balance<MASK>(sh, a.prm, b, cells);
         __syncthreads();
     }
 
     {   // r0 = y - (A + c 11^T) x0
-        const float* hsrc[2] = {a.x, (OP == CgOp::Masked ? a.acc : (OP == CgOp::HelmholtzVarying ? A.op.k : nullptr))};
+        const float* hsrc[2] = {a.x, xsrc};
         const float* esrc[2] = {a.rhs, nullptr};
         sweep(nullptr, [&](const RingUnit& u, float& acc0, float& acc1) {
             REpiResidual0<PH> epi{a.r, sh.mean[u.b], sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r), adaptive};
@@ -1358,25 +1240,12 @@ k_cg_ring(CgRingArgs A)
         });
     }
     barrier_and_reduce(nullptr);
-    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-        const double d0 = sh.sum0[b], d0tol = sh.sum1[b];
-        sh.delta[b] = d0;
-        const float tol = fmaxf(a.prm.rtol * a.prm.rtol * (float)d0tol, a.prm.atol * a.prm.atol);
-        sh.tol_sq[b] = tol; sh.rsq0[b] = (float)d0;
-        const bool conv = (float)d0 <= tol;
-        const bool divg = !isfinite((float)d0);
-        sh.conv[b] = conv; sh.divg[b] = divg; sh.iters[b] = 0;
-        sh.cont[b] = (!conv && !divg && a.prm.max_iter > 0) ? 1 : 0;
-        sh.beta[b] = 0.f; sh.alpha[b] = 0.f; sh.aprev[b] = 0.f;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) { int any = 0; for (int b = 0; b < batch; ++b) any |= sh.cont[b]; *sh.any_cont = any; }
-    __syncthreads();
+    cg_start(sh, a.prm, batch);
 
+    // one-sweep CG: d_k lives in D[k % 3]: pass k reads d_k and d_{k-1} with halos while other CTAs write d_{k+1}.  a.r holds r_0 only.
+    float* const D[3] = {a.d0, a.d1, A.d2};
     if constexpr (FUSED) {
         static_assert(DIM == 3 && !GENERIC && !DIST && !ADAPT && OP == CgOp::Poisson, "the one-sweep CG is 3-D, branch-free, single-GPU CG only");
-        // d_k lives in D[k % 3]: pass k reads d_k and d_{k-1} with halos while other CTAs write d_{k+1}.  a.r holds r_0 only.
-        float* const D[3] = {a.d0, a.d1, A.d2};
         float* const tile = rg.stage0 + (size_t)cfg.R * cfg.stage_floats;
         FusedGroups fg;
         fused_groups_init(fg, cfg, g, a.pf);
@@ -1428,14 +1297,7 @@ k_cg_ring(CgRingArgs A)
             for (int b = threadIdx.x; b < batch; b += blockDim.x) {
                 if (!sh.cont[b]) continue;
                 const double dn = sh.sum1[b], dq = sh.sum0[b];
-                sh.delta[b] = dn;
-                const int it = ++sh.iters[b];
-                const float rsq = fabsf((float)dn);
-                const bool conv = rsq <= sh.tol_sq[b];
-                const bool divg = !isfinite(rsq) || (rsq / sh.rsq0[b] > 1e5f && it >= 8);
-                sh.conv[b] = conv; sh.divg[b] = divg;
-                sh.cont[b] = (!conv && !divg && it < a.prm.max_iter) ? 1 : 0;
-                if (sh.cont[b]) {                    // an entry that stops keeps alpha_k: the x step it may still owe
+                if (cg_iteration_done(sh, a.prm, b, dn)) {       // an entry that stops keeps alpha_k: the x step it may still owe
                     sh.aprev[b] = sh.alpha[b];
                     sh.bprev[b] = sh.beta[b];
                     sh.alpha[b] = (dq != 0.0) ? (float)(dn / dq) : 0.f;
@@ -1449,26 +1311,10 @@ k_cg_ring(CgRingArgs A)
                 const double nxt = dn - 2.0 * al * sh.sum0[b] + al * al * sh.sum1[b];
                 sh.beta[b] = (dn != 0.0) ? (float)(nxt / dn) : 0.f;
             }
-            __syncthreads();
-            if (threadIdx.x == 0) { int any = 0; for (int b = 0; b < batch; ++b) any |= sh.cont[b]; *sh.any_cont = any; }
-            __syncthreads();
+            cg_count_running(sh, batch);
             reg ^= 1;
         }
         region = reg == 1 ? 2 : 0;                   // 2-sum slots that the last pass F did not use
-        // entries that stopped after an odd number of iterations still owe x the step alpha_k d_k of their last pass k
-        RingUnit u;
-        for (int k = 0; ring_next_unit<DIM>(cfg, g, k, u); ++k) {
-            const int it = sh.iters[u.b];
-            if (!(it & 1)) continue;
-            const float al = sh.alpha[u.b];
-            const float* dl = D[(it - 1) % 3];
-            ring_unit_cells<DIM>(cfg, g, a.pf, tg, u, [&](long long off, int) {
-                float4 xv = *reinterpret_cast<const float4*>(a.x + off);
-                const float4 dv = *reinterpret_cast<const float4*>(dl + off);
-                xv.x += al * dv.x; xv.y += al * dv.y; xv.z += al * dv.z; xv.w += al * dv.w;
-                *reinterpret_cast<float4*>(a.x + off) = xv;
-            });
-        }
     }
 
     // a.prm.method == PHI_SOLVER_CG_ADAPTIVE (_linalg.py:93-128) reuses both passes: pass A forms d' = r - c d (beta = -c) and
@@ -1477,29 +1323,13 @@ k_cg_ring(CgRingArgs A)
     float* lo_dnew = cm.lo_d1; float* hi_dnew = cm.hi_d1; float* lo_dold = cm.lo_d0; float* hi_dold = cm.hi_d0;
     bool x_pending = false;      // all running entries are at the same iteration, so one flag describes them all
     while (!FUSED && *sh.any_cont && comm_ok) {
-        if (cfg.dbg & 1) {} else if constexpr (!ADAPT) {   // pass A
-            const float* hsrc[3] = {a.r, dold, (OP == CgOp::Masked ? a.acc : (OP == CgOp::HelmholtzVarying ? A.op.k : nullptr))};
-            const float* esrc[2] = {nullptr, nullptr};
+        {   // pass A; CG-adaptive also sums d'.r (r once more, element-wise)
+            const float* hsrc[3] = {a.r, dold, xsrc};
+            const float* esrc[2] = {ADAPT ? a.r : nullptr, nullptr};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
-                REpiPassA<PH> epi{dnew, 0.f, 0.f, peer_halo(lo_dnew, hi_dnew)};
-                if constexpr (OP == CgOp::Poisson) ring_process_unit<GENERIC, DIM, 2, 0>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, epi);
-                else cg_op_unit<DIM, GENERIC, OP, 2, 0>(rg, A, tg, hsrc, esrc, sh.beta[u.b], u, epi);
-                acc0 += epi.acc0; acc1 += epi.acc1;
-            });
-        } else if constexpr (OP == CgOp::Poisson) { // pass A of CG-adaptive: additionally d'.r (r once more, element-wise)
-            const float* hsrc[2] = {a.r, dold};
-            const float* esrc[2] = {a.r, nullptr};
-            sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
-                REpiPassAAdapt<PH> epi{dnew, 0.f, 0.f, peer_halo(lo_dnew, hi_dnew)};
-                ring_process_unit<GENERIC, DIM, 2, 1>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, epi);
-                acc0 += epi.acc0; acc1 += epi.acc1;
-            });
-        } else {                                    // the same with obstacles: the mask in the haloed slot after r and dold
-            const float* hsrc[3] = {a.r, dold, a.acc};
-            const float* esrc[2] = {a.r, nullptr};
-            sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
-                REpiPassAAdapt<PH> epi{dnew, 0.f, 0.f, peer_halo(lo_dnew, hi_dnew)};
-                cg_op_unit<DIM, GENERIC, OP, 2, 1>(rg, A, tg, hsrc, esrc, sh.beta[u.b], u, epi);
+                REpiPassA<PH, ADAPT> epi{dnew, 0.f, 0.f, peer_halo(lo_dnew, hi_dnew)};
+                if constexpr (OP == CgOp::Poisson) ring_process_unit<GENERIC, DIM, 2, ADAPT ? 1 : 0>(rg, cfg, g, a.pf, tg, hsrc, esrc, sh.beta[u.b], u, epi);
+                else cg_op_unit<DIM, GENERIC, OP, 2, ADAPT ? 1 : 0>(rg, A, tg, hsrc, esrc, sh.beta[u.b], u, epi);
                 acc0 += epi.acc0; acc1 += epi.acc1;
             });
         }
@@ -1520,8 +1350,8 @@ k_cg_ring(CgRingArgs A)
             sh.offs[b] = coffs * (float)S;
         }
         __syncthreads();
-        if (cfg.dbg & 2) {} else if (!x_pending) {   // pass B, odd iteration: r only, the x update is deferred
-            const float* hsrc[2] = {dnew, (OP == CgOp::Masked ? a.acc : (OP == CgOp::HelmholtzVarying ? A.op.k : nullptr))};
+        if (!x_pending) {                           // pass B, odd iteration: r only, the x update is deferred
+            const float* hsrc[2] = {dnew, xsrc};
             const float* esrc[3] = {a.r, nullptr, nullptr};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
                 REpiPassBr<PH, ADAPT> epi{a.r, sh.alpha[u.b], ADAPT ? 0.f : sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
@@ -1530,7 +1360,7 @@ k_cg_ring(CgRingArgs A)
                 acc0 += epi.acc0; if (ADAPT) acc1 += epi.acc1;
             });
         } else {            // pass B, even iteration: x += alpha_prev d_prev + alpha d
-            const float* hsrc[2] = {dnew, (OP == CgOp::Masked ? a.acc : (OP == CgOp::HelmholtzVarying ? A.op.k : nullptr))};
+            const float* hsrc[2] = {dnew, xsrc};
             const float* esrc[3] = {a.x, a.r, dold};
             sweep(sh.cont, [&](const RingUnit& u, float& acc0, float& acc1) {
                 REpiPassB<PH, ADAPT> epi{a.x, a.r, sh.alpha[u.b], sh.aprev[u.b], ADAPT ? 0.f : sh.offs[u.b], 0.f, 0.f, peer_halo(cm.lo_r, cm.hi_r)};
@@ -1548,34 +1378,30 @@ k_cg_ring(CgRingArgs A)
             // CG: d' = r + (|r'|^2 / |r|^2) d;  CG-adaptive: d' = r - ((r.Ad) / (d.Ad)) d  (_linalg.py:120)
             if (adaptive) sh.beta[b] = (dprev != 0.0) ? -(float)(sh.sum1[b] / dprev) : 0.f;
             else sh.beta[b] = (dprev != 0.0) ? (float)(dn / dprev) : 0.f;
-            sh.delta[b] = dn;
-            const int it = ++sh.iters[b];
-            const float rsq = fabsf((float)dn);
-            const bool conv = rsq <= sh.tol_sq[b];
-            const bool divg = !isfinite(rsq) || (rsq / sh.rsq0[b] > 1e5f && it >= 8);
-            sh.conv[b] = conv; sh.divg[b] = divg;
-            sh.cont[b] = (!conv && !divg && it < a.prm.max_iter) ? 1 : 0;
+            cg_iteration_done(sh, a.prm, b, dn);
         }
-        __syncthreads();
-        if (threadIdx.x == 0) { int any = 0; for (int b = 0; b < batch; ++b) any |= sh.cont[b]; *sh.any_cont = any; }
-        __syncthreads();
+        cg_count_running(sh, batch);
         float* t = dold; dold = dnew; dnew = t;
         t = lo_dold; lo_dold = lo_dnew; lo_dnew = t;
         t = hi_dold; hi_dold = hi_dnew; hi_dnew = t;
     }
 
-    // entries that stopped after an odd number of iterations still owe x their last step; odd iterations write d1
+    // entries that stopped after an odd number of iterations still owe x the step alpha d of their last iteration, whose direction
+    // is in d1 (two sweeps: odd iterations write d1) or D[(it - 1) % 3] (pass F).  Pass F tiles hold whole float4 groups; keeping the
+    // partial-group path out of the one-sweep kernel keeps its register allocation (24 B more spill loads with it).
     RingUnit u;
-    for (int k = 0; !FUSED && ring_next_unit<DIM>(cfg, g, k, u); ++k) {
-        if (!(sh.iters[u.b] & 1)) continue;
+    for (int k = 0; ring_next_unit<DIM>(cfg, g, k, u); ++k) {
+        const int it = sh.iters[u.b];
+        if (!(it & 1)) continue;
         const float al = sh.alpha[u.b];
+        const float* dl = FUSED ? D[(it - 1) % 3] : a.d1;
         ring_unit_cells<DIM>(cfg, g, a.pf, tg, u, [&](long long off, int nvalid) {
-            if (nvalid == 4) {
+            if (FUSED || nvalid == 4) {
                 float4 xv = *reinterpret_cast<const float4*>(a.x + off);
-                const float4 dv = *reinterpret_cast<const float4*>(a.d1 + off);
+                const float4 dv = *reinterpret_cast<const float4*>(dl + off);
                 xv.x += al * dv.x; xv.y += al * dv.y; xv.z += al * dv.z; xv.w += al * dv.w;
                 *reinterpret_cast<float4*>(a.x + off) = xv;
-            } else for (int j = 0; j < nvalid; ++j) a.x[off + j] += al * a.d1[off + j];
+            } else for (int j = 0; j < nvalid; ++j) a.x[off + j] += al * dl[off + j];
         });
     }
 
@@ -1587,7 +1413,7 @@ k_cg_ring(CgRingArgs A)
         });
         barrier_and_reduce(nullptr);
         for (int k = 0; ring_next_unit<DIM>(cfg, g, k, u); ++k) {
-            const float m = MASK ? (sh.sum1[u.b] > 0.0 ? (float)(sh.sum0[u.b] / sh.sum1[u.b]) : 0.f) : (float)(sh.sum0[u.b] / cells);
+            const float m = cg_projection_mean<MASK>(sh, u.b, cells);
             ring_unit_cells<DIM>(cfg, g, a.pf, tg, u, [&](long long off, int nvalid) {
                 for (int j = 0; j < nvalid; ++j) a.x[off + j] -= MASK ? m * a.acc[off + j] : m;
             });
@@ -1595,14 +1421,7 @@ k_cg_ring(CgRingArgs A)
     }
 
     if (cm.n > 1 && blockIdx.x == 0 && threadIdx.x == 0) *cm.seq = seq;
-    if (blockIdx.x == 0) {
-        for (int b = threadIdx.x; b < batch; b += blockDim.x) {
-            PhiCgResult res;
-            res.iterations = sh.iters[b]; res.converged = sh.conv[b]; res.diverged = comm_ok ? sh.divg[b] : -1;
-            res.residual_sq = fabsf((float)sh.delta[b]); res.tol_sq = sh.tol_sq[b]; res.initial_residual_sq = sh.rsq0[b];
-            a.result[b] = res;
-        }
-    }
+    cg_write_result(sh, a.result, batch, comm_ok);
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------------
@@ -1643,9 +1462,6 @@ static bool ring_config(const DGrid& g, int lines_a, int lines_b, int reserve_by
     while (g.dim == 2 && c.TY > 1 && c.TY / 2 >= g.n[1]) c.TY /= 2;
     c.groups = (c.TY * c.nx4 + consumers - 1) / consumers;
     c.shfl_ok = (c.nx4 % 32 == 0) ? 1 : 0;
-    { const char* e = getenv("PHICUDA_RING_HINT"); c.hint = (e && e[0] == '1') ? 1 : 0; }
-    { const char* e = getenv("PHICUDA_RING_MERGE"); c.merge = (e && e[0] == '0') ? 0 : 1; }
-    { const char* e = getenv("PHICUDA_RING_DEBUG"); c.dbg = e ? atoi(e) : 0; }
     if (g.dim == 3) {
         c.nyt = (g.n[1] + c.TY - 1) / c.TY;
         // z chunking: every unit pays two halo planes plus a pipeline start (~2.5 plane loads, RING_UNIT_OVERHEAD), and
@@ -1847,8 +1663,6 @@ int phi_launch_cg_ring(const CgLaunch& l, const CommDev* cm, cudaStream_t s)
     A.op = l.op;
     a.result = l.result; a.prm = l.prm;
     if (cm) A.cm = *cm; else { memset(&A.cm, 0, sizeof(A.cm)); A.cm.n = 1; A.cm.lower = A.cm.upper = -1; }
-    // grid.sync + block-0 send is the default multi-GPU barrier; PHICUDA_COMM_MERGE=1 selects the merged barrier
-    { const char* e = getenv("PHICUDA_COMM_MERGE"); A.comm_merge = (e && e[0] == '1') ? 1 : 0; }
     void* args[] = {&A};
     e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(threads), args, smem, s);
     if (e != cudaSuccess) { phi_set_error("cg ring: cooperative launch failed: %s", cudaGetErrorString(e)); return (int)e; }
