@@ -114,6 +114,7 @@ int         phicuda_device_info(char* name, size_t name_len, int* sm_count, int*
 #define PHI_KERNEL_CG_RING       3   /* k_cg_ring       (persistent, TMA ring) */
 #define PHI_KERNEL_CG_MARCH      4   /* k_cg_poisson    (persistent, register marching) */
 #define PHI_KERNEL_STENCIL_RING  5   /* k_div_ring / k_gradsub_ring / k_advect_ring: see `stencil` */
+#define PHI_KERNEL_RD_RING       6   /* k_rd_ring       (persistent, TMA ring): phicuda_reaction_diffusion_f32 */
 typedef struct PhiLaunchInfo {
     int32_t kernel;        /* PHI_KERNEL_* */
     int32_t generic;       /* 1: variant with per-tile boundary handling, 0: branch-free variant (every tile qualifies) */
@@ -315,6 +316,22 @@ int phicuda_plume_step_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const Phi
                                   const float* inflow, const float* accessible, const float* const face_factors[3],
                                   const PhiPlumeParams* sp, const PhiCgParams* prm, PhiCgResult* result,
                                   float* scratch, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- N7  reaction-diffusion: the Reaction_Diffusion notebook's Gray-Scott step --------------------------------------------
+ * `substeps` times, on centred arrays u and v of the grid (every batch entry with the same parameters):
+ *   uvv = u * v**2;  su = du * laplace(u) - uvv + f * (1 - u);  sv = dv * laplace(v) + uvv - (f + k) * v;
+ *   u = u + dt * su;  v = v + dt * sv
+ * laplace as phicuda_laplace_f32, ghost cells of u from bc->comp[0] and of v from bc->comp[1].  Every operation is rounded as the
+ * reference's float32 field arithmetic rounds it.  Boundaries: PERIODIC, ZERO_GRADIENT and constant 0 per side, the same kinds for u
+ * and v - the extrapolations that the reference's step maps to themselves; a non-zero constant becomes 2c - c^2 after one step
+ * and returns PHI_ERR_UNSUPPORTED.  The update is in place and the call never allocates: all substeps run in one persistent
+ * kernel (PHI_KERNEL_RD_RING), 16 B/cell per substep (+ 16 B/cell once for an odd count), state ping-ponging through `scratch`
+ * (phicuda_reaction_diffusion_scratch_bytes).  substeps == 0 leaves u and v untouched.  Single GPU, no z-slabs; grid lines that do
+ * not fit the ring return PHI_ERR_UNSUPPORTED with the widest line that does.  Every argument check runs before the first CUDA
+ * call: a refused call leaves u and v untouched. */
+size_t phicuda_reaction_diffusion_scratch_bytes(const PhiGrid* g);
+int phicuda_reaction_diffusion_f32(const PhiGrid* g, const PhiVBC* bc, float* u, float* v, float du, float dv, float f, float k,
+                                   float dt, int32_t substeps, float* scratch, size_t scratch_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -43,7 +43,7 @@ class PhiLaunchInfo(C.Structure):
                                          'total_units', 'grid_ctas', 'split')]
 
 
-KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING = range(6)
+KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING, KERNEL_RD_RING = range(7)
 
 
 class PhiPlumeParams(C.Structure):
@@ -108,6 +108,9 @@ PROTOTYPES = {
     'phicuda_plume_step_masked_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiBC), F3, C.c_void_p, C.c_void_p, C.c_void_p,
                                                 C.c_void_p, F3, _P(PhiPlumeParams), _P(PhiCgParams), C.c_void_p, C.c_void_p,
                                                 C.c_void_p, C.c_size_t, C.c_void_p]),
+    'phicuda_reaction_diffusion_scratch_bytes': (C.c_size_t, [_P(PhiGrid)]),
+    'phicuda_reaction_diffusion_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float,
+                                                 C.c_float, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 

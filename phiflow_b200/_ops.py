@@ -439,6 +439,26 @@ def diffuse_implicit_varying(dom: Domain, spec, u, k, dt: float, rtol=1e-5, atol
     return x
 
 
+def reaction_diffusion(dom: Domain, spec, u, v, du: float, dv: float, f: float, k: float, dt: float, substeps: int = 1):
+    """`substeps` Gray-Scott substeps of the Reaction_Diffusion notebook in one launch (include/phicuda.h, N7):
+    uvv = u * v**2, u += dt * (du * laplace(u) - uvv + f * (1 - u)), v += dt * (dv * laplace(v) + uvv - (f + k) * v).
+    u, v: centred arrays of `dom`; spec: one boundary spec for both, or [spec_u, spec_v] (same kinds, constants 0).
+    Returns new arrays (u', v'); the inputs are not modified and may be the same tensor."""
+    require_cuda()
+    assert dom.halo == 0, "reaction-diffusion is not offered on z-slabs"
+    shape = dom._shape(dom.cext)
+    assert tuple(u.shape) == shape and tuple(v.shape) == shape, f"u, v: shapes {tuple(u.shape)}, {tuple(v.shape)} are not centred arrays of the domain"
+    un, vn = u.clone(), v.clone()
+    if getattr(dom, '_rd_scratch', None) is None:
+        n = _lib.load().phicuda_reaction_diffusion_scratch_bytes(C.byref(dom.grid))
+        dom._rd_scratch = torch.empty(n // 4, dtype=torch.float32, device=dom.device)
+    s = dom._rd_scratch
+    _lib.check(_lib.load().phicuda_reaction_diffusion_f32(C.byref(dom.grid), C.byref(make_vbc(spec, 2)), _ptr(un), _ptr(vn), C.c_float(du),
+                                                          C.c_float(dv), C.c_float(f), C.c_float(k), C.c_float(dt), C.c_int32(substeps),
+                                                          _ptr(s), C.c_size_t(4 * s.numel()), _stream()))
+    return un, vn
+
+
 def mul_faces(dom: Domain, vbc, v, mask):
     """v_c *= mask_c on the stored faces (apply_boundary_conditions for stationary obstacles, fluid.py:212-240)."""
     require_cuda()

@@ -679,4 +679,54 @@ int phicuda_plume_step_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const Phi
     return plume_step(g, vbc, sbc, v, s, p, inflow, accessible, face_factors, sp, prm, result, scratch, workspace, workspace_bytes, stream);
 }
 
+size_t phicuda_reaction_diffusion_scratch_bytes(const PhiGrid* g)
+{
+    return g ? 2 * centred_elems(g) * sizeof(float) : 0;
+}
+
+int phicuda_reaction_diffusion_f32(const PhiGrid* g, const PhiVBC* bc, float* u, float* v, float du, float dv, float f, float k,
+                                   float dt, int32_t substeps, float* scratch, size_t scratch_bytes, void* stream)
+{
+    // every check runs before the first CUDA call: a refused call leaves u and v untouched
+    DGrid dg; DField fu, fv;
+    CHECK(phi_make_dgrid(g, &dg));
+    if (!bc || !u || !v || !scratch) { phi_set_error("reaction_diffusion: NULL argument"); return PHI_ERR_INVALID; }
+    if (substeps < 0) { phi_set_error("reaction_diffusion: substeps must be >= 0, got %d", substeps); return PHI_ERR_INVALID; }
+    if (!std::isfinite(du) || !std::isfinite(dv) || !std::isfinite(f) || !std::isfinite(k) || !std::isfinite(dt)) {
+        phi_set_error("reaction_diffusion: du, dv, f, k and dt must be finite"); return PHI_ERR_INVALID;
+    }
+    const size_t n = centred_elems(g);
+    const size_t need = phicuda_reaction_diffusion_scratch_bytes(g);
+    if (scratch_bytes < need) { phi_set_error("reaction_diffusion: scratch %zu < %zu bytes", scratch_bytes, need); return PHI_ERR_INVALID; }
+    auto overlap = [](const float* a, size_t na, const float* b, size_t nb) { return a < b + nb && b < a + na; };
+    if (overlap(u, n, v, n)) { phi_set_error("reaction_diffusion: u and v must be distinct arrays (they overlap)"); return PHI_ERR_INVALID; }
+    if (overlap(scratch, 2 * n, u, n) || overlap(scratch, 2 * n, v, n)) {
+        phi_set_error("reaction_diffusion: scratch overlaps u or v"); return PHI_ERR_INVALID;
+    }
+    if (g->halo != 0) { phi_set_error("reaction_diffusion: z-slab grids are not supported"); return PHI_ERR_UNSUPPORTED; }
+    CHECK(phi_make_centered(g, &bc->comp[0], &fu)); CHECK(phi_make_centered(g, &bc->comp[1], &fv));
+    for (int a = 0; a < g->dim; ++a) {
+        if (bc->comp[0].lo[a] != bc->comp[1].lo[a] || bc->comp[0].hi[a] != bc->comp[1].hi[a]) {
+            phi_set_error("reaction_diffusion: the boundary kinds of u and v must agree (axis %d)", a); return PHI_ERR_UNSUPPORTED;
+        }
+        for (int c = 0; c < 2; ++c)
+            if ((bc->comp[c].lo[a] == PHI_BC_CONST && bc->comp[c].clo[a] != 0.f) || (bc->comp[c].hi[a] == PHI_BC_CONST && bc->comp[c].chi[a] != 0.f)) {
+                phi_set_error("reaction_diffusion: non-zero constant boundary on axis %d of %s: the reference's step turns a constant c into "
+                              "2c - c^2 (field (-) number keeps the field's extrapolation), so its ghosts are not fixed", a, c ? "v" : "u");
+                return PHI_ERR_UNSUPPORTED;
+            }
+    }
+    if (!phi_ring_enabled()) { phi_set_error("reaction_diffusion: runs on the TMA ring kernel only, which PHICUDA_NO_RING switches off"); return PHI_ERR_UNSUPPORTED; }
+    if (!phi_rd_ring_fits(dg)) {
+        phi_set_error("reaction_diffusion: grid lines of %d cells do not fit the TMA ring (%d-D: at most %d cells)", g->n[0], g->dim, phi_rd_ring_max_width(dg));
+        return PHI_ERR_UNSUPPORTED;
+    }
+    if (substeps == 0) return 0;
+    RdParams p;
+    p.du = du; p.dv = dv; p.f = f; p.fk = f + k; p.dt = dt;
+    const int e = phi_launch_reaction_diffusion(dg, fu, u, v, scratch, scratch + n, p, substeps, (cudaStream_t)stream);
+    if (e == -100) { phi_set_error("reaction_diffusion: the grid does not fit the TMA ring on this device"); return PHI_ERR_UNSUPPORTED; }
+    return cuda_fail(e, "reaction_diffusion");
+}
+
 }  // extern "C"

@@ -93,3 +93,9 @@ bool phi_cg_ring_fits(const DGrid& g, CgOp op);
 // widest grid line the ring CG takes for g's other extents and batch (host-only; error messages of refused solves)
 int phi_cg_ring_max_width(const DGrid& g, CgOp op, bool adapt);
 int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField* cf, cudaStream_t s);
+// N7 reaction-diffusion on the TMA ring (ring_kernels.cu).  fk = f + k, rounded to float once.  -100: the grid does not fit the ring.
+struct RdParams { float du, dv, f, fk, dt; };
+bool phi_rd_ring_fits(const DGrid& g);                 // host-only, no CUDA call
+int phi_rd_ring_max_width(const DGrid& g);             // widest line (cells) the ring takes for g's other extents; host-only
+int phi_launch_reaction_diffusion(const DGrid& g, const DField& f, float* u, float* v, float* su, float* sv, const RdParams& p,
+                                  int substeps, cudaStream_t s);

@@ -274,6 +274,33 @@ __device__ __forceinline__ void groups_tile(ThreadGroups& tg, const RingCfg& cfg
     }
 }
 
+// Epilogues that declare kTwoFields (reaction-diffusion, N7) take the two haloed arrays of a stage as two fields: ring_compute_any
+// runs the consumer once per field (field 1 on the stage pointers moved by one haloed array), tells the epilogue the field and the
+// group k of each call, and both consumers form the stencil with stencil_ref - so a cell's bits do not depend on the consumer, the
+// tile or the variant that computed it.
+template <class E, class = void> struct RingTwoFields : std::false_type {};
+template <class E> struct RingTwoFields<E, std::void_t<decltype(E::kTwoFields)>> : std::integral_constant<bool, E::kTwoFields> {};
+
+// sum over axes of (lower + upper - 2 c) / dx^2 in oracle_np.laplace's order, each operation rounded on its own (no contraction)
+__device__ __forceinline__ float lap_axis(float lo, float hi, float c, float idx2)
+{ return __fmul_rn(__fsub_rn(__fadd_rn(lo, hi), __fmul_rn(2.f, c)), idx2); }
+template <int DIM>
+__device__ __forceinline__ float lap_ref(float c, float l, float r, float ym, float yp, float zm, float zp, float ix2, float iy2, float iz2)
+{
+    const float s = __fadd_rn(lap_axis(l, r, c, ix2), lap_axis(ym, yp, c, iy2));
+    return DIM == 3 ? __fadd_rn(s, lap_axis(zm, zp, c, iz2)) : s;
+}
+// l4 / r4: the x-1 / x+1 neighbours of the four cells
+template <int DIM>
+__device__ __forceinline__ float4 stencil_ref(const float4& c, const float4& l4, const float4& r4, const float4& ym, const float4& yp,
+                                              const float4& zm, const float4& zp, float ix2, float iy2, float iz2)
+{
+    return make_float4(lap_ref<DIM>(c.x, l4.x, r4.x, ym.x, yp.x, zm.x, zp.x, ix2, iy2, iz2),
+                       lap_ref<DIM>(c.y, l4.y, r4.y, ym.y, yp.y, zm.y, zp.y, ix2, iy2, iz2),
+                       lap_ref<DIM>(c.z, l4.z, r4.z, ym.z, yp.z, zm.z, zp.z, ix2, iy2, iz2),
+                       lap_ref<DIM>(c.w, l4.w, r4.w, ym.w, yp.w, zm.w, zp.w, ix2, iy2, iz2));
+}
+
 // ---- consumer: one plane of one tile ---------------------------------------------------------------------------------
 // sm/sc/sp: stages holding planes z-1, z, z+1 (sm/sp unused in 2-D).  Values of the differenced array are h0 (+ beta*h1).
 // Operators with an extra haloed slot (cg_op_xslot) run the face-minimum stencil
@@ -386,6 +413,10 @@ __device__ __forceinline__ void ring_compute(const RingCfg& cfg, const DGrid& g,
                 if (ac.w == 0.f) q.w = c.w;
                 epi.set_acc(ac);
             }
+        } else if constexpr (RingTwoFields<Epi>::value) {
+            const float4 zm = DIM == 3 ? (zm_const ? f4_splat(pf.clo[2]) : val4(sm, rc)) : c;
+            const float4 zp = DIM == 3 ? (zp_const ? f4_splat(pf.chi[2]) : val4(sp, rc)) : c;
+            q = stencil_ref<DIM>(c, make_float4(xl, c.x, c.y, c.z), r4, ym, yp, zm, zp, ix2, iy2, iz2);
         } else {
         q.x = (xl + r4.x - 2.f * c.x) * ix2 + (ym.x + yp.x - 2.f * c.x) * iy2;
         q.y = (c.x + r4.y - 2.f * c.y) * ix2 + (ym.y + yp.y - 2.f * c.y) * iy2;
@@ -404,6 +435,7 @@ __device__ __forceinline__ void ring_compute(const RingCfg& cfg, const DGrid& g,
         if (NE >= 1) e0 = *reinterpret_cast<const float4*>(sc + e0off + tg.eoff[k]);
         if (NE >= 2) e1 = *reinterpret_cast<const float4*>(sc + e1off + tg.eoff[k]);
         if (NE >= 3) e2 = *reinterpret_cast<const float4*>(sc + e1off + cfg.TY * pitch + tg.eoff[k]);
+        if constexpr (RingTwoFields<Epi>::value) epi.k = k;
         epi(plane_off + tg.goff[k], c, q, nvalid, e0, e1, e2);
     }
 }
@@ -451,6 +483,10 @@ __device__ __forceinline__ void ring_compute_fast(const RingCfg& cfg, const DGri
             if (tg.needr & (1u << k)) { xr = sc[tg.xro[k]]; if (use1) xr = fmaf(beta, sc[h1 + tg.xro[k]], xr); }
         }
         float4 q;
+        if constexpr (RingTwoFields<Epi>::value) {
+            const float4 zm = DIM == 3 ? val4(sm, rc) : c, zp = DIM == 3 ? val4(sp, rc) : c;
+            q = stencil_ref<DIM>(c, make_float4(xl, c.x, c.y, c.z), make_float4(c.y, c.z, c.w, xr), ym, yp, zm, zp, ix2, iy2, iz2);
+        } else {
         q.x = fmaf(ix2, xl + c.y, fmaf(iy2, ym.x + yp.x, -cc * c.x));
         q.y = fmaf(ix2, c.x + c.z, fmaf(iy2, ym.y + yp.y, -cc * c.y));
         q.z = fmaf(ix2, c.y + c.w, fmaf(iy2, ym.z + yp.z, -cc * c.z));
@@ -464,17 +500,19 @@ __device__ __forceinline__ void ring_compute_fast(const RingCfg& cfg, const DGri
             q.w = fmaf(iz2, zm.w + zp.w, q.w);
             if (MZ) { zs.m[k & 1] = c; zs.c[k & 1] = zp; }
         }
+        }
         float4 e0 = f4_splat(0.f), e1 = f4_splat(0.f), e2 = f4_splat(0.f);
         if (NE >= 1) e0 = *reinterpret_cast<const float4*>(sc + e0off + tg.eoff[k]);
         if (NE >= 2) e1 = *reinterpret_cast<const float4*>(sc + e1off + tg.eoff[k]);
         if (NE >= 3) e2 = *reinterpret_cast<const float4*>(sc + e1off + cfg.TY * pitch + tg.eoff[k]);
+        if constexpr (RingTwoFields<Epi>::value) epi.k = k;
         epi(plane_off + tg.goff[k], c, q, 4, e0, e1, e2);
     }
     zs.have = MARCH && DIM == 3 && G <= 2;
 }
 
 template <bool GENERIC, int DIM, int NH, int NE, bool MARCH, CgOp OP, class Epi>
-__device__ __forceinline__ void ring_compute_any(const RingCfg& cfg, const DGrid& g, const DField& pf, const ThreadGroups& tg,
+__device__ __forceinline__ void ring_compute_sel(const RingCfg& cfg, const DGrid& g, const DField& pf, const ThreadGroups& tg,
                                                  bool fast, const float* sm, const float* sc, const float* sp, float beta,
                                                  long long plane_off, int z, Epi& epi, ZMarch& zs, const CgOperator* od)
 {
@@ -486,6 +524,23 @@ __device__ __forceinline__ void ring_compute_any(const RingCfg& cfg, const DGrid
     }
     zs.have = false;
     if (GENERIC) ring_compute<DIM, NH, NE>(cfg, g, pf, tg, sm, sc, sp, beta, plane_off, z, epi, od);
+}
+
+template <bool GENERIC, int DIM, int NH, int NE, bool MARCH, CgOp OP, class Epi>
+__device__ __forceinline__ void ring_compute_any(const RingCfg& cfg, const DGrid& g, const DField& pf, const ThreadGroups& tg,
+                                                 bool fast, const float* sm, const float* sc, const float* sp, float beta,
+                                                 long long plane_off, int z, Epi& epi, ZMarch& zs, const CgOperator* od)
+{
+    if constexpr (RingTwoFields<Epi>::value) {
+        static_assert(NH == 2 && NE == 0 && !MARCH && OP == CgOp::Poisson, "two fields: both haloed arrays, nothing else staged");
+        const int h1 = (cfg.TY + 2) * cfg.pitch;
+        epi.field = 0;
+        ring_compute_sel<GENERIC, DIM, NH, NE, MARCH, OP>(cfg, g, pf, tg, fast, sm, sc, sp, 0.f, plane_off, z, epi, zs, od);
+        epi.field = 1;
+        ring_compute_sel<GENERIC, DIM, NH, NE, MARCH, OP>(cfg, g, pf, tg, fast, sm + h1, sc + h1, sp + h1, 0.f, plane_off, z, epi, zs, od);
+    } else {
+        ring_compute_sel<GENERIC, DIM, NH, NE, MARCH, OP>(cfg, g, pf, tg, fast, sm, sc, sp, beta, plane_off, z, epi, zs, od);
+    }
 }
 
 // ---- one unit: producer streams its planes, consumers march through them --------------------------------------------------
@@ -565,7 +620,7 @@ __device__ __forceinline__ void ring_process_unit(Ring& rg, const RingCfg& cfg, 
     constexpr bool XSLOT = cg_op_xslot(OP);
     const bool producer = (int)threadIdx.x >= cfg.consumers;
     if (producer) {
-        const int nh = (NH == 2 && beta == 0.f) ? 1 : NH;          // first CG iteration: d' = r, old direction not read
+        const int nh = (NH == 2 && beta == 0.f && !RingTwoFields<Epi>::value) ? 1 : NH;   // first CG iteration: d' = r, old direction not read
         ProdUnit pu;
         prod_unit_setup<DIM, OP == CgOp::HelmholtzVarying>(pu, cfg, g, pf, ((1u << nh) - 1u) | (XSLOT ? (1u << NH) : 0u), NH + (XSLOT ? 1 : 0), NE, hsrc, esrc, u.b, u.y0, kb);
         if (DIM == 3) {
@@ -583,8 +638,10 @@ __device__ __forceinline__ void ring_process_unit(Ring& rg, const RingCfg& cfg, 
     if (GENERIC) groups_tile(tg, cfg, g, pf, u.y0);      // also needed on fast tiles: planes with constant z ghosts take the slow path
     long long plane_off = (long long)u.b * pf.sb + (long long)u.y0 * pf.sy + (DIM == 3 ? (long long)u.z0 * pf.sz : 0);
     if (DIM == 3) {
-        // kernels that contain only the branch-free path pick the group count once per unit, not once per plane
-        if (!GENERIC && cfg.groups == 2) ring_consume_planes<GENERIC, NH, NE, MARCH, 2, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
+        // kernels that contain only the branch-free path pick the group count once per unit, not once per plane (two-field
+        // epilogues go through ring_compute_any, which runs the consumer once per field)
+        if constexpr (RingTwoFields<Epi>::value) ring_consume_planes<GENERIC, NH, NE, MARCH, 0, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
+        else if (!GENERIC && cfg.groups == 2) ring_consume_planes<GENERIC, NH, NE, MARCH, 2, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
         else if (!GENERIC && cfg.groups == 4) ring_consume_planes<GENERIC, NH, NE, MARCH, 4, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
         else if (!GENERIC) ring_consume_planes<GENERIC, NH, NE, MARCH, 1, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
         else ring_consume_planes<GENERIC, NH, NE, MARCH, 0, OP>(rg, cfg, g, pf, tg, tile_fast, beta, plane_off, u, epi, od);
@@ -1779,4 +1836,125 @@ int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField* cf, cuda
         m.rhs = yb;
     }
     return phi_launch_cg_ring(m, nullptr, s);
+}
+
+// ---- N7 reaction-diffusion (Gray-Scott, the Reaction_Diffusion notebook) ------------------------------------------------------
+// One substep of the notebook's step, per cell, in the reference's operation order (field arithmetic, one rounding per operation):
+//   uvv = u * v**2;  su = du * laplace(u) - uvv + f * (1 - u);  sv = dv * laplace(v) + uvv - (f + k) * v;  u' = u + dt su, v' = v + dt sv
+// u and v are staged as the two haloed arrays of one stage (same boundary kinds, zero constants: the ghosts of both fields are
+// fixed points of the reference's extrapolation arithmetic).  The consumer runs once per field (RingTwoFields): field 0 keeps u and
+// laplace(u) of each of the thread's groups in registers, field 1 forms both updates.  16 B/cell per substep.
+__device__ __forceinline__ void rd_cell(const RdParams& p, float u, float lu, float v, float lv, float& uo, float& vo)
+{
+    const float uvv = __fmul_rn(u, __fmul_rn(v, v));
+    const float su = __fadd_rn(__fsub_rn(__fmul_rn(p.du, lu), uvv), __fmul_rn(p.f, __fsub_rn(1.f, u)));
+    const float sv = __fsub_rn(__fadd_rn(__fmul_rn(p.dv, lv), uvv), __fmul_rn(p.fk, v));
+    uo = __fadd_rn(u, __fmul_rn(p.dt, su));
+    vo = __fadd_rn(v, __fmul_rn(p.dt, sv));
+}
+
+struct REpiReactionDiffusion {
+    static constexpr bool kTwoFields = true;
+    float* un; float* vn; RdParams p;
+    int field, k;                                  // set by the consumer before each call
+    float4 cu[RING_G], lu[RING_G];                 // u and laplace(u) of group k, field 0 -> field 1
+    __device__ __forceinline__ void set_plane(int, int) {}
+    __device__ __forceinline__ void set_acc(const float4&) {}
+    __device__ __forceinline__ void operator()(long long off, const float4& c, const float4& q, int nvalid, const float4&, const float4&, const float4&)
+    {
+        if (field == 0) { cu[k] = c; lu[k] = q; return; }
+        float4 a, b;
+        rd_cell(p, cu[k].x, lu[k].x, c.x, q.x, a.x, b.x);
+        rd_cell(p, cu[k].y, lu[k].y, c.y, q.y, a.y, b.y);
+        rd_cell(p, cu[k].z, lu[k].z, c.z, q.z, a.z, b.z);
+        rd_cell(p, cu[k].w, lu[k].w, c.w, q.w, a.w, b.w);
+        if (nvalid == 4) { *reinterpret_cast<float4*>(un + off) = a; *reinterpret_cast<float4*>(vn + off) = b; }
+        else for (int j = 0; j < nvalid; ++j) { un[off + j] = f4_get(a, j); vn[off + j] = f4_get(b, j); }
+    }
+};
+
+// All substeps of one call in one cooperative launch.  The state ping-pongs between (u, v) and the scratch (su, sv) so that the last
+// substep writes (u, v); an odd count first copies (u, v) into the scratch.  Between substeps: the generic-proxy stores of this
+// substep must be visible to the TMA (async proxy) loads of the next one, whose halo lines other CTAs wrote - the sequence k_cg_ring
+// uses between passes.
+template <int DIM, bool GENERIC>
+__global__ void __launch_bounds__(RING_THREADS, 1)
+k_rd_ring(DGrid g, DField f, RingCfg cfg, float* u, float* v, float* su, float* sv, RdParams p, int substeps)
+{
+    extern __shared__ __align__(128) unsigned char smem[];
+    Ring rg;
+    ring_init(rg, smem, cfg);
+    cg::grid_group grid = cg::this_grid();
+    ThreadGroups tg;
+    groups_init(tg, cfg, g, f);
+    auto barrier = [&] { fence_proxy_async(); grid.sync(); fence_proxy_async(); };
+    float* src[2] = {u, v};
+    float* dst[2] = {su, sv};
+    if (substeps & 1) {
+        for (int unit = blockIdx.x; unit < cfg.total_units; unit += gridDim.x)
+            ring_unit_cells<DIM>(cfg, g, f, tg, ring_unit<DIM>(cfg, g, unit), [&](long long off, int nvalid) {
+                for (int j = 0; j < nvalid; ++j) { su[off + j] = u[off + j]; sv[off + j] = v[off + j]; }
+            });
+        barrier();
+        src[0] = su; src[1] = sv; dst[0] = u; dst[1] = v;
+    }
+    for (int s = 0; s < substeps; ++s) {
+        const float* hsrc[2] = {src[0], src[1]};
+        const float* esrc[2] = {nullptr, nullptr};
+        REpiReactionDiffusion epi;
+        epi.un = dst[0]; epi.vn = dst[1]; epi.p = p;
+        for (int unit = blockIdx.x; unit < cfg.total_units; unit += gridDim.x)
+            ring_process_unit<GENERIC, DIM, 2, 0, false>(rg, cfg, g, f, tg, hsrc, esrc, 0.f, ring_unit<DIM>(cfg, g, unit), epi);
+        if (s + 1 < substeps) barrier();
+        float* t0 = src[0]; float* t1 = src[1];
+        src[0] = dst[0]; src[1] = dst[1]; dst[0] = t0; dst[1] = t1;
+    }
+}
+
+// stage = u and v with their halo lines: 2 TY + 4 lines; the whole shared memory, one CTA per SM (cooperative launch)
+static bool rd_ring_config(const DGrid& g, int target_units, RingCfg* c)
+{
+    return ring_config(g, 2, 4, 0, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, target_units, c);
+}
+
+int phi_rd_ring_max_width(const DGrid& g)
+{
+    if (g.halo != 0) return 0;
+    for (int w = g.cext[0] < 4096 ? g.cext[0] / 4 * 4 : 4096; w >= 4; w -= 4) {       // ty * nx4 <= RING_G * 256: no line beyond 4096
+        DGrid h = g; h.n[0] = w; h.cext[0] = w;
+        RingCfg c;
+        if (rd_ring_config(h, 1, &c)) return w;
+    }
+    return 0;
+}
+
+bool phi_rd_ring_fits(const DGrid& g)
+{
+    RingCfg c;
+    return g.halo == 0 && rd_ring_config(g, 1, &c);
+}
+
+int phi_launch_reaction_diffusion(const DGrid& g, const DField& f, float* u, float* v, float* su, float* sv, const RdParams& p,
+                                  int substeps, cudaStream_t s)
+{
+    const int sms = phi_sm_count();
+    RingCfg cfg;
+    if (!rd_ring_config(g, sms, &cfg)) return -100;
+    const size_t smem = 128 + (size_t)cfg.R * cfg.stage_floats * 4;
+    const bool generic = !ring_all_fast(g, f, cfg);
+    const void* fn = g.dim == 3 ? (generic ? (const void*)k_rd_ring<3, true> : (const void*)k_rd_ring<3, false>)
+                                : (generic ? (const void*)k_rd_ring<2, true> : (const void*)k_rd_ring<2, false>);
+    int per_sm = 0;
+    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, RING_THREADS, smem);
+    if (e != cudaSuccess) return (int)e;
+    if (per_sm < 1) return -100;
+    int grid = sms * per_sm;
+    if (grid > cfg.total_units) grid = cfg.total_units;
+    DGrid ga = g; DField fa = f; RdParams pa = p; int ns = substeps;
+    void* args[] = {&ga, &fa, &cfg, &u, &v, &su, &sv, &pa, &ns};
+    e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(RING_THREADS), args, smem, s);
+    if (e != cudaSuccess) { phi_set_error("reaction_diffusion: cooperative launch failed: %s", cudaGetErrorString(e)); return (int)e; }
+    note_ring_launch(PHI_KERNEL_RD_RING, cfg, generic, false, false, grid);
+    return 0;
 }

@@ -428,6 +428,17 @@ class CenteredGrid(_Grid):
 
     __rmul__ = __mul__
 
+    def __rsub__(self, other):
+        """number - field keeps the field's extrapolation (phi/field/_field.py:788-813)."""
+        return (self * -1.0) + other
+
+    def __neg__(self):
+        return self * -1.0
+
+    def __pow__(self, power):
+        _require(isinstance(power, numbers.Real) and not isinstance(power, bool), "a power other than a plain number")
+        return self.with_values(self.data ** float(power))
+
 
 class StaggeredGrid(_Grid):
     """StaggeredGrid(values, boundary, bounds, x=..., y=...)  (phi/field/_grid.py:89-176).
@@ -750,6 +761,37 @@ def _implicit_varying(fld, k, dt, solve: Solve):
 
 
 diffuse = SimpleNamespace(explicit=explicit, implicit=implicit)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# reaction-diffusion  (examples/grids/Reaction_Diffusion.ipynb)
+# ----------------------------------------------------------------------------------------------------------------------
+def _fixed_point_side(s):
+    """Sides whose extrapolation the step maps to itself: PhiML's field arithmetic keeps a field's own extrapolation when it is
+    combined with a number, so a constant c turns into 2c - c**2 after one step; only c = 0 stays."""
+    return s in ('periodic', 'zg') or (isinstance(s, float) and s == 0.0)
+
+
+def reaction_diffusion(u: CenteredGrid, v: CenteredGrid, du: float, dv: float, f: float, k: float, dt: float, substeps: int = 1):
+    """The Reaction_Diffusion notebook's Gray-Scott step, `substeps` times in one kernel launch:
+        uvv = u * v**2;  su = du * field.laplace(u) - uvv + f * (1 - u);  sv = dv * field.laplace(v) + uvv - (f + k) * v
+        return u + dt * su, v + dt * sv
+    with the rounding of the reference's float32 field arithmetic.  Returns new fields (u', v'); u and v are not modified and may be
+    the same field (the notebook passes u0, u0).  Boundaries: PERIODIC, ZERO_GRADIENT and ZERO per side, the same kinds for u and
+    v; a non-zero constant drifts under the reference's step and raises NotImplementedError."""
+    plain = lambda x: isinstance(x, numbers.Real) and not isinstance(x, bool)
+    _require(isinstance(u, CenteredGrid) and isinstance(v, CenteredGrid), "reaction-diffusion of non-centred fields")
+    _require(u.vector_scale is None and v.vector_scale is None, "reaction-diffusion of vector fields")
+    _require(u._same_grid(v), "reaction-diffusion of fields on different grids")
+    _require(all(plain(x) for x in (du, dv, f, k, dt)), "reaction-diffusion with Field / per-batch parameters")
+    _require(isinstance(substeps, int) and substeps >= 0, f"substeps = {substeps!r}")
+    su, sv = u.spec, v.spec
+    _require(all(_fixed_point_side(s) for spec in (su, sv) for ax in spec for s in ax),
+             f"reaction-diffusion with a non-zero constant boundary ({u.boundary}, {v.boundary}): the reference's step moves it to 2c - c**2")
+    _require(all(a == b or (not isinstance(a, str) and not isinstance(b, str)) for ax_u, ax_v in zip(su, sv) for a, b in zip(ax_u, ax_v)),
+             "reaction-diffusion with different boundary kinds for u and v")
+    un, vn = ops.reaction_diffusion(u.dom, [su, sv], u.data, v.data, float(du), float(dv), float(f), float(k), float(dt), substeps)
+    return u.with_values(un), v.with_values(vn)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
