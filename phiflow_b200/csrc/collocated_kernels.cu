@@ -10,8 +10,10 @@
 // Solve() = 'auto' = CG-adaptive (PhiML/phiml/backend/_linalg.py:93-128) is what converges on it; that is the solver here, with
 // the reference's rank-1 matrix_offset for rank-deficient systems (linear(), _linalg.py:784-789).
 //
-// This is NOT the tuned path (the north-star workloads are staggered): one thread per cell, four launches per iteration, dot
-// products through double atomics, the host reads the per-entry status every few iterations (the entry point is a `_host` call).
+// This is NOT the tuned path (the north-star workloads are staggered): one thread per cell, seven launches per iteration, the
+// host reads the per-entry status every few iterations (the entry point is a `_host` call).  Dot products are summed in double
+// in a fixed order - per block (warp butterflies, then the four warps in turn), then per entry over the blocks (k_co_reduce) -
+// so the same call gives the same bits every time and a batch entry's result does not depend on its neighbours.
 // It exists so that CenteredGrid velocities run on the GPU with the reference's semantics instead of falling through.
 #include "phi_internal.cuh"
 #include "launch.cuh"
@@ -20,7 +22,7 @@ struct CoVec { DField f[3]; const float* p[3]; };          // three centred arra
 struct CoOut { float* p[3]; };
 
 struct CoStatus {            // per batch entry, device memory
-    double dx_dy, dx_r, s_dx, rsq, r_dy;     // accumulators (zeroed by the kernel that consumes them last)
+    double dx_dy, dx_r, s_dx, rsq, r_dy;     // dot products, written by k_co_reduce
     float tol_sq, rsq0, last_rsq, pad_;
     int iterations, cont, converged, diverged;
 };
@@ -35,12 +37,34 @@ __device__ __forceinline__ bool co_index(const DGrid& g, int& b, int& x, int& y,
     return x < g.n[0] && y < g.n[1];
 }
 
-__device__ __forceinline__ void co_block_add(double* dst, double v)
+// Blocks of one batch entry: ceil(n_x / 128) x n_y x n_z (co_grid); this block's index among them.
+__device__ __forceinline__ int co_block_of_entry(const DGrid& g)
 {
-    // warp shuffle reduction, one atomic per warp
+    const int z = g.dim == 3 ? blockIdx.z % g.n[2] : 0;
+    return (z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+}
+
+// Block sums of N values in a fixed order (butterfly per warp, then warps 0..3 in turn), stored as this block's partials
+// part[k * slot + entry * nblk + block], k < N.  Every thread of the block must call it.
+template <int N>
+__device__ __forceinline__ void co_block_partials(const double (&v)[N], double* __restrict__ part, const DGrid& g, int bb, size_t slot)
+{
+    __shared__ double w[N][4];
+    double s[N];
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0 && v != 0.0) atomicAdd(dst, v);
+    for (int k = 0; k < N; ++k) {
+        s[k] = v[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
+        if ((threadIdx.x & 31) == 0) w[k][threadIdx.x >> 5] = s[k];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const int nblk = gridDim.x * gridDim.y * (g.dim == 3 ? g.n[2] : 1);
+        const size_t at = (size_t)bb * nblk + co_block_of_entry(g);
+#pragma unroll
+        for (int k = 0; k < N; ++k) part[k * slot + at] = ((w[k][0] + w[k][1]) + w[k][2]) + w[k][3];
+    }
 }
 
 // g_c = (p[i + e_c] - p[i - e_c]) / (2 dx_c), ghosts from pf.   SUB: v_c -= g_c (final correction) instead of storing g_c.
@@ -67,11 +91,12 @@ k_co_gradient(const __grid_constant__ DGrid g, const __grid_constant__ DField pf
 template <int DIM, int MODE>
 __global__ void __launch_bounds__(128)
 k_co_divergence(const __grid_constant__ DGrid g, const __grid_constant__ CoVec v, const __grid_constant__ DField cf, float* __restrict__ out,
-                const float* __restrict__ dir, const float* __restrict__ r, CoStatus* __restrict__ st)
+                const float* __restrict__ dir, const float* __restrict__ r, const CoStatus* __restrict__ st, double* __restrict__ part,
+                size_t slot)
 {
     int b, x, y, z;
     const bool in = co_index<DIM>(g, b, x, y, z);
-    double a0 = 0, a1 = 0, a2 = 0;
+    double a[3] = {0, 0, 0};
     const bool live = in && (MODE == 0 || st[b].cont);
     if (live) {
         float acc = 0.f;
@@ -84,39 +109,39 @@ k_co_divergence(const __grid_constant__ DGrid g, const __grid_constant__ CoVec v
         }
         const long long off = (long long)b * cf.sb + (long long)z * cf.sz + (long long)y * cf.sy + x;
         out[off] = acc;
-        if (MODE == 1) { const float d = dir[off]; a0 = (double)d * acc; a1 = (double)d * r[off]; a2 = d; }
+        if (MODE == 1) { const float d = dir[off]; a[0] = (double)d * acc; a[1] = (double)d * r[off]; a[2] = d; }
     }
     if (MODE == 1) {
-        // all threads of a block share b (one grid line per block row): reduce per warp
+        // all threads of a block share b (one grid line per block row)
         const int bb = (DIM == 3) ? blockIdx.z / g.n[2] : blockIdx.z;
-        co_block_add(&st[bb].dx_dy, a0); co_block_add(&st[bb].dx_r, a1); co_block_add(&st[bb].s_dx, a2);
+        co_block_partials<3>(a, part, g, bb, slot);
     }
 }
 
 // Element-wise pieces of the CG-adaptive iteration (_linalg.py:109-122); q = A dir + c * sum(dir) with c = matrix_offset.
-//   PHASE 0 (initial residual): r = y - q(x0); dir = r; accumulates |r|^2 and |y|^2
-//   PHASE 1: step = (dir.r) / (dir.q); x += step dir; r -= step q; accumulates |r|^2 and r.q
-//   PHASE 2: dir = r - ((r.q) / (dir.q)) dir; block 0 of every batch entry advances the iteration count and the stopping rule
+//   PHASE 0 (initial residual): r = y - q(x0); dir = r; block partials of |r|^2 and |y|^2
+//   PHASE 1: step = (dir.r) / (dir.q); x += step dir; r -= step q; block partials of |r|^2 and r.q
+//   PHASE 2: dir = r - ((r.q) / (dir.q)) dir  (k_co_control then advances the iteration count and the stopping rule)
 template <int DIM, int PHASE>
 __global__ void __launch_bounds__(128)
 k_co_update(const __grid_constant__ DGrid g, const __grid_constant__ DField cf, float* __restrict__ x, float* __restrict__ r, float* __restrict__ dir,
             const float* __restrict__ q, const float* __restrict__ y, float offset, CoStatus* __restrict__ st,
-            const float* __restrict__ means, const double* __restrict__ x0sums)
+            const float* __restrict__ means, const double* __restrict__ x0sums, double* __restrict__ part, size_t slot)
 {
     int b, xx, yy, zz;
     const bool in = co_index<DIM>(g, b, xx, yy, zz);
     const int bb = (DIM == 3) ? blockIdx.z / g.n[2] : blockIdx.z;
     const long long off = (long long)bb * cf.sb + (long long)zz * cf.sz + (long long)yy * cf.sy + xx;
     CoStatus& s = st[bb];
-    double a0 = 0, a1 = 0;
+    double a[2] = {0, 0};
     if (PHASE == 0) {
         if (in) {
             const float yv = y[off] - (means ? means[bb] : 0.f);
             const float rv = yv - (q[off] + offset * (float)x0sums[bb]);
             r[off] = rv; dir[off] = rv;
-            a0 = (double)rv * rv; a1 = (double)yv * yv;
+            a[0] = (double)rv * rv; a[1] = (double)yv * yv;
         }
-        co_block_add(&s.rsq, a0); co_block_add(&s.r_dy, a1);          // r_dy doubles as |y|^2 during set-up
+        co_block_partials<2>(a, part, g, bb, slot);                    // r_dy doubles as |y|^2 during set-up
         return;
     }
     if (!s.cont) return;
@@ -129,9 +154,9 @@ k_co_update(const __grid_constant__ DGrid g, const __grid_constant__ DField cf, 
             x[off] = x[off] + step * dir[off];
             const float rv = r[off] - step * qv;
             r[off] = rv;
-            a0 = (double)rv * rv; a1 = (double)rv * qv;
+            a[0] = (double)rv * rv; a[1] = (double)rv * qv;
         }
-        co_block_add(&s.rsq, a0); co_block_add(&s.r_dy, a1);
+        co_block_partials<2>(a, part, g, bb, slot);
         return;
     }
     // PHASE 2
@@ -152,29 +177,56 @@ __global__ void k_co_control(CoStatus* st, int batch, int phase, float rtol, flo
         s.converged = fabsf(rsq) <= s.tol_sq; s.diverged = !isfinite(rsq);
         s.iterations = 0;
         s.cont = (!s.converged && !s.diverged && max_iter > 0) ? 1 : 0;
-        s.rsq = 0; s.r_dy = 0; s.dx_dy = 0; s.dx_r = 0; s.s_dx = 0;
         return;
     }
     if (!s.cont) return;
-    if (phase == 1) { s.rsq = 0; s.r_dy = 0; return; }              // before PHASE 1 accumulates
-    // phase 2: after the direction update - the operator application that follows refills dx_dy, dx_r, s_dx
+    // phase 2: after the direction update
     const float rsq = fabsf((float)s.rsq);
     s.iterations += 1;
     s.converged = rsq <= s.tol_sq;
     s.diverged = !isfinite(rsq) || (rsq / s.rsq0 > 1e5f && s.iterations >= 8);
     s.cont = (!s.converged && !s.diverged && s.iterations < max_iter) ? 1 : 0;
     s.last_rsq = rsq;                  // residual_sq for the result record
-    s.dx_dy = 0; s.dx_r = 0; s.s_dx = 0;
 }
 
-__global__ void k_co_mean(const __grid_constant__ DGrid g, const __grid_constant__ DField cf, const float* __restrict__ a, double* __restrict__ sums)
+// One block per batch entry: sums the block partials of each of `nq` values in a fixed order (a strided pass per thread, then a
+// tree over the threads) into the entry's status fields (what = 0: dir.q, dir.r, sum(dir); 1: |r|^2, r.q or |y|^2) or into
+// sums[b] (what = 2).  running: skip entries that have stopped - their partials were not written.
+__global__ void __launch_bounds__(256) k_co_reduce(const double* __restrict__ part, size_t slot, int nblk, CoStatus* st, double* sums,
+                                                   int what, int running)
+{
+    const int b = blockIdx.x;
+    if (running && !st[b].cont) return;
+    const int nq = what == 0 ? 3 : (what == 1 ? 2 : 1);
+    __shared__ double red[3][256];
+    for (int k = 0; k < nq; ++k) {
+        const double* p = part + k * slot + (size_t)b * nblk;
+        double s = 0;
+        for (int j = threadIdx.x; j < nblk; j += blockDim.x) s += p[j];
+        red[k][threadIdx.x] = s;
+    }
+    __syncthreads();
+    for (int h = blockDim.x / 2; h > 0; h >>= 1) {
+        if (threadIdx.x < h) for (int k = 0; k < nq; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + h];
+        __syncthreads();
+    }
+    if (threadIdx.x != 0) return;
+    CoStatus& s = st[b];
+    if (what == 0)      { s.dx_dy = red[0][0]; s.dx_r = red[1][0]; s.s_dx = red[2][0]; }
+    else if (what == 1) { s.rsq = red[0][0]; s.r_dy = red[1][0]; }
+    else                sums[b] = red[0][0];
+}
+
+// block partials of sum(a) per batch entry
+__global__ void __launch_bounds__(128)
+k_co_sum(const __grid_constant__ DGrid g, const __grid_constant__ DField cf, const float* __restrict__ a, double* __restrict__ part)
 {
     int b, x, y, z;
     const bool in = g.dim == 3 ? co_index<3>(g, b, x, y, z) : co_index<2>(g, b, x, y, z);
     const int bb = (g.dim == 3) ? blockIdx.z / g.n[2] : blockIdx.z;
-    double v = 0;
-    if (in) v = a[(long long)bb * cf.sb + (long long)z * cf.sz + (long long)y * cf.sy + x];
-    co_block_add(&sums[bb], v);
+    double v[1] = {0};
+    if (in) v[0] = a[(long long)bb * cf.sb + (long long)z * cf.sz + (long long)y * cf.sy + x];
+    co_block_partials<1>(v, part, g, bb, 0);
 }
 
 __global__ void k_co_finish(const CoStatus* st, PhiCgResult* result, const double* sums, float* means, double cells, int batch, int what)
@@ -198,12 +250,14 @@ k_co_sub_mean(const __grid_constant__ DGrid g, const __grid_constant__ DField cf
 }
 
 static dim3 co_grid(const DGrid& g) { return dim3((g.n[0] + 127) / 128, g.n[1], g.n[2] * g.batch); }
+static int co_blocks_per_entry(const DGrid& g) { return (g.n[0] + 127) / 128 * g.n[1] * g.n[2]; }
 
 size_t phi_collocated_workspace_bytes(const DGrid& g)
 {
     const size_t arr = ((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float) + 255) / 256 * 256;
-    // r, dir, q, div, 3 gradient components + status + sums of div / of x0 + means
-    return 7 * arr + (size_t)g.batch * (sizeof(CoStatus) + 2 * sizeof(double) + sizeof(float)) + 1024;
+    // r, dir, q, div, 3 gradient components + block partials of up to 3 dot products + status + sums of div / of x0 + means
+    return 7 * arr + 3 * (size_t)g.batch * co_blocks_per_entry(g) * sizeof(double)
+         + (size_t)g.batch * (sizeof(CoStatus) + 2 * sizeof(double) + sizeof(float)) + 1024;
 }
 
 // Host-synchronising: reads the per-entry status every `poll` iterations.
@@ -216,7 +270,10 @@ int phi_make_incompressible_collocated(const DGrid& g, const DField vfields[3], 
     unsigned char* ws = (unsigned char*)workspace;
     float* r = (float*)ws; float* dir = (float*)(ws + arr); float* q = (float*)(ws + 2 * arr); float* div = (float*)(ws + 3 * arr);
     CoOut grad; for (int c = 0; c < 3; ++c) grad.p[c] = (float*)(ws + (4 + c) * arr);
-    CoStatus* st = (CoStatus*)(ws + 7 * arr);
+    const int nblk = co_blocks_per_entry(g);
+    const size_t slot = (size_t)g.batch * nblk;
+    double* part = (double*)(ws + 7 * arr);
+    CoStatus* st = (CoStatus*)(part + 3 * slot);
     double* sums = (double*)(st + g.batch);
     double* xsums = sums + g.batch;
     float* means = (float*)(xsums + g.batch);
@@ -230,29 +287,39 @@ int phi_make_incompressible_collocated(const DGrid& g, const DField vfields[3], 
     const bool d3 = g.dim == 3;
 #define CO_LAUNCH(K2, K3, ...) do { if (d3) K3<<<grid, block, 0, s>>>(__VA_ARGS__); else K2<<<grid, block, 0, s>>>(__VA_ARGS__); } while (0)
     // right-hand side: divergence of the input velocity, balanced when the system is rank deficient (fluid.py:145-148, 205-209)
-    CO_LAUNCH((k_co_divergence<2, 0>), (k_co_divergence<3, 0>), g, vin, cf, div, nullptr, nullptr, st);
+    CO_LAUNCH((k_co_divergence<2, 0>), (k_co_divergence<3, 0>), g, vin, cf, div, nullptr, nullptr, st, part, slot);
     if (balance) {
-        k_co_mean<<<grid, block, 0, s>>>(g, cf, div, sums);
+        k_co_sum<<<grid, block, 0, s>>>(g, cf, div, part);
+        k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, sums, 2, 0);
         k_co_finish<<<tb, 64, 0, s>>>(st, result, sums, means, cells, B, 0);
     }
     auto apply = [&](const float* vec, bool loop) {          // q = A vec (and, inside the loop, the dot products)
         CO_LAUNCH((k_co_gradient<2, false>), (k_co_gradient<3, false>), g, pf, vec, grad, loop ? st : nullptr);
-        if (loop) CO_LAUNCH((k_co_divergence<2, 1>), (k_co_divergence<3, 1>), g, gvec, cf, q, vec, r, st);
-        else      CO_LAUNCH((k_co_divergence<2, 0>), (k_co_divergence<3, 0>), g, gvec, cf, q, nullptr, nullptr, st);
+        if (loop) {
+            CO_LAUNCH((k_co_divergence<2, 1>), (k_co_divergence<3, 1>), g, gvec, cf, q, vec, r, st, part, slot);
+            k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, nullptr, 0, 1);
+        } else {
+            CO_LAUNCH((k_co_divergence<2, 0>), (k_co_divergence<3, 0>), g, gvec, cf, q, nullptr, nullptr, st, part, slot);
+        }
     };
     // r0 = y - (A + c 11^T) x0
-    if (prm.matrix_offset != 0.f) k_co_mean<<<grid, block, 0, s>>>(g, cf, p, xsums);
+    if (prm.matrix_offset != 0.f) {
+        k_co_sum<<<grid, block, 0, s>>>(g, cf, p, part);
+        k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, xsums, 2, 0);
+    }
     apply(p, false);
-    CO_LAUNCH((k_co_update<2, 0>), (k_co_update<3, 0>), g, cf, p, r, dir, q, div, prm.matrix_offset, st, balance ? means : nullptr, xsums);
+    CO_LAUNCH((k_co_update<2, 0>), (k_co_update<3, 0>), g, cf, p, r, dir, q, div, prm.matrix_offset, st, balance ? means : nullptr, xsums,
+              part, slot);
+    k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, nullptr, 1, 0);
     k_co_control<<<tb, 64, 0, s>>>(st, B, 0, prm.rtol, prm.atol, prm.max_iter);
     apply(dir, true);
     int h_cont = 1;
     CoStatus* hst = (CoStatus*)malloc(sizeof(CoStatus) * B);
     if (!hst) { phi_set_error("collocated: out of host memory"); return PHI_ERR_INVALID; }
     for (int it = 0; it < prm.max_iter && h_cont; ++it) {
-        k_co_control<<<tb, 64, 0, s>>>(st, B, 1, prm.rtol, prm.atol, prm.max_iter);
-        CO_LAUNCH((k_co_update<2, 1>), (k_co_update<3, 1>), g, cf, p, r, dir, q, div, prm.matrix_offset, st, nullptr, xsums);
-        CO_LAUNCH((k_co_update<2, 2>), (k_co_update<3, 2>), g, cf, p, r, dir, q, div, prm.matrix_offset, st, nullptr, xsums);
+        CO_LAUNCH((k_co_update<2, 1>), (k_co_update<3, 1>), g, cf, p, r, dir, q, div, prm.matrix_offset, st, nullptr, xsums, part, slot);
+        k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, nullptr, 1, 1);
+        CO_LAUNCH((k_co_update<2, 2>), (k_co_update<3, 2>), g, cf, p, r, dir, q, div, prm.matrix_offset, st, nullptr, xsums, part, slot);
         k_co_control<<<tb, 64, 0, s>>>(st, B, 2, prm.rtol, prm.atol, prm.max_iter);
         apply(dir, true);
         if ((it & 7) == 7 || it + 1 == prm.max_iter) {
@@ -283,10 +350,10 @@ int phi_wide_laplace(const DGrid& g, const DField vfields0[3], const DField& pf,
     const dim3 grid = co_grid(g), block(128);
     if (g.dim == 3) {
         k_co_gradient<3, false><<<grid, block, 0, s>>>(g, pf, x, grad, nullptr);
-        k_co_divergence<3, 0><<<grid, block, 0, s>>>(g, gvec, cf, y, nullptr, nullptr, nullptr);
+        k_co_divergence<3, 0><<<grid, block, 0, s>>>(g, gvec, cf, y, nullptr, nullptr, nullptr, nullptr, 0);
     } else {
         k_co_gradient<2, false><<<grid, block, 0, s>>>(g, pf, x, grad, nullptr);
-        k_co_divergence<2, 0><<<grid, block, 0, s>>>(g, gvec, cf, y, nullptr, nullptr, nullptr);
+        k_co_divergence<2, 0><<<grid, block, 0, s>>>(g, gvec, cf, y, nullptr, nullptr, nullptr, nullptr, 0);
     }
     return (int)cudaGetLastError();
 }

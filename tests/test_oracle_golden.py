@@ -138,21 +138,24 @@ def test_cg_adaptive_matches_phiml_solve_linear(name, tag, rtol):
 GOLD_COL = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'phiml_collocated.npz'))
 
 
-@pytest.mark.parametrize('name', ['zero', 'open', 'periodic', 'mixed', 'one', 'mixed3'])
+@pytest.mark.parametrize('name', ['zero', 'open', 'periodic', 'mixed', 'one', 'mixed3', 'lid', 'inflow3'])
 def test_collocated_gradient_divergence_matrix_match_phiml(name):
     """CenteredGrid-velocity variant (SURVEY.md Appendix A; fluid.py:154-155,197-202): central gradient, centred divergence
-    and the traced wide-stencil operator of the vendored PhiML vs the oracle."""
-    vbc = spec_from_arr(GOLD_COL[f'{name}/bc'])
+    and the traced wide-stencil operator of the vendored PhiML vs the oracle.  'lid' and 'inflow3' carry per-component constants
+    (a vector-valued ConstantExtrapolation): each component's divergence term sees its own constant, the operator none."""
+    arr = GOLD_COL[f'{name}/bc']
+    vbc = [spec_from_arr(a) for a in arr] if arr.ndim == 3 else spec_from_arr(arr)
     dx = GOLD_COL[f'{name}/dx']
     p = GOLD_COL[f'{name}/p']
     d = p.ndim
     pbc = O.pressure_bc(vbc)
+    kinds = O.kinds_of(vbc)
     for c, g in enumerate(O.gradient_centered(p, dx, pbc)):
         np.testing.assert_allclose(g, GOLD_COL[f'{name}/grad{c}'], rtol=1e-6, atol=1e-6)
     comps = [GOLD_COL[f'{name}/v{c}'] for c in range(d)]
     np.testing.assert_allclose(O.divergence_centered(comps, dx, O.component_bcs(vbc, d)), GOLD_COL[f'{name}/div'], rtol=1e-6, atol=2e-6)
-    np.testing.assert_allclose(O.wide_laplace(p, dx, pbc, vbc), GOLD_COL[f'{name}/lap'], rtol=1e-5, atol=1e-5)
-    A = O.wide_poisson_matrix(p.shape, dx, vbc)
+    np.testing.assert_allclose(O.wide_laplace(p, dx, pbc, kinds), GOLD_COL[f'{name}/lap'], rtol=1e-5, atol=1e-5)
+    A = O.wide_poisson_matrix(p.shape, dx, kinds)
     np.testing.assert_allclose(A.toarray(), GOLD_COL[f'{name}/matrix'], rtol=1e-6, atol=1e-6)
     np.testing.assert_allclose(A.dot(p.ravel()).reshape(p.shape), GOLD_COL[f'{name}/lap'], rtol=1e-5, atol=1e-5)
 
