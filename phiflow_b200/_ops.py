@@ -519,7 +519,7 @@ def make_incompressible_centered(dom: Domain, vbc, v: List[torch.Tensor], p: tor
     CENTRED arrays, updated in place; returns (v, p).  Solver: CG-adaptive, what the reference's default Solve() runs.
     Synchronises the stream (the iteration loop polls the stopping flags from the host)."""
     require_cuda()
-    _, res = dom.workspace()
+    res = dom.results()
     ws = _collocated_workspace(dom)
     p = dom.alloc_centered() if p is None else p
     prm = cg_params(vbc, rtol=rtol, atol=atol, max_iter=max_iter, method='CG-adaptive')

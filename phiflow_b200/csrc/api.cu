@@ -572,7 +572,7 @@ int phicuda_make_incompressible_centered_host_f32(const PhiGrid* g, const PhiVBC
     if (!v || !p || !prm || !result || !workspace) { phi_set_error("make_incompressible_centered: NULL argument"); return PHI_ERR_INVALID; }
     for (int c = 0; c < g->dim; ++c) if (!v[c]) { phi_set_error("make_incompressible_centered: component %d is NULL", c); return PHI_ERR_INVALID; }
     if (prm->method != PHI_SOLVER_CG_ADAPTIVE) { phi_set_error("make_incompressible_centered: the wide-stencil operator is not symmetric - use PHI_SOLVER_CG_ADAPTIVE (Solve('auto'))"); return PHI_ERR_UNSUPPORTED; }
-    return cuda_fail(phi_make_incompressible_collocated(dg, vf, vf0, pf, cf, v, p, *prm, prm->balance_rhs, result, workspace, workspace_bytes,
+    return cuda_fail(phi_make_incompressible_collocated(dg, vf, vf0, pf, cf, v, p, *prm, result, workspace, workspace_bytes,
                                                         (cudaStream_t)stream), "make_incompressible_centered");
 }
 

@@ -14,7 +14,8 @@ struct CgArgs {
     PhiCgParams prm;
 };
 
-struct CgShared {                   // per-thread view of the CTA's shared memory (pointers carved from one dynamic block)
+struct CgShared {                   // per-entry state of a solve: pointers carved from one block of shared memory (the CTA's dynamic
+                                    // block) or of global memory (the collocated solve's workspace)
     double (*warp_acc)[32];   // [2][warps] (up to 32 warps per CTA)
     double* sum0;                  // reduced accumulator 0 per batch entry
     double* sum1;
@@ -39,7 +40,7 @@ __host__ __device__ inline size_t cg_smem_bytes(int batch)
          + (b8 + 2) * sizeof(int) + 3 * (b8 + 16);
 }
 
-__device__ __forceinline__ CgShared cg_carve(unsigned char* base, int batch)
+__host__ __device__ __forceinline__ CgShared cg_carve(unsigned char* base, int batch)
 {
     const size_t b8 = ((size_t)batch + 1) / 2 * 2;
     CgShared sh;

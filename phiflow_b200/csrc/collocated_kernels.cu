@@ -11,21 +11,22 @@
 // the reference's rank-1 matrix_offset for rank-deficient systems (linear(), _linalg.py:784-789).
 //
 // This is NOT the tuned path (the north-star workloads are staggered): one thread per cell, seven launches per iteration, the
-// host reads the per-entry status every few iterations (the entry point is a `_host` call).  Dot products are summed in double
+// host reads the per-entry running flags every 8 iterations (the entry point is a `_host` call).  Dot products are summed in double
 // in a fixed order - per block (warp butterflies, then the four warps in turn), then per entry over the blocks (k_co_reduce) -
 // so the same call gives the same bits every time and a batch entry's result does not depend on its neighbours.
+// The per-entry bookkeeping - balanced right-hand side, start, stopping rule (stop_on_l2 with the divergence test) and result
+// record - is that of the persistent CG kernels (cg_common.cuh), on a CgShared view of the workspace.
 // It exists so that CenteredGrid velocities run on the GPU with the reference's semantics instead of falling through.
 #include "phi_internal.cuh"
 #include "launch.cuh"
+#include "cg_common.cuh"
+
+#include <vector>
 
 struct CoVec { DField f[3]; const float* p[3]; };          // three centred arrays with their own boundaries
 struct CoOut { float* p[3]; };
-
-struct CoStatus {            // per batch entry, device memory
-    double dx_dy, dx_r, s_dx, rsq, r_dy;     // dot products, written by k_co_reduce
-    float tol_sq, rsq0, last_rsq, pad_;
-    int iterations, cont, converged, diverged;
-};
+// per batch entry, written by k_co_reduce: dir.q, dir.r, sum(dir) (operator application), |r|^2, r.q (phase 1)
+struct CoDots { double *dq, *dr, *sd, *rr, *rq; };
 
 template <int DIM>
 __device__ __forceinline__ bool co_index(const DGrid& g, int& b, int& x, int& y, int& z)
@@ -71,11 +72,11 @@ __device__ __forceinline__ void co_block_partials(const double (&v)[N], double* 
 template <int DIM, bool SUB>
 __global__ void __launch_bounds__(128)
 k_co_gradient(const __grid_constant__ DGrid g, const __grid_constant__ DField pf, const float* __restrict__ p, const __grid_constant__ CoOut out,
-              const CoStatus* __restrict__ st)
+              const unsigned char* __restrict__ cont)
 {
     int b, x, y, z;
     const bool in = co_index<DIM>(g, b, x, y, z);
-    if (!in || (st && !st[b].cont)) return;
+    if (!in || (cont && !cont[b])) return;
     const long long off = (long long)b * pf.sb + (long long)z * pf.sz + (long long)y * pf.sy + x;
 #pragma unroll
     for (int c = 0; c < DIM; ++c) {
@@ -91,13 +92,13 @@ k_co_gradient(const __grid_constant__ DGrid g, const __grid_constant__ DField pf
 template <int DIM, int MODE>
 __global__ void __launch_bounds__(128)
 k_co_divergence(const __grid_constant__ DGrid g, const __grid_constant__ CoVec v, const __grid_constant__ DField cf, float* __restrict__ out,
-                const float* __restrict__ dir, const float* __restrict__ r, const CoStatus* __restrict__ st, double* __restrict__ part,
+                const float* __restrict__ dir, const float* __restrict__ r, const unsigned char* __restrict__ cont, double* __restrict__ part,
                 size_t slot)
 {
     int b, x, y, z;
     const bool in = co_index<DIM>(g, b, x, y, z);
     double a[3] = {0, 0, 0};
-    const bool live = in && (MODE == 0 || st[b].cont);
+    const bool live = in && (MODE == 0 || cont[b]);
     if (live) {
         float acc = 0.f;
 #pragma unroll
@@ -119,36 +120,37 @@ k_co_divergence(const __grid_constant__ DGrid g, const __grid_constant__ CoVec v
 }
 
 // Element-wise pieces of the CG-adaptive iteration (_linalg.py:109-122); q = A dir + c * sum(dir) with c = matrix_offset.
-//   PHASE 0 (initial residual): r = y - q(x0); dir = r; block partials of |r|^2 and |y|^2
+//   PHASE 0 (initial residual): r = y - mean - q(x0) with sh.sum1 = sum(x0); dir = r; block partials of |r|^2 and |y|^2
 //   PHASE 1: step = (dir.r) / (dir.q); x += step dir; r -= step q; block partials of |r|^2 and r.q
 //   PHASE 2: dir = r - ((r.q) / (dir.q)) dir  (k_co_control then advances the iteration count and the stopping rule)
+// The offset terms are formed here from the double sums, not taken from cg_balance's rounded sh.offs: nvcc contracts
+// q + c * (float)sum into one FFMA, and the bits of the solve depend on it.
 template <int DIM, int PHASE>
 __global__ void __launch_bounds__(128)
 k_co_update(const __grid_constant__ DGrid g, const __grid_constant__ DField cf, float* __restrict__ x, float* __restrict__ r, float* __restrict__ dir,
-            const float* __restrict__ q, const float* __restrict__ y, float offset, CoStatus* __restrict__ st,
-            const float* __restrict__ means, const double* __restrict__ x0sums, double* __restrict__ part, size_t slot)
+            const float* __restrict__ q, const float* __restrict__ y, float offset, const CgShared sh, const CoDots d,
+            double* __restrict__ part, size_t slot)
 {
     int b, xx, yy, zz;
     const bool in = co_index<DIM>(g, b, xx, yy, zz);
     const int bb = (DIM == 3) ? blockIdx.z / g.n[2] : blockIdx.z;
     const long long off = (long long)bb * cf.sb + (long long)zz * cf.sz + (long long)yy * cf.sy + xx;
-    CoStatus& s = st[bb];
     double a[2] = {0, 0};
     if (PHASE == 0) {
         if (in) {
-            const float yv = y[off] - (means ? means[bb] : 0.f);
-            const float rv = yv - (q[off] + offset * (float)x0sums[bb]);
+            const float yv = y[off] - sh.mean[bb];
+            const float rv = yv - (q[off] + offset * (float)sh.sum1[bb]);
             r[off] = rv; dir[off] = rv;
             a[0] = (double)rv * rv; a[1] = (double)yv * yv;
         }
-        co_block_partials<2>(a, part, g, bb, slot);                    // r_dy doubles as |y|^2 during set-up
+        co_block_partials<2>(a, part, g, bb, slot);
         return;
     }
-    if (!s.cont) return;
-    const double S = s.s_dx;
-    const double dxdy = s.dx_dy + (double)offset * S * S;               // dir . (A dir + c sum(dir))
+    if (!sh.cont[bb]) return;
+    const double S = d.sd[bb];
+    const double dxdy = d.dq[bb] + (double)offset * S * S;              // dir . (A dir + c sum(dir))
     if (PHASE == 1) {
-        const float step = dxdy != 0.0 ? (float)(s.dx_r / dxdy) : 0.f;  // divide_no_nan
+        const float step = dxdy != 0.0 ? (float)(d.dr[bb] / dxdy) : 0.f;  // divide_no_nan
         if (in) {
             const float qv = q[off] + offset * (float)S;
             x[off] = x[off] + step * dir[off];
@@ -160,44 +162,40 @@ k_co_update(const __grid_constant__ DGrid g, const __grid_constant__ DField cf, 
         return;
     }
     // PHASE 2
-    const float coef = dxdy != 0.0 ? (float)(s.r_dy / dxdy) : 0.f;
+    const float coef = dxdy != 0.0 ? (float)(d.rq[bb] / dxdy) : 0.f;
     if (in) dir[off] = r[off] - coef * dir[off];
 }
 
-// one thread per batch entry, between the phases: bookkeeping of the accumulators and of the stopping rule (stop_on_l2)
-__global__ void k_co_control(CoStatus* st, int batch, int phase, float rtol, float atol, int max_iter)
+// Per-entry bookkeeping between the phases (cg_common.cuh).  k_co_balance and k_co_control run one thread per batch entry,
+// k_co_start and k_co_result one block.
+// sum0 = sum(y), sum1 = sum(x0) -> the balanced right-hand side (sh.mean)
+__global__ void k_co_balance(const CgShared sh, const PhiCgParams prm, int batch, double cells)
 {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= batch) return;
-    CoStatus& s = st[b];
-    if (phase == 0) {                 // after the initial residual: tolerance relative to |y|^2 (_linalg.py:109)
-        const float rsq = (float)s.rsq;
-        s.tol_sq = fmaxf(rtol * rtol * (float)s.r_dy, atol * atol);
-        s.rsq0 = fabsf(rsq);
-        s.converged = fabsf(rsq) <= s.tol_sq; s.diverged = !isfinite(rsq);
-        s.iterations = 0;
-        s.cont = (!s.converged && !s.diverged && max_iter > 0) ? 1 : 0;
-        return;
-    }
-    if (!s.cont) return;
-    // phase 2: after the direction update
-    const float rsq = fabsf((float)s.rsq);
-    s.iterations += 1;
-    s.converged = rsq <= s.tol_sq;
-    s.diverged = !isfinite(rsq) || (rsq / s.rsq0 > 1e5f && s.iterations >= 8);
-    s.cont = (!s.converged && !s.diverged && s.iterations < max_iter) ? 1 : 0;
-    s.last_rsq = rsq;                  // residual_sq for the result record
+    if (b < batch) cg_balance<false>(sh, prm, b, cells);
 }
 
-// One block per batch entry: sums the block partials of each of `nq` values in a fixed order (a strided pass per thread, then a
-// tree over the threads) into the entry's status fields (what = 0: dir.q, dir.r, sum(dir); 1: |r|^2, r.q or |y|^2) or into
-// sums[b] (what = 2).  running: skip entries that have stopped - their partials were not written.
-__global__ void __launch_bounds__(256) k_co_reduce(const double* __restrict__ part, size_t slot, int nblk, CoStatus* st, double* sums,
-                                                   int what, int running)
+// sum0 = |r0|^2, sum1 = |y|^2 -> tolerance, flags and rsq0 (CG-adaptive's tolerance is relative to |y|^2, _linalg.py:109)
+__global__ void k_co_start(const CgShared sh, const PhiCgParams prm, int batch) { cg_start(sh, prm, batch); }
+
+// rr = |r|^2 after the direction update -> iteration count and stopping rule of the running entries
+__global__ void k_co_control(const CgShared sh, const PhiCgParams prm, int batch, const double* __restrict__ rr)
+{
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < batch && sh.cont[b]) cg_iteration_done(sh, prm, b, rr[b]);
+}
+
+__global__ void k_co_result(const CgShared sh, PhiCgResult* result, int batch) { cg_write_result(sh, result, batch, true); }
+
+// One block per batch entry: sums the block partials of each of up to three values in a fixed order (a strided pass per thread,
+// then a tree over the threads) into out0[b], out1[b], out2[b] (nullptr: fewer values).  cont: skip entries that have stopped -
+// their partials were not written.
+__global__ void __launch_bounds__(256) k_co_reduce(const double* __restrict__ part, size_t slot, int nblk, const unsigned char* __restrict__ cont,
+                                                   double* out0, double* out1, double* out2)
 {
     const int b = blockIdx.x;
-    if (running && !st[b].cont) return;
-    const int nq = what == 0 ? 3 : (what == 1 ? 2 : 1);
+    if (cont && !cont[b]) return;
+    const int nq = out2 ? 3 : (out1 ? 2 : 1);
     __shared__ double red[3][256];
     for (int k = 0; k < nq; ++k) {
         const double* p = part + k * slot + (size_t)b * nblk;
@@ -211,127 +209,109 @@ __global__ void __launch_bounds__(256) k_co_reduce(const double* __restrict__ pa
         __syncthreads();
     }
     if (threadIdx.x != 0) return;
-    CoStatus& s = st[b];
-    if (what == 0)      { s.dx_dy = red[0][0]; s.dx_r = red[1][0]; s.s_dx = red[2][0]; }
-    else if (what == 1) { s.rsq = red[0][0]; s.r_dy = red[1][0]; }
-    else                sums[b] = red[0][0];
+    out0[b] = red[0][0];
+    if (nq > 1) out1[b] = red[1][0];
+    if (nq > 2) out2[b] = red[2][0];
 }
 
-// block partials of sum(a) per batch entry
+// block partials of sum(y) and sum(x0) per batch entry (x0 == nullptr: 0)
 __global__ void __launch_bounds__(128)
-k_co_sum(const __grid_constant__ DGrid g, const __grid_constant__ DField cf, const float* __restrict__ a, double* __restrict__ part)
+k_co_sum(const __grid_constant__ DGrid g, const __grid_constant__ DField cf, const float* __restrict__ y, const float* __restrict__ x0,
+         double* __restrict__ part, size_t slot)
 {
-    int b, x, y, z;
-    const bool in = g.dim == 3 ? co_index<3>(g, b, x, y, z) : co_index<2>(g, b, x, y, z);
+    int b, x, yy, z;
+    const bool in = g.dim == 3 ? co_index<3>(g, b, x, yy, z) : co_index<2>(g, b, x, yy, z);
     const int bb = (g.dim == 3) ? blockIdx.z / g.n[2] : blockIdx.z;
-    double v[1] = {0};
-    if (in) v[0] = a[(long long)bb * cf.sb + (long long)z * cf.sz + (long long)y * cf.sy + x];
-    co_block_partials<1>(v, part, g, bb, 0);
-}
-
-__global__ void k_co_finish(const CoStatus* st, PhiCgResult* result, const double* sums, float* means, double cells, int batch, int what)
-{
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= batch) return;
-    if (what == 0) { means[b] = (float)(sums[b] / cells); return; }
-    PhiCgResult res;
-    res.iterations = st[b].iterations; res.converged = st[b].converged; res.diverged = st[b].diverged;
-    res.residual_sq = st[b].iterations > 0 ? st[b].last_rsq : st[b].rsq0; res.tol_sq = st[b].tol_sq; res.initial_residual_sq = st[b].rsq0;
-    result[b] = res;
-}
-
-template <int DIM>
-__global__ void __launch_bounds__(128)
-k_co_sub_mean(const __grid_constant__ DGrid g, const __grid_constant__ DField cf, float* __restrict__ a, const float* __restrict__ means)
-{
-    int b, x, y, z;
-    if (!co_index<DIM>(g, b, x, y, z)) return;
-    a[(long long)b * cf.sb + (long long)z * cf.sz + (long long)y * cf.sy + x] -= means[b];
+    double v[2] = {0, 0};
+    if (in) {
+        const long long off = (long long)bb * cf.sb + (long long)z * cf.sz + (long long)yy * cf.sy + x;
+        v[0] = y[off];
+        if (x0) v[1] = x0[off];
+    }
+    co_block_partials<2>(v, part, g, bb, slot);
 }
 
 static dim3 co_grid(const DGrid& g) { return dim3((g.n[0] + 127) / 128, g.n[1], g.n[2] * g.batch); }
 static int co_blocks_per_entry(const DGrid& g) { return (g.n[0] + 127) / 128 * g.n[1] * g.n[2]; }
+static size_t co_round(size_t bytes) { return (bytes + 255) / 256 * 256; }
+static size_t co_array_bytes(const DGrid& g) { return co_round((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float)); }
+static size_t co_state_bytes(int batch) { return co_round(cg_smem_bytes(batch)); }
+static size_t co_dots_bytes(int batch) { return co_round(5 * (size_t)batch * sizeof(double)); }
 
+// r, dir, q, div, 3 gradient components | per-entry state (CgShared) | the CoDots | block partials of up to 3 values per entry,
+// each part 256-byte aligned (k_co_reduce reads the partials warp-wide: an unaligned base costs it a sector more per load)
 size_t phi_collocated_workspace_bytes(const DGrid& g)
 {
-    const size_t arr = ((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float) + 255) / 256 * 256;
-    // r, dir, q, div, 3 gradient components + block partials of up to 3 dot products + status + sums of div / of x0 + means
-    return 7 * arr + 3 * (size_t)g.batch * co_blocks_per_entry(g) * sizeof(double)
-         + (size_t)g.batch * (sizeof(CoStatus) + 2 * sizeof(double) + sizeof(float)) + 1024;
+    return 7 * co_array_bytes(g) + co_state_bytes(g.batch) + co_dots_bytes(g.batch) + 3 * (size_t)g.batch * co_blocks_per_entry(g) * sizeof(double);
 }
 
-// Host-synchronising: reads the per-entry status every `poll` iterations.
+// Host-synchronising: reads the per-entry running flags every 8 iterations.
 int phi_make_incompressible_collocated(const DGrid& g, const DField vfields[3], const DField vfields0[3], const DField& pf, const DField& cf,
-                                       float* const v[3], float* p, const PhiCgParams& prm, int balance, PhiCgResult* result,
+                                       float* const v[3], float* p, const PhiCgParams& prm, PhiCgResult* result,
                                        void* workspace, size_t ws_bytes, cudaStream_t s)
 {
     if (ws_bytes < phi_collocated_workspace_bytes(g)) { phi_set_error("collocated: workspace %zu < %zu bytes", ws_bytes, phi_collocated_workspace_bytes(g)); return PHI_ERR_WORKSPACE; }
-    const size_t arr = ((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float) + 255) / 256 * 256;
+    const int B = g.batch, tb = (B + 63) / 64;
+    const size_t arr = co_array_bytes(g);
     unsigned char* ws = (unsigned char*)workspace;
     float* r = (float*)ws; float* dir = (float*)(ws + arr); float* q = (float*)(ws + 2 * arr); float* div = (float*)(ws + 3 * arr);
     CoOut grad; for (int c = 0; c < 3; ++c) grad.p[c] = (float*)(ws + (4 + c) * arr);
+    unsigned char* state = ws + 7 * arr;
+    const CgShared sh = cg_carve(state, B);
+    double* dots = (double*)(state + co_state_bytes(B));
+    const CoDots d = {dots, dots + B, dots + 2 * B, dots + 3 * B, dots + 4 * B};
     const int nblk = co_blocks_per_entry(g);
-    const size_t slot = (size_t)g.batch * nblk;
-    double* part = (double*)(ws + 7 * arr);
-    CoStatus* st = (CoStatus*)(part + 3 * slot);
-    double* sums = (double*)(st + g.batch);
-    double* xsums = sums + g.batch;
-    float* means = (float*)(xsums + g.batch);
-    const int B = g.batch, tb = (B + 63) / 64;
+    const size_t slot = (size_t)B * nblk;
+    double* part = (double*)((unsigned char*)dots + co_dots_bytes(B));
     const dim3 grid = co_grid(g), block(128);
     const double cells = (double)g.n[0] * g.n[1] * g.n[2];
-    cudaError_t e = cudaMemsetAsync(st, 0, (size_t)B * (sizeof(CoStatus) + 2 * sizeof(double) + sizeof(float)), s);
+    cudaError_t e = cudaMemsetAsync(state, 0, co_state_bytes(B), s);
     if (e) return (int)e;
     CoVec vin, gvec;
     for (int c = 0; c < 3; ++c) { vin.f[c] = vfields[c]; vin.p[c] = v[c]; gvec.f[c] = vfields0[c]; gvec.p[c] = grad.p[c]; }
     const bool d3 = g.dim == 3;
 #define CO_LAUNCH(K2, K3, ...) do { if (d3) K3<<<grid, block, 0, s>>>(__VA_ARGS__); else K2<<<grid, block, 0, s>>>(__VA_ARGS__); } while (0)
-    // right-hand side: divergence of the input velocity, balanced when the system is rank deficient (fluid.py:145-148, 205-209)
-    CO_LAUNCH((k_co_divergence<2, 0>), (k_co_divergence<3, 0>), g, vin, cf, div, nullptr, nullptr, st, part, slot);
-    if (balance) {
-        k_co_sum<<<grid, block, 0, s>>>(g, cf, div, part);
-        k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, sums, 2, 0);
-        k_co_finish<<<tb, 64, 0, s>>>(st, result, sums, means, cells, B, 0);
+    // right-hand side: divergence of the input velocity, balanced when the system is rank deficient (fluid.py:145-148, 205-209),
+    // and sum(x0) for the offset c 11^T x0 of r0.  sum(x0) is taken only with c != 0: with c = 0 the term c * (float)sum(x0) must
+    // be exactly +0, which a negative or non-finite sum would break.
+    CO_LAUNCH((k_co_divergence<2, 0>), (k_co_divergence<3, 0>), g, vin, cf, div, nullptr, nullptr, nullptr, part, slot);
+    if (prm.balance_rhs || prm.matrix_offset != 0.f) {
+        k_co_sum<<<grid, block, 0, s>>>(g, cf, div, prm.matrix_offset != 0.f ? p : nullptr, part, slot);
+        k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, nullptr, sh.sum0, sh.sum1, nullptr);
+        k_co_balance<<<tb, 64, 0, s>>>(sh, prm, B, cells);
     }
     auto apply = [&](const float* vec, bool loop) {          // q = A vec (and, inside the loop, the dot products)
-        CO_LAUNCH((k_co_gradient<2, false>), (k_co_gradient<3, false>), g, pf, vec, grad, loop ? st : nullptr);
+        CO_LAUNCH((k_co_gradient<2, false>), (k_co_gradient<3, false>), g, pf, vec, grad, loop ? sh.cont : nullptr);
         if (loop) {
-            CO_LAUNCH((k_co_divergence<2, 1>), (k_co_divergence<3, 1>), g, gvec, cf, q, vec, r, st, part, slot);
-            k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, nullptr, 0, 1);
+            CO_LAUNCH((k_co_divergence<2, 1>), (k_co_divergence<3, 1>), g, gvec, cf, q, vec, r, sh.cont, part, slot);
+            k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, sh.cont, d.dq, d.dr, d.sd);
         } else {
-            CO_LAUNCH((k_co_divergence<2, 0>), (k_co_divergence<3, 0>), g, gvec, cf, q, nullptr, nullptr, st, part, slot);
+            CO_LAUNCH((k_co_divergence<2, 0>), (k_co_divergence<3, 0>), g, gvec, cf, q, nullptr, nullptr, nullptr, part, slot);
         }
     };
     // r0 = y - (A + c 11^T) x0
-    if (prm.matrix_offset != 0.f) {
-        k_co_sum<<<grid, block, 0, s>>>(g, cf, p, part);
-        k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, xsums, 2, 0);
-    }
     apply(p, false);
-    CO_LAUNCH((k_co_update<2, 0>), (k_co_update<3, 0>), g, cf, p, r, dir, q, div, prm.matrix_offset, st, balance ? means : nullptr, xsums,
-              part, slot);
-    k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, nullptr, 1, 0);
-    k_co_control<<<tb, 64, 0, s>>>(st, B, 0, prm.rtol, prm.atol, prm.max_iter);
+    CO_LAUNCH((k_co_update<2, 0>), (k_co_update<3, 0>), g, cf, p, r, dir, q, div, prm.matrix_offset, sh, d, part, slot);
+    k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, nullptr, sh.sum0, sh.sum1, nullptr);
+    k_co_start<<<1, 64, 0, s>>>(sh, prm, B);
     apply(dir, true);
     int h_cont = 1;
-    CoStatus* hst = (CoStatus*)malloc(sizeof(CoStatus) * B);
-    if (!hst) { phi_set_error("collocated: out of host memory"); return PHI_ERR_INVALID; }
+    std::vector<unsigned char> hcont(B);
     for (int it = 0; it < prm.max_iter && h_cont; ++it) {
-        CO_LAUNCH((k_co_update<2, 1>), (k_co_update<3, 1>), g, cf, p, r, dir, q, div, prm.matrix_offset, st, nullptr, xsums, part, slot);
-        k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, st, nullptr, 1, 1);
-        CO_LAUNCH((k_co_update<2, 2>), (k_co_update<3, 2>), g, cf, p, r, dir, q, div, prm.matrix_offset, st, nullptr, xsums, part, slot);
-        k_co_control<<<tb, 64, 0, s>>>(st, B, 2, prm.rtol, prm.atol, prm.max_iter);
+        CO_LAUNCH((k_co_update<2, 1>), (k_co_update<3, 1>), g, cf, p, r, dir, q, div, prm.matrix_offset, sh, d, part, slot);
+        k_co_reduce<<<B, 256, 0, s>>>(part, slot, nblk, sh.cont, d.rr, d.rq, nullptr);
+        CO_LAUNCH((k_co_update<2, 2>), (k_co_update<3, 2>), g, cf, p, r, dir, q, div, prm.matrix_offset, sh, d, part, slot);
+        k_co_control<<<tb, 64, 0, s>>>(sh, prm, B, d.rr);
         apply(dir, true);
         if ((it & 7) == 7 || it + 1 == prm.max_iter) {
-            e = cudaMemcpyAsync(hst, st, sizeof(CoStatus) * B, cudaMemcpyDeviceToHost, s);
+            e = cudaMemcpyAsync(hcont.data(), sh.cont, B, cudaMemcpyDeviceToHost, s);
             if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-            if (e) { free(hst); return (int)e; }
+            if (e) return (int)e;
             h_cont = 0;
-            for (int b = 0; b < B; ++b) h_cont |= hst[b].cont;
+            for (unsigned char c : hcont) h_cont |= c;
         }
     }
-    free(hst);
-    k_co_finish<<<tb, 64, 0, s>>>(st, result, sums, means, cells, B, 1);
+    k_co_result<<<1, 64, 0, s>>>(sh, result, B);
     // v -= grad p
     CoOut vout; for (int c = 0; c < 3; ++c) vout.p[c] = v[c];
     CO_LAUNCH((k_co_gradient<2, true>), (k_co_gradient<3, true>), g, pf, p, vout, nullptr);
@@ -343,7 +323,7 @@ int phi_make_incompressible_collocated(const DGrid& g, const DField vfields[3], 
 int phi_wide_laplace(const DGrid& g, const DField vfields0[3], const DField& pf, const DField& cf, const float* x, float* y,
                      void* workspace, size_t ws_bytes, cudaStream_t s)
 {
-    const size_t arr = ((size_t)g.cext[0] * g.cext[1] * g.cext[2] * g.batch * sizeof(float) + 255) / 256 * 256;
+    const size_t arr = co_array_bytes(g);
     if (ws_bytes < 3 * arr) { phi_set_error("wide_laplace: workspace %zu < %zu bytes", ws_bytes, 3 * arr); return PHI_ERR_WORKSPACE; }
     CoOut grad; CoVec gvec;
     for (int c = 0; c < 3; ++c) { grad.p[c] = (float*)((unsigned char*)workspace + c * arr); gvec.f[c] = vfields0[c]; gvec.p[c] = grad.p[c]; }

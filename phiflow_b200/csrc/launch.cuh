@@ -30,7 +30,7 @@ int phi_launch_grid_sample(const DGrid& g, const DField& f, const float* grid, c
 // CenteredGrid (collocated) velocities, wide stencil (collocated_kernels.cu)
 size_t phi_collocated_workspace_bytes(const DGrid& g);
 int phi_make_incompressible_collocated(const DGrid& g, const DField vfields[3], const DField vfields0[3], const DField& pf, const DField& cf,
-                                       float* const v[3], float* p, const PhiCgParams& prm, int balance, PhiCgResult* result,
+                                       float* const v[3], float* p, const PhiCgParams& prm, PhiCgResult* result,
                                        void* workspace, size_t ws_bytes, cudaStream_t s);
 int phi_wide_laplace(const DGrid& g, const DField vfields0[3], const DField& pf, const DField& cf, const float* x, float* y,
                      void* workspace, size_t ws_bytes, cudaStream_t s);

@@ -1,7 +1,8 @@
 """
 The pressure-solve contract of the CenteredGrid (collocated, wide-stencil) projection, phicuda_make_incompressible_centered_host_f32
-(csrc/collocated_kernels.cu): its own host loop, which polls the stopping flags every 8 iterations, its own stopping rule, result
-record and matrix-offset handling.  Every CenteredGrid projection runs through it (phi_cuda façade and _ops), so it is held to what
+(csrc/collocated_kernels.cu): its own host loop, which polls the stopping flags every 8 iterations, and its own matrix-offset terms,
+with the stopping rule, result record and right-hand-side balancing of the persistent CG kernels (csrc/cg_common.cuh).  Every
+CenteredGrid projection runs through it (phi_cuda façade and _ops), so it is held to what
 test_gpu_cg_contract.py holds the staggered solvers to, against the oracle (oracle/oracle_np.py, pinned against PhiML by
 tests/golden/phiml_collocated.npz):
   * the stencils cell by cell, at bounds derived from the operations (not relative to max|ref|), with scalar, mixed and
