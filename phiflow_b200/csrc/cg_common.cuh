@@ -31,13 +31,16 @@ struct CgShared {                   // per-entry state of a solve: pointers carv
     int* any_cont;
     unsigned char *cont, *conv, *divg;
     float* bprev;                  // beta of the previous iteration (one-sweep ring CG: r_k = d_k - beta_k d_{k-1})
+    float* aprev2;                 // one-sweep ring CG: alpha_{k-2} and beta_{k-1}, which rebuild d_{k-2} for a three-direction
+    float* bprev2;                 // x update
+    int* owed;                     // one-sweep ring CG: directions whose step x still owes (0 .. 2)
 };
 
 __host__ __device__ inline size_t cg_smem_bytes(int batch)
 {
     const size_t b8 = ((size_t)batch + 1) / 2 * 2;      // keep 8-byte alignment of what follows
-    return 2 * 32 * sizeof(double) + 3 * b8 * sizeof(double) + 8 * b8 * sizeof(float)
-         + (b8 + 2) * sizeof(int) + 3 * (b8 + 16);
+    return 2 * 32 * sizeof(double) + 3 * b8 * sizeof(double) + 10 * b8 * sizeof(float)
+         + (2 * b8 + 2) * sizeof(int) + 3 * (b8 + 16);
 }
 
 __host__ __device__ __forceinline__ CgShared cg_carve(unsigned char* base, int batch)
@@ -61,7 +64,10 @@ __host__ __device__ __forceinline__ CgShared cg_carve(unsigned char* base, int b
     sh.cont = p; p += b8 + 16;
     sh.conv = p; p += b8;
     sh.divg = p; p += (b8 + 3) / 4 * 4;            // divg starts 4-byte aligned (b8 is even)
-    sh.bprev = (float*)p;
+    sh.bprev = (float*)p; p += b8 * sizeof(float);
+    sh.aprev2 = (float*)p; p += b8 * sizeof(float);
+    sh.bprev2 = (float*)p; p += b8 * sizeof(float);
+    sh.owed = (int*)p;
     return sh;
 }
 

@@ -929,11 +929,17 @@ __device__ __forceinline__ void ring_unit_cells(const RingCfg& cfg, const DGrid&
 // beta_{k+2} = (|r_{k+1}|^2 - 2 alpha r.q + alpha^2 |q|^2) / |r_{k+1}|^2 (= |r_{k+2}|^2 / |r_{k+1}|^2 in exact arithmetic).  The
 // stopping rule still uses the true |r_{k+1}|^2, and the look-ahead is rebuilt from it every iteration, so its rounding does not
 // accumulate.  r is not stored: the previous pass formed d_k = r_k + beta_k d_{k-1}, so r_k = d_k - beta_k d_{k-1} is recovered in
-// registers (its rounding error is relative to |d_k|, a small multiple of |r_k|, and does not grow with k; r_0 = d_0).  Bytes per
-// iteration: d_k, d_{k-1} read, d_{k+1} written (12 B/cell) + x += alpha_{k-1} d_{k-1} + alpha_k d_k every second iteration, with
-// d_{k-1} already staged (8 B/cell) = 16 B/cell, against 30 for the two sweeps of k_cg_ring.
+// registers (its rounding error is relative to |d_k|, a small multiple of |r_k|, and does not grow with k; r_0 = d_0).
+// x is read and written every third iteration: sweep k then applies alpha_{k-2} d_{k-2} + alpha_{k-1} d_{k-1} + alpha_k d_k.  d_{k-2}
+// is not read back (other CTAs overwrite its buffer with d_{k+1}) but rebuilt from what is staged: d_{k-1} = r_{k-1} + beta_{k-1}
+// d_{k-2} and r_{k-1} = r_k + alpha_{k-1} A d_{k-1}, with r_k = d_k - beta_k d_{k-1}, so the update is
+//   x += (alpha_{k-1} + g (1 + beta_k)) d_{k-1} + (alpha_k - g) d_k - g alpha_{k-1} A d_{k-1},   g = alpha_{k-2} / beta_{k-1},
+// with A d_{k-1} formed on the owned cells from the d_{k-1} stage.  Guard (fused_xmode): a sweep that starts owing one direction
+// while its beta_k (the divisor of the next sweep) is below FUSED_XBETA_MIN applies alpha_{k-1} d_{k-1} + alpha_k d_k at once.  An
+// entry that stops owing steps gets them after the loop.  Bytes per iteration: d_k, d_{k-1} read, d_{k+1} written (12 B/cell) + the
+// x read and write every third iteration (8/3 B/cell) = 14.7 B/cell, against 30 for the two sweeps of k_cg_ring.
 // Stage layout: d_k (TY+4 lines: halo 2 in y, because d_{k+1} is needed on the halo lines), d_{k-1} (TY+2 lines, not fetched in
-// iteration 0).  x has no halo and is read only on owned cells of every second iteration, so it does not travel through the ring:
+// iteration 0).  x has no halo and is read only on owned cells of every third iteration, so it does not travel through the ring:
 // consumers load it from global memory one plane ahead.  d_{k+1} of each plane goes to a triple-buffered shared tile (TY+2 lines)
 // from which the q_{k+1} stencil takes its y and warp-edge x neighbours; consumers sync on a named barrier once per plane.
 // Only for 3-D, the branch-free tiling, periodic y and z, one GPU, CG without matrix offset or obstacles (phi_launch_cg_ring).
@@ -1049,10 +1055,27 @@ struct FusedPass {
     const float* d; const float* dprev;                   // d_k, d_{k-1} (nullptr in iteration 0, where r_0 = d_0)
     float* dn; float* x;                                  // d_{k+1}, solution (x == nullptr: no x update this iteration)
     float alpha, aprev, beta, bprev;                      // alpha_k, alpha_{k-1}, beta_{k+1}, beta_k
+    float xd, xdp, xq;                                    // three-direction sweep: x += xd d_k + xdp d_{k-1} + xq A d_{k-1}
 };
 
+// beta_{k-1} below this is not divided by: the x step of a sweep that starts owing one direction is then applied at once (two
+// directions) instead of being deferred to a three-direction sweep.  The rebuilt d_{k-2} carries a rounding error of about
+// eps / sqrt(beta_{k-1}) relative to |d_{k-2}|; 1e-2 bounds that at ten times the rounding of a stored direction.
+#define FUSED_XBETA_MIN 1e-2f
+
+// x update of a pass F sweep from the directions x owes at its start and beta_k (its bprev): 0 none (the step of d_k is deferred),
+// 2 x += alpha_{k-1} d_{k-1} + alpha_k d_k, 3 the same + alpha_{k-2} d_{k-2}.  The same on every CTA: both inputs are per-entry
+// state that every CTA reduces alike.
+__device__ __forceinline__ int fused_xmode(int owed, float bprev)
+{
+    return owed == 2 ? 3 : (owed == 1 && !(fabsf(bprev) >= FUSED_XBETA_MIN)) ? 2 : 0;
+}
+
 // One unit of pass F: producer warp streams planes z0-2 .. z1+1, consumers march planes p = z0-1 .. z1 (d_{k+1} on the haloed
-// region) and, one plane behind, q_{k+1} on the owned planes.  acc: d.q, |r|^2, r.q, |q|^2 of this thread.
+// region) and, one plane behind, q_{k+1} on the owned planes.  acc: d.q, |r|^2, r.q, |q|^2 of this thread.  X3: a three-direction
+// sweep, which also forms A d_{k-1} on the owned planes; it releases the stage of each plane one plane later, so that d_{k-1} of
+// plane p-1 is still staged (pass F runs with at least 4 stages).  That allocates better than carrying the plane in registers.
+template <bool X3>
 __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, const DGrid& g, const DField& pf, const FusedGroups& fg,
                                                 const FusedPass& P, float* tile, const RingUnit& u, float (&acc)[4])
 {
@@ -1098,7 +1121,7 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
     float4 n2[FUSED_GI], n1[FUSED_GI];           // d_{k+1} on planes p-2, p-1
     float4 r1[FUSED_GI];                         // r_{k+1} on plane p-1
     float4 xv[FUSED_GI];                         // x on plane p (x-update iterations), loaded during plane p-1
-    SlotIt cur = rg.pos, nxt = cur; nxt.next(cfg.R);
+    SlotIt cur = rg.pos, nxt = cur, prv = cur; nxt.next(cfg.R);   // prv (X3): the plane before cur, still held
     ring_wait_full(rg, cur); ring_wait_full(rg, nxt);
     {
         const float* s0 = ring_ptr(rg, cfg, cur);
@@ -1144,7 +1167,21 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
             if (own) {
                 *reinterpret_cast<float4*>(dnp + fg.gi[k]) = dv;
                 acc[1] += dot4(rv, rv);
-                if (xp) {                                    // odd k: d_{k-1} is staged
+                if constexpr (X3) {                          // A d_{k-1} from the d_{k-1} stages of planes p-1, p, p+1
+                    const int od = pb + fg.ti[k];
+                    const float4 ym = lds4(sc, od - pitch), yp = lds4(sc, od + pitch), zpp = lds4(sn, od);
+                    float xl = __shfl_up_sync(0xffffffffu, dp.w, 1), xr = __shfl_down_sync(0xffffffffu, dp.x, 1);
+                    const float ev = sc[pb + fg.ei[k]];
+                    if (lane == 0) xl = ev;
+                    if (lane == 31) xr = ev;
+                    const float4 q = stencil7(dp, xl, xr, ym, yp, lds4(ring_ptr(rg, cfg, prv), od), zpp, ix2, iy2, iz2, cc);
+                    float4 x4 = xv[k];
+                    x4.x = fmaf(P.xq, q.x, fmaf(P.xdp, dp.x, fmaf(P.xd, c.x, x4.x)));
+                    x4.y = fmaf(P.xq, q.y, fmaf(P.xdp, dp.y, fmaf(P.xd, c.y, x4.y)));
+                    x4.z = fmaf(P.xq, q.z, fmaf(P.xdp, dp.z, fmaf(P.xd, c.z, x4.z)));
+                    x4.w = fmaf(P.xq, q.w, fmaf(P.xdp, dp.w, fmaf(P.xd, c.w, x4.w)));
+                    *reinterpret_cast<float4*>(xp + fg.gi[k]) = x4;
+                } else if (xp) {                             // two directions: d_{k-1} is staged
                     float4 x4 = xv[k];
                     x4.x += aprev * dp.x; x4.y += aprev * dp.y; x4.z += aprev * dp.z; x4.w += aprev * dp.w;
                     x4.x += alpha * c.x; x4.y += alpha * c.y; x4.z += alpha * c.z; x4.w += alpha * c.w;
@@ -1154,7 +1191,8 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
             n0[k] = dv; r0[k] = rv;
             dm[k] = c; dc[k] = zp;
         }
-        ring_release(rg, cur);
+        if constexpr (X3) { if (i > 0) ring_release(rg, prv); prv = cur; }
+        else ring_release(rg, cur);
         if (xp && i < nz) {                          // x of the next owned plane, in flight while q_{k+1} is formed
 #pragma unroll
             for (int k = 0; k < FUSED_GI; ++k)
@@ -1183,6 +1221,7 @@ __device__ __forceinline__ void ring_fused_unit(Ring& rg, const RingCfg& cfg, co
         cur = nxt; nxt.next(cfg.R);
         plane_off += pf.sz;
     }
+    if constexpr (X3) ring_release(rg, prv);
     ring_release(rg, cur);
     rg.pos = nxt;
     asm volatile("bar.sync 1, %0;" ::"r"(cfg.consumers) : "memory");          // the next unit rewrites the tile
@@ -1306,6 +1345,8 @@ k_cg_ring(CgRingArgs A)
         float* const tile = rg.stage0 + (size_t)cfg.R * cfg.stage_floats;
         FusedGroups fg;
         fused_groups_init(fg, cfg, g, a.pf);
+        for (int b = threadIdx.x; b < batch; b += blockDim.x) sh.owed[b] = 0;
+        __syncthreads();
         if (*sh.any_cont) {                          // d_0 = r_0; alpha_0 = |r_0|^2 / d_0.A d_0, beta_1 from |A d_0|^2
             const float* hsrc[2] = {a.r, nullptr};
             const float* esrc[2] = {nullptr, nullptr};
@@ -1331,7 +1372,7 @@ k_cg_ring(CgRingArgs A)
         for (int k = 0; *sh.any_cont; ++k) {
             FusedPass P;
             P.d = D[k % 3]; P.dprev = k > 0 ? D[(k + 2) % 3] : nullptr;
-            P.dn = D[(k + 1) % 3]; P.x = (k & 1) ? a.x : nullptr;
+            P.dn = D[(k + 1) % 3];
             int cur_b = cfg.split ? 0 : -1;
             float acc[4] = {0.f, 0.f, 0.f, 0.f};
             RingUnit u;
@@ -1343,7 +1384,15 @@ k_cg_ring(CgRingArgs A)
                     cur_b = u.b; acc[0] = acc[1] = acc[2] = acc[3] = 0.f;
                 }
                 P.alpha = sh.alpha[u.b]; P.aprev = sh.aprev[u.b]; P.beta = sh.beta[u.b]; P.bprev = sh.bprev[u.b];
-                ring_fused_unit(rg, cfg, g, a.pf, fg, P, tile, u, acc);
+                const int xm = fused_xmode(sh.owed[u.b], P.bprev);
+                P.x = xm ? a.x : nullptr;
+                if (xm == 3) {                       // d_{k-2} = ((1 + beta_k) d_{k-1} - d_k - alpha_{k-1} A d_{k-1}) / beta_{k-1}
+                    const double gam = (double)sh.aprev2[u.b] / sh.bprev2[u.b];
+                    P.xd = (float)(P.alpha - gam);
+                    P.xdp = (float)(P.aprev + gam * (1.0 + P.bprev));
+                    P.xq = (float)(-gam * P.aprev);
+                    ring_fused_unit<true>(rg, cfg, g, a.pf, fg, P, tile, u, acc);
+                } else ring_fused_unit<false>(rg, cfg, g, a.pf, fg, P, tile, u, acc);
             }
             if (cur_b >= 0) { flush_partials(sh, a.partials, 2 * reg, batch, cur_b, acc[0], acc[1]);
                               flush_partials(sh, a.partials, 2 * reg + 1, batch, cur_b, acc[2], acc[3]); }
@@ -1354,7 +1403,11 @@ k_cg_ring(CgRingArgs A)
             for (int b = threadIdx.x; b < batch; b += blockDim.x) {
                 if (!sh.cont[b]) continue;
                 const double dn = sh.sum1[b], dq = sh.sum0[b];
-                if (cg_iteration_done(sh, a.prm, b, dn)) {       // an entry that stops keeps alpha_k: the x step it may still owe
+                const int ow = sh.owed[b];
+                sh.owed[b] = fused_xmode(ow, sh.bprev[b]) ? 0 : ow + 1;
+                if (cg_iteration_done(sh, a.prm, b, dn)) {       // an entry that stops keeps alpha_k, alpha_{k-1}: the steps it owes
+                    sh.aprev2[b] = sh.aprev[b];
+                    sh.bprev2[b] = sh.bprev[b];
                     sh.aprev[b] = sh.alpha[b];
                     sh.bprev[b] = sh.beta[b];
                     sh.alpha[b] = (dq != 0.0) ? (float)(dn / dq) : 0.f;
@@ -1443,18 +1496,26 @@ k_cg_ring(CgRingArgs A)
         t = hi_dold; hi_dold = hi_dnew; hi_dnew = t;
     }
 
-    // entries that stopped after an odd number of iterations still owe x the step alpha d of their last iteration, whose direction
-    // is in d1 (two sweeps: odd iterations write d1) or D[(it - 1) % 3] (pass F).  Pass F tiles hold whole float4 groups; keeping the
-    // partial-group path out of the one-sweep kernel keeps its register allocation (24 B more spill loads with it).
+    // entries that stopped after an odd number of iterations (two sweeps) still owe x the step alpha d of their last iteration,
+    // whose direction is in d1 (odd iterations write d1).  Pass F entries owe up to two steps (sh.owed): alpha_k d_k of their last
+    // iteration k = it - 1, in D[(it - 1) % 3], and alpha_{k-1} d_{k-1}, in D[(it + 1) % 3].  Pass F tiles hold whole float4 groups;
+    // keeping the partial-group path out of the one-sweep kernel keeps its register allocation (24 B more spill loads with it).
     RingUnit u;
     for (int k = 0; ring_next_unit<DIM>(cfg, g, k, u); ++k) {
         const int it = sh.iters[u.b];
-        if (!(it & 1)) continue;
+        const int owe = FUSED ? sh.owed[u.b] : (it & 1);
+        if (!owe) continue;
         const float al = sh.alpha[u.b];
         const float* dl = FUSED ? D[(it - 1) % 3] : a.d1;
+        const float ap = sh.aprev[u.b];
+        const float* dl2 = D[(it + 1) % 3];
         ring_unit_cells<DIM>(cfg, g, a.pf, tg, u, [&](long long off, int nvalid) {
             if (FUSED || nvalid == 4) {
                 float4 xv = *reinterpret_cast<const float4*>(a.x + off);
+                if (FUSED && owe == 2) {
+                    const float4 dp = *reinterpret_cast<const float4*>(dl2 + off);
+                    xv.x += ap * dp.x; xv.y += ap * dp.y; xv.z += ap * dp.z; xv.w += ap * dp.w;
+                }
                 const float4 dv = *reinterpret_cast<const float4*>(dl + off);
                 xv.x += al * dv.x; xv.y += al * dv.y; xv.z += al * dv.z; xv.w += al * dv.w;
                 *reinterpret_cast<float4*>(a.x + off) = xv;

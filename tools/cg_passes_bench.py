@@ -6,9 +6,7 @@
 The plume of bench.py is advanced `--warmup` steps; then, `--rounds` times, each form (PHICUDA_CG_PASSES unset = one sweep per
 iteration where it applies, =2 = two sweeps) runs the next plume step from the same saved state, in alternating order.  Reported per
 form: the pressure solve's time (CUDA events recorded by the library around the solve), its iterations, and the achieved HBM rate
-for the algorithmic byte counts cells * (16 it + 40) (one-sweep: d_k, d_{k-1} read and d_{k+1} written, 12 B/cell per iteration, +
-the x read and write every second iteration; set-up passes 32 + the q_0 sweep 8) and cells * (30 it + 32) (two-sweep, the count
-bench.py reports)."""
+for the algorithmic byte counts of one_sweep_bytes (one-sweep) and cells * (30 it + 32) (two-sweep, the count bench.py reports)."""
 import argparse
 import json
 import os
@@ -22,6 +20,15 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 from phiflow_b200 import _ops as ops  # noqa: E402
 from phiflow_b200._clocks import ClockSampler  # noqa: E402
+
+
+def one_sweep_bytes(cells, it):
+    """Bytes of a one-sweep solve of `it` iterations: d_k, d_{k-1} read and d_{k+1} written (12 B/cell per iteration), the x read
+    and write of every third sweep (8 B/cell), the steps still owed after the loop (it % 3 = 1: x and d_k, 12 B/cell; = 2: x, d_k
+    and d_{k-1}, 16 B/cell), set-up passes 32 + the q_0 sweep 8.  Counts the cadence without the small-beta guard, which makes a
+    sweep apply two steps early; it does not trigger on the plume's solves."""
+    it = np.asarray(it, np.int64)
+    return cells * (12.0 * it + 8.0 * (it // 3) + np.choose(it % 3, [0.0, 12.0, 16.0]) + 40.0)
 
 
 def main():
@@ -79,7 +86,7 @@ def main():
             'step_ms_median': float(np.median([r['step_ms'] for r in rs])),
             'iterations': sorted(set(int(i) for i in it)),
             'ms_per_iteration': float(np.median(ms / it)),
-            'gbs_at_16B': float(np.median(cells * (16.0 * it + 40.0) / t / 1e9)),
+            'gbs_one_sweep_bytes': float(np.median(one_sweep_bytes(cells, it) / t / 1e9)),
             'gbs_at_30B': float(np.median(cells * (30.0 * it + 32.0) / t / 1e9)),
             'ring': {k: rs[0][k] for k in ('TY', 'stages', 'split', 'grid_ctas')}}
     out['speedup_cg_median'] = out['2_sweep']['cg_ms_per_solve']['median'] / out['1_sweep']['cg_ms_per_solve']['median']
