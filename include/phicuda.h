@@ -115,6 +115,7 @@ int         phicuda_device_info(char* name, size_t name_len, int* sm_count, int*
 #define PHI_KERNEL_CG_MARCH      4   /* k_cg_poisson    (persistent, register marching) */
 #define PHI_KERNEL_STENCIL_RING  5   /* k_div_ring / k_gradsub_ring / k_advect_ring: see `stencil` */
 #define PHI_KERNEL_RD_RING       6   /* k_rd_ring       (persistent, TMA ring): phicuda_reaction_diffusion_f32 */
+#define PHI_KERNEL_WAVE_RING     7   /* k_wave_ring     (persistent, TMA ring): phicuda_wave_f32 */
 typedef struct PhiLaunchInfo {
     int32_t kernel;        /* PHI_KERNEL_* */
     int32_t generic;       /* 1: variant with per-tile boundary handling, 0: branch-free variant (every tile qualifies) */
@@ -332,6 +333,32 @@ int phicuda_plume_step_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const Phi
 size_t phicuda_reaction_diffusion_scratch_bytes(const PhiGrid* g);
 int phicuda_reaction_diffusion_f32(const PhiGrid* g, const PhiVBC* bc, float* u, float* v, float du, float dv, float f, float k,
                                    float dt, int32_t substeps, float* scratch, size_t scratch_bytes, void* stream);
+
+/* ---- N8  wave step: the Waves notebook's explicit wave equation with a moving source disc ------------------------------------
+ * `substeps` times, on centred arrays h_c (current) and h_p (previous) of the grid, with disc s of `discs` in substep s:
+ *   h_c = where(disc_s, value_s, h_c);  h_p = where(disc_s, value_s, h_p);
+ *   h_n = 2 * h_c - h_p + dd * (k_speed * laplace(h_c) - k_damp * (h_c - h_p));  (h_c, h_p) = (h_n, h_c)
+ * laplace as phicuda_laplace_f32 with ghost cells from `bc`.  Boundaries: PERIODIC, ZERO_GRADIENT and constant 0 per side - the
+ * extrapolations that the reference's step maps to themselves; a non-zero constant c becomes c - c = 0 after one step (2.0 * h_c
+ * keeps h_c's extrapolation) and returns PHI_ERR_UNSUPPORTED.  Every operation is rounded as the reference's float32 field arithmetic rounds it.  disc_s holds the cells whose
+ * centre p satisfies ((p_x - c_x)^2 + (p_y - c_y)^2) [+ (p_z - c_z)^2] <= radius_sq in float32 (Sphere.lies_inside), with the
+ * cell centres taken from `centers`: n[0] x coordinates, then n[1] y, then n[2] z (host memory), as the caller's grid computes
+ * them.  One disc per substep for every batch entry; `present == 0` stamps nothing.  `discs` and `centers` are host arrays,
+ * copied into `scratch` (phicuda_wave_scratch_bytes) on `stream` - a copy from pageable memory, which waits for the stream's
+ * earlier work.  The update is in place and the call never allocates: on return h_c holds the newest state and h_p the
+ * previous, stamped one, for either parity of `substeps`.  All substeps run in one persistent kernel (PHI_KERNEL_WAVE_RING),
+ * 12 B/cell per substep (+ 12 B/cell once for an odd count).  substeps == 0 returns before any CUDA call.  Single GPU, no
+ * z-slabs; grid lines that do not fit the ring return PHI_ERR_UNSUPPORTED with the widest line that does.  Every argument check
+ * runs before the first CUDA call: a refused call leaves h_c and h_p untouched. */
+typedef struct PhiWaveDisc {
+    float   center[3];     /* x, y[, z] */
+    float   value;         /* stamped value */
+    int32_t present;       /* 0: no disc in this substep */
+} PhiWaveDisc;
+size_t phicuda_wave_scratch_bytes(const PhiGrid* g, int32_t substeps);
+int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, float dd, float k_speed, float k_damp,
+                     const PhiWaveDisc* discs, float radius_sq, const float* centers, int32_t substeps, void* scratch,
+                     size_t scratch_bytes, void* stream);
 
 #ifdef __cplusplus
 }

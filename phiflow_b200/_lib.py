@@ -43,7 +43,11 @@ class PhiLaunchInfo(C.Structure):
                                          'total_units', 'grid_ctas', 'split')]
 
 
-KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING, KERNEL_RD_RING = range(7)
+KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING, KERNEL_RD_RING, KERNEL_WAVE_RING = range(8)
+
+
+class PhiWaveDisc(C.Structure):
+    _fields_ = [('center', C.c_float * 3), ('value', C.c_float), ('present', C.c_int32)]
 
 
 class PhiPlumeParams(C.Structure):
@@ -111,6 +115,9 @@ PROTOTYPES = {
     'phicuda_reaction_diffusion_scratch_bytes': (C.c_size_t, [_P(PhiGrid)]),
     'phicuda_reaction_diffusion_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float,
                                                  C.c_float, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'phicuda_wave_scratch_bytes': (C.c_size_t, [_P(PhiGrid), C.c_int32]),
+    'phicuda_wave_f32': (C.c_int, [_P(PhiGrid), _P(PhiBC), C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, _P(PhiWaveDisc),
+                                   C.c_float, _P(C.c_float), C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 

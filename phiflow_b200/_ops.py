@@ -459,6 +459,37 @@ def reaction_diffusion(dom: Domain, spec, u, v, du: float, dv: float, f: float, 
     return un, vn
 
 
+def wave(dom: Domain, spec, h_c, h_p, dd: float, k_speed: float, k_damp: float, discs, radius_sq: float, centers, substeps: int = 1):
+    """`substeps` steps of the Waves notebook's wave equation in one launch (include/phicuda.h, N8): per substep s the disc s is
+    stamped on both states, then h_n = 2 h_c - h_p + dd (k_speed laplace(h_c) - k_damp (h_c - h_p)) and (h_c, h_p) = (h_n, h_c).
+    discs: `substeps` entries (center, value), or None for a substep without a disc; radius_sq: float32 r^2; centers: per-axis cell
+    centres (x, then y[, z]) as float32.  Returns new arrays (h_c', h_p'); the inputs are not modified and may be the same tensor."""
+    require_cuda()
+    assert dom.halo == 0, "the wave step is not offered on z-slabs"
+    shape = dom._shape(dom.cext)
+    assert tuple(h_c.shape) == shape and tuple(h_p.shape) == shape, f"h_c, h_p: shapes {tuple(h_c.shape)}, {tuple(h_p.shape)} are not centred arrays of the domain"
+    assert len(discs) == substeps, f"{len(discs)} discs for {substeps} substeps"
+    table = (_lib.PhiWaveDisc * max(substeps, 1))()
+    for d, entry in zip(table, discs):
+        if entry is not None:
+            center, value = entry
+            for a, c in enumerate(center):
+                d.center[a] = float(c)
+            d.value, d.present = float(value), 1
+    coords = np.ascontiguousarray(centers, dtype=np.float32)
+    assert coords.size == sum(dom.res), f"{coords.size} cell centres for resolution {dom.res}"
+    hc, hp = h_c.clone(), h_p.clone()
+    lib = _lib.load()
+    n = lib.phicuda_wave_scratch_bytes(C.byref(dom.grid), substeps)
+    scratch = getattr(dom, '_wave_scratch', None)
+    if scratch is None or 4 * scratch.numel() < n:
+        scratch = dom._wave_scratch = torch.empty((n + 3) // 4, dtype=torch.float32, device=dom.device)
+    _lib.check(lib.phicuda_wave_f32(C.byref(dom.grid), C.byref(make_bc(spec)), _ptr(hc), _ptr(hp), C.c_float(dd), C.c_float(k_speed),
+                                    C.c_float(k_damp), table, C.c_float(radius_sq), coords.ctypes.data_as(C.POINTER(C.c_float)),
+                                    C.c_int32(substeps), _ptr(scratch), C.c_size_t(4 * scratch.numel()), _stream()))
+    return hc, hp
+
+
 def mul_faces(dom: Domain, vbc, v, mask):
     """v_c *= mask_c on the stored faces (apply_boundary_conditions for stationary obstacles, fluid.py:212-240)."""
     require_cuda()

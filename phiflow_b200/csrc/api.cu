@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <vector>
 #include "phi_internal.cuh"
 #include "cg_common.cuh"
 #include "launch.cuh"
@@ -727,6 +728,99 @@ int phicuda_reaction_diffusion_f32(const PhiGrid* g, const PhiVBC* bc, float* u,
     const int e = phi_launch_reaction_diffusion(dg, fu, u, v, scratch, scratch + n, p, substeps, (cudaStream_t)stream);
     if (e == -100) { phi_set_error("reaction_diffusion: the grid does not fit the TMA ring on this device"); return PHI_ERR_UNSUPPORTED; }
     return cuda_fail(e, "reaction_diffusion");
+}
+
+// scratch of the wave step: [one centred array, for an odd count][substeps WaveDisc][cell centres along each axis]
+static size_t wave_tmp_bytes(const PhiGrid* g) { return (centred_elems(g) * sizeof(float) + 15) / 16 * 16; }
+static size_t wave_table_bytes(const PhiGrid* g, int32_t substeps)
+{
+    return (size_t)substeps * sizeof(WaveDisc) + (size_t)(g->n[0] + g->n[1] + (g->dim == 3 ? g->n[2] : 0)) * sizeof(float);
+}
+
+size_t phicuda_wave_scratch_bytes(const PhiGrid* g, int32_t substeps)
+{
+    return g && substeps >= 0 ? wave_tmp_bytes(g) + wave_table_bytes(g, substeps) : 0;
+}
+
+int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, float dd, float k_speed, float k_damp,
+                     const PhiWaveDisc* discs, float radius_sq, const float* centers, int32_t substeps, void* scratch,
+                     size_t scratch_bytes, void* stream)
+{
+    // every check runs before the first CUDA call: a refused call leaves h_c and h_p untouched
+    DGrid dg; DField f;
+    CHECK(phi_make_dgrid(g, &dg));
+    if (!bc || !h_c || !h_p || !discs || !centers || !scratch) { phi_set_error("wave: NULL argument"); return PHI_ERR_INVALID; }
+    if (substeps < 0) { phi_set_error("wave: substeps must be >= 0, got %d", substeps); return PHI_ERR_INVALID; }
+    if (!std::isfinite(dd) || !std::isfinite(k_speed) || !std::isfinite(k_damp) || !std::isfinite(radius_sq)) {
+        phi_set_error("wave: dd, k_speed, k_damp and radius_sq must be finite"); return PHI_ERR_INVALID;
+    }
+    const int naxis = g->n[0] + g->n[1] + (g->dim == 3 ? g->n[2] : 0);
+    for (int i = 0; i < naxis; ++i)
+        if (!std::isfinite(centers[i])) { phi_set_error("wave: cell centre %d is not finite", i); return PHI_ERR_INVALID; }
+    for (int s = 0; s < substeps; ++s) {
+        if (!discs[s].present) continue;
+        bool ok = std::isfinite(discs[s].value);
+        for (int a = 0; a < g->dim; ++a) ok = ok && std::isfinite(discs[s].center[a]);
+        if (!ok) { phi_set_error("wave: disc %d has a non-finite centre or value", s); return PHI_ERR_INVALID; }
+    }
+    const size_t n = centred_elems(g);
+    const size_t need = phicuda_wave_scratch_bytes(g, substeps);
+    if (scratch_bytes < need) { phi_set_error("wave: scratch %zu < %zu bytes", scratch_bytes, need); return PHI_ERR_INVALID; }
+    auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
+        const char* x = (const char*)a; const char* y = (const char*)b; return x < y + nb && y < x + na;
+    };
+    if (overlap(h_c, 4 * n, h_p, 4 * n)) { phi_set_error("wave: h_c and h_p must be distinct arrays (they overlap)"); return PHI_ERR_INVALID; }
+    if (overlap(scratch, need, h_c, 4 * n) || overlap(scratch, need, h_p, 4 * n)) {
+        phi_set_error("wave: scratch overlaps h_c or h_p"); return PHI_ERR_INVALID;
+    }
+    if (g->halo != 0) { phi_set_error("wave: z-slab grids are not supported"); return PHI_ERR_UNSUPPORTED; }
+    CHECK(phi_make_centered(g, bc, &f));
+    for (int a = 0; a < g->dim; ++a)
+        if ((bc->lo[a] == PHI_BC_CONST && bc->clo[a] != 0.f) || (bc->hi[a] == PHI_BC_CONST && bc->chi[a] != 0.f)) {
+            phi_set_error("wave: non-zero constant boundary on axis %d: the reference's step turns a constant c into c - c = 0 "
+                          "(2.0 * h_c keeps h_c's extrapolation), so its ghosts are not fixed", a);
+            return PHI_ERR_UNSUPPORTED;
+        }
+    if (!phi_ring_enabled()) { phi_set_error("wave: runs on the TMA ring kernel only, which PHICUDA_NO_RING switches off"); return PHI_ERR_UNSUPPORTED; }
+    if (!phi_wave_ring_fits(dg)) {
+        phi_set_error("wave: grid lines of %d cells do not fit the TMA ring (%d-D: at most %d cells)", g->n[0], g->dim, phi_wave_ring_max_width(dg));
+        return PHI_ERR_UNSUPPORTED;
+    }
+    if (substeps == 0) return 0;
+    // the disc table: per axis the index range of cells whose own term fl(fl(p - c)^2) is <= r^2 (the float32 operations of the
+    // kernel's test), which holds every cell of the disc because a float sum of non-negative terms is no smaller than any term
+    std::vector<unsigned char> table(wave_table_bytes(g, substeps));
+    WaveDisc* wd = reinterpret_cast<WaveDisc*>(table.data());
+    for (int s = 0; s < substeps; ++s) {
+        WaveDisc d; memset(&d, 0, sizeof(d));
+        d.value = discs[s].value;
+        for (int a = 0; a < 3; ++a) d.c[a] = a < g->dim ? discs[s].center[a] : 0.f;
+        bool empty = !discs[s].present;
+        const float* p = centers;
+        for (int a = 0; a < g->dim && !empty; p += g->n[a], ++a) {
+            int lo = g->n[a], hi = 0;
+            for (int i = 0; i < g->n[a]; ++i) {
+                const float t = p[i] - d.c[a];
+                const float t2 = t * t;
+                if (t2 <= radius_sq) { if (i < lo) lo = i; hi = i + 1; }
+            }
+            if (lo >= hi) empty = true;
+            d.lo[a] = lo; d.hi[a] = hi;
+        }
+        if (g->dim == 2) { d.lo[2] = 0; d.hi[2] = 1; }
+        if (empty) for (int a = 0; a < 3; ++a) d.lo[a] = d.hi[a] = 0;
+        wd[s] = d;
+    }
+    memcpy(table.data() + (size_t)substeps * sizeof(WaveDisc), centers, (size_t)naxis * sizeof(float));
+    unsigned char* dtab = (unsigned char*)scratch + wave_tmp_bytes(g);
+    cudaError_t ce = cudaMemcpyAsync(dtab, table.data(), table.size(), cudaMemcpyHostToDevice, (cudaStream_t)stream);
+    if (ce != cudaSuccess) return cuda_fail((int)ce, "wave");
+    WaveParams wp;
+    wp.dd = dd; wp.k_speed = k_speed; wp.k_damp = k_damp; wp.r2 = radius_sq;
+    const int e = phi_launch_wave(dg, f, h_c, h_p, (float*)scratch, reinterpret_cast<const WaveDisc*>(dtab),
+                                  reinterpret_cast<const float*>(dtab + (size_t)substeps * sizeof(WaveDisc)), wp, substeps, (cudaStream_t)stream);
+    if (e == -100) { phi_set_error("wave: the grid does not fit the TMA ring on this device"); return PHI_ERR_UNSUPPORTED; }
+    return cuda_fail(e, "wave");
 }
 
 }  // extern "C"

@@ -99,3 +99,14 @@ bool phi_rd_ring_fits(const DGrid& g);                 // host-only, no CUDA cal
 int phi_rd_ring_max_width(const DGrid& g);             // widest line (cells) the ring takes for g's other extents; host-only
 int phi_launch_reaction_diffusion(const DGrid& g, const DField& f, float* u, float* v, float* su, float* sv, const RdParams& p,
                                   int substeps, cudaStream_t s);
+// N8 the Waves notebook's wave step on the TMA ring (ring_kernels.cu).  -100: the grid does not fit the ring.
+// WaveDisc: the disc stamped in one substep; lo / hi: per axis the index range of cells whose own axis term (p - c)^2 is <= r^2, a
+// box that holds every cell of the disc (empty, lo = hi = 0, when the substep has no disc).
+struct WaveDisc { float c[3]; float value; int lo[3], hi[3]; };
+struct WaveParams { float dd, k_speed, k_damp, r2; };
+bool phi_wave_ring_fits(const DGrid& g);               // host-only, no CUDA call
+int phi_wave_ring_max_width(const DGrid& g);           // widest line (cells) the ring takes for g's other extents; host-only
+// discs: `substeps` entries in device memory; coords: per-axis cell centres (n[0] x, then n[1] y, then n[2] z) in device memory;
+// tmp: one centred array, written only for an odd substep count
+int phi_launch_wave(const DGrid& g, const DField& f, float* hc, float* hp, float* tmp, const WaveDisc* discs, const float* coords,
+                    const WaveParams& p, int substeps, cudaStream_t s);

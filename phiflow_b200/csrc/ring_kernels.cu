@@ -280,6 +280,9 @@ __device__ __forceinline__ void groups_tile(ThreadGroups& tg, const RingCfg& cfg
 // tile or the variant that computed it.
 template <class E, class = void> struct RingTwoFields : std::false_type {};
 template <class E> struct RingTwoFields<E, std::void_t<decltype(E::kTwoFields)>> : std::integral_constant<bool, E::kTwoFields> {};
+// Epilogues that declare kRefStencil (the wave step, N8) take the one haloed array's laplacian from stencil_ref as well, for the same reason.
+template <class E, class = void> struct RingRefStencil : RingTwoFields<E> {};
+template <class E> struct RingRefStencil<E, std::void_t<decltype(E::kRefStencil)>> : std::integral_constant<bool, E::kRefStencil> {};
 
 // sum over axes of (lower + upper - 2 c) / dx^2 in oracle_np.laplace's order, each operation rounded on its own (no contraction)
 __device__ __forceinline__ float lap_axis(float lo, float hi, float c, float idx2)
@@ -413,7 +416,7 @@ __device__ __forceinline__ void ring_compute(const RingCfg& cfg, const DGrid& g,
                 if (ac.w == 0.f) q.w = c.w;
                 epi.set_acc(ac);
             }
-        } else if constexpr (RingTwoFields<Epi>::value) {
+        } else if constexpr (RingRefStencil<Epi>::value) {
             const float4 zm = DIM == 3 ? (zm_const ? f4_splat(pf.clo[2]) : val4(sm, rc)) : c;
             const float4 zp = DIM == 3 ? (zp_const ? f4_splat(pf.chi[2]) : val4(sp, rc)) : c;
             q = stencil_ref<DIM>(c, make_float4(xl, c.x, c.y, c.z), r4, ym, yp, zm, zp, ix2, iy2, iz2);
@@ -483,7 +486,7 @@ __device__ __forceinline__ void ring_compute_fast(const RingCfg& cfg, const DGri
             if (tg.needr & (1u << k)) { xr = sc[tg.xro[k]]; if (use1) xr = fmaf(beta, sc[h1 + tg.xro[k]], xr); }
         }
         float4 q;
-        if constexpr (RingTwoFields<Epi>::value) {
+        if constexpr (RingRefStencil<Epi>::value) {
             const float4 zm = DIM == 3 ? val4(sm, rc) : c, zp = DIM == 3 ? val4(sp, rc) : c;
             q = stencil_ref<DIM>(c, make_float4(xl, c.x, c.y, c.z), make_float4(c.y, c.z, c.w, xr), ym, yp, zm, zp, ix2, iy2, iz2);
         } else {
@@ -2017,5 +2020,187 @@ int phi_launch_reaction_diffusion(const DGrid& g, const DField& f, float* u, flo
     e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(RING_THREADS), args, smem, s);
     if (e != cudaSuccess) { phi_set_error("reaction_diffusion: cooperative launch failed: %s", cudaGetErrorString(e)); return (int)e; }
     note_ring_launch(PHI_KERNEL_RD_RING, cfg, generic, false, false, grid);
+    return 0;
+}
+
+// ---- N8 wave step (the Waves notebook) -------------------------------------------------------------------------------------------
+// One substep of the notebook's step, per cell, with the disc of substep s stamped on both states first:
+//   h_c' = where(disc_s, v_s, h_c);  h_p' = where(disc_s, v_s, h_p)
+//   h_n = ((2 h_c') - h_p') + dd ((k_speed laplace(h_c')) - (k_damp (h_c' - h_p'))),   returns (h_n, h_c')
+// each operation rounded on its own, as the reference's float32 field arithmetic rounds it.  h_c is the one haloed array of a stage,
+// h_p the one element-wise array: it is read only at its own cell, so h_n overwrites h_p in place and the two arrays swap roles every
+// substep.  The stamp costs no pass over the grid: the stored h_c of substep s is always already stamped (by the epilogue of substep
+// s - 1, which stamps disc s on the h_n it writes, or by a pre-pass over disc 0's box), and h_p is stamped as it is read.
+// disc_s = { cells with ((p_x - c_x)^2 + (p_y - c_y)^2) [+ (p_z - c_z)^2] <= r^2 } at the float32 cell centres p (Sphere.lies_inside).
+struct WaveCoords { const float* p[3]; };     // cell centres along x, y, z
+__device__ __forceinline__ bool wave_in_disc(const WaveDisc& d, const WaveCoords& pc, float r2, int x, int y, int z, int dim)
+{
+    float t = __fsub_rn(pc.p[0][x], d.c[0]);
+    float s = __fmul_rn(t, t);
+    t = __fsub_rn(pc.p[1][y], d.c[1]);
+    s = __fadd_rn(s, __fmul_rn(t, t));
+    if (dim == 3) { t = __fsub_rn(pc.p[2][z], d.c[2]); s = __fadd_rn(s, __fmul_rn(t, t)); }
+    return s <= r2;
+}
+
+// the unit's lines [y0, y0 + TY) of planes [z0, z1) meet the disc's box
+template <int DIM>
+__device__ __forceinline__ bool wave_unit_hit(const WaveDisc& d, const RingCfg& cfg, const RingUnit& u)
+{
+    return d.lo[0] < d.hi[0] && d.lo[1] < u.y0 + cfg.TY && d.hi[1] > u.y0 && (DIM == 2 || (d.lo[2] < u.z1 && d.hi[2] > u.z0));
+}
+
+template <int DIM>
+struct REpiWave {
+    static constexpr bool kRefStencil = true;
+    float* hn;                 // h_n (the h_p array, or the scratch in the last substep of an odd count)
+    float* hc_out;             // the last substep of an odd count: h_c' goes to the h_p array; nullptr otherwise
+    WaveCoords pc; WaveParams p;
+    WaveDisc dp, dn;           // disc of this substep (stamped on h_p) and of the next one (stamped on h_n)
+    bool hit_p, hit_n;         // per unit: the unit meets dp's / dn's box
+    long long bbase, sz; int sy, z;
+    __device__ __forceinline__ void set_plane(int zz, int) { z = zz < 0 ? 0 : zz; }
+    __device__ __forceinline__ void set_acc(const float4&) {}
+    __device__ __forceinline__ void stamp(float4& v, const WaveDisc& d, int x0, int y, int nvalid) const
+    {
+        if (y < d.lo[1] || y >= d.hi[1] || x0 + 4 <= d.lo[0] || x0 >= d.hi[0] || (DIM == 3 && (z < d.lo[2] || z >= d.hi[2]))) return;
+        for (int j = 0; j < nvalid; ++j)
+            if (wave_in_disc(d, pc, p.r2, x0 + j, y, z, DIM)) f4_set(v, j, d.value);
+    }
+    __device__ __forceinline__ float cell(float c, float q, float hp) const
+    {
+        const float damp = __fmul_rn(p.k_damp, __fsub_rn(c, hp));
+        return __fadd_rn(__fsub_rn(__fmul_rn(2.f, c), hp), __fmul_rn(p.dd, __fsub_rn(__fmul_rn(p.k_speed, q), damp)));
+    }
+    __device__ __forceinline__ void operator()(long long off, const float4& c, const float4& q, int nvalid, const float4& e0, const float4&, const float4&)
+    {
+        float4 hp = e0;
+        int x0 = 0, y = 0;
+        if (hit_p || hit_n) {
+            const int rel = (int)(off - bbase - z * sz);
+            y = rel / sy; x0 = rel - y * sy;
+        }
+        if (hit_p) stamp(hp, dp, x0, y, nvalid);
+        float4 h = make_float4(cell(c.x, q.x, hp.x), cell(c.y, q.y, hp.y), cell(c.z, q.z, hp.z), cell(c.w, q.w, hp.w));
+        if (hit_n) stamp(h, dn, x0, y, nvalid);
+        if (nvalid == 4) {
+            *reinterpret_cast<float4*>(hn + off) = h;
+            if (hc_out) *reinterpret_cast<float4*>(hc_out + off) = c;
+        } else {
+            for (int j = 0; j < nvalid; ++j) { hn[off + j] = f4_get(h, j); if (hc_out) hc_out[off + j] = f4_get(c, j); }
+        }
+    }
+};
+
+// All substeps of one call in one cooperative launch.  Before the loop, disc 0 is stamped on h_c over its box.  Substep s reads the
+// array a (h_c, staged with halo lines) and b (h_p, element-wise) and writes h_n into b; then a and b swap.  After an even count
+// the newest state is in hc and the previous (stamped) one in hp.  For an odd count the last substep writes h_n into the scratch and
+// h_c' into hp, and a final pass copies the scratch into hc.  12 B/cell per substep (+ 12 B/cell once for an odd count, + the box of
+// disc 0).  Between substeps the fence / grid-sync / async-proxy-fence sequence of k_rd_ring.
+template <int DIM, bool GENERIC>
+__global__ void __launch_bounds__(RING_THREADS, 1)
+k_wave_ring(DGrid g, DField f, RingCfg cfg, float* hc, float* hp, float* tmp, const WaveDisc* discs, const float* coords, WaveParams p,
+            int substeps)
+{
+    extern __shared__ __align__(128) unsigned char smem[];
+    Ring rg;
+    ring_init(rg, smem, cfg);
+    cg::grid_group grid = cg::this_grid();
+    ThreadGroups tg;
+    groups_init(tg, cfg, g, f);
+    auto barrier = [&] { fence_proxy_async(); grid.sync(); fence_proxy_async(); };
+    const bool odd = substeps & 1;
+    const WaveCoords pc = {{coords, coords + g.n[0], coords + g.n[0] + g.n[1]}};
+    {
+        const WaveDisc d = discs[0];
+        const int bx = d.hi[0] - d.lo[0], by = d.hi[1] - d.lo[1], bz = DIM == 3 ? d.hi[2] - d.lo[2] : 1;
+        if (bx > 0 && by > 0 && bz > 0) {
+            const long long cells = (long long)bx * by * bz * g.batch;
+            for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < cells; i += (long long)gridDim.x * blockDim.x) {
+                long long r = i;
+                const int x = d.lo[0] + (int)(r % bx); r /= bx;
+                const int y = d.lo[1] + (int)(r % by); r /= by;
+                const int z = DIM == 3 ? d.lo[2] + (int)(r % bz) : 0;
+                const int b = (int)(r / bz);
+                if (wave_in_disc(d, pc, p.r2, x, y, z, DIM))
+                    hc[(long long)b * f.sb + (long long)z * f.sz + (long long)y * f.sy + x] = d.value;
+            }
+            barrier();
+        }
+    }
+    float* a = hc;
+    float* b = hp;
+    for (int s = 0; s < substeps; ++s) {
+        const bool last_odd = odd && s == substeps - 1;
+        REpiWave<DIM> epi;
+        epi.hn = last_odd ? tmp : b;
+        epi.hc_out = last_odd ? b : nullptr;
+        epi.pc = pc; epi.p = p; epi.z = 0; epi.sy = (int)f.sy; epi.sz = f.sz;
+        epi.dp = discs[s];
+        if (s + 1 < substeps) epi.dn = discs[s + 1];
+        const float* hsrc[1] = {a};
+        const float* esrc[1] = {b};
+        for (int unit = blockIdx.x; unit < cfg.total_units; unit += gridDim.x) {
+            const RingUnit u = ring_unit<DIM>(cfg, g, unit);
+            epi.hit_p = wave_unit_hit<DIM>(epi.dp, cfg, u);
+            epi.hit_n = s + 1 < substeps && wave_unit_hit<DIM>(epi.dn, cfg, u);
+            epi.bbase = (long long)u.b * f.sb;
+            ring_process_unit<GENERIC, DIM, 1, 1, false>(rg, cfg, g, f, tg, hsrc, esrc, 0.f, u, epi);
+        }
+        if (s + 1 < substeps || last_odd) barrier();
+        float* t = a; a = b; b = t;
+    }
+    if (odd)
+        for (int unit = blockIdx.x; unit < cfg.total_units; unit += gridDim.x)
+            ring_unit_cells<DIM>(cfg, g, f, tg, ring_unit<DIM>(cfg, g, unit), [&](long long off, int nvalid) {
+                for (int j = 0; j < nvalid; ++j) hc[off + j] = tmp[off + j];
+            });
+}
+
+// stage = h_c with its halo lines + h_p: 2 TY + 2 lines; the whole shared memory, one CTA per SM (cooperative launch)
+static bool wave_ring_config(const DGrid& g, int target_units, RingCfg* c)
+{
+    return ring_config(g, 2, 2, 0, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, target_units, c);
+}
+
+int phi_wave_ring_max_width(const DGrid& g)
+{
+    if (g.halo != 0) return 0;
+    for (int w = g.cext[0] < 4096 ? g.cext[0] / 4 * 4 : 4096; w >= 4; w -= 4) {       // ty * nx4 <= RING_G * 256: no line beyond 4096
+        DGrid h = g; h.n[0] = w; h.cext[0] = w;
+        RingCfg c;
+        if (wave_ring_config(h, 1, &c)) return w;
+    }
+    return 0;
+}
+
+bool phi_wave_ring_fits(const DGrid& g)
+{
+    RingCfg c;
+    return g.halo == 0 && wave_ring_config(g, 1, &c);
+}
+
+int phi_launch_wave(const DGrid& g, const DField& f, float* hc, float* hp, float* tmp, const WaveDisc* discs, const float* coords,
+                    const WaveParams& p, int substeps, cudaStream_t s)
+{
+    const int sms = phi_sm_count();
+    RingCfg cfg;
+    if (!wave_ring_config(g, sms, &cfg)) return -100;
+    const size_t smem = 128 + (size_t)cfg.R * cfg.stage_floats * 4;
+    const bool generic = !ring_all_fast(g, f, cfg);
+    const void* fn = g.dim == 3 ? (generic ? (const void*)k_wave_ring<3, true> : (const void*)k_wave_ring<3, false>)
+                                : (generic ? (const void*)k_wave_ring<2, true> : (const void*)k_wave_ring<2, false>);
+    int per_sm = 0;
+    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, RING_THREADS, smem);
+    if (e != cudaSuccess) return (int)e;
+    if (per_sm < 1) return -100;
+    int grid = sms * per_sm;
+    if (grid > cfg.total_units) grid = cfg.total_units;
+    DGrid ga = g; DField fa = f; WaveParams pa = p; int ns = substeps;
+    void* args[] = {&ga, &fa, &cfg, &hc, &hp, &tmp, &discs, &coords, &pa, &ns};
+    e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(RING_THREADS), args, smem, s);
+    if (e != cudaSuccess) { phi_set_error("wave: cooperative launch failed: %s", cudaGetErrorString(e)); return (int)e; }
+    note_ring_launch(PHI_KERNEL_WAVE_RING, cfg, generic, false, false, grid);
     return 0;
 }

@@ -4,9 +4,10 @@
 
 Mirrored (same names, argument meaning and error behaviour; reference file:line in each docstring):
     Box, Sphere, union, geom.infinite_cylinder, CenteredGrid, StaggeredGrid, extrapolation (ZERO, ONE, PERIODIC, ZERO_GRADIENT, BOUNDARY, combine_sides),
-    Solve, SolveTape, NotConverged, Diverged, field.{divergence, laplace, spatial_gradient}, resample,
+    Solve, SolveTape, NotConverged, Diverged, math.{sin, PI, rotate_vector}, field.{divergence, laplace, spatial_gradient, where}, resample,
     advect.{semi_lagrangian, mac_cormack, advect}, diffuse.{explicit, implicit}, fluid.{make_incompressible, incompressible_step},
     write / read (field.write / field.read: the reference's .npz field files, see field_io.py).
+Fused notebook steps (one kernel launch for all substeps of a call): reaction_diffusion (Reaction_Diffusion), wave_step (Waves).
 Fields hold device tensors in the library layout (DESIGN.md section 2); `.numpy()` returns the reference's (x, y[, z]) arrays.
 Anything outside the fast path raises NotImplementedError (where the reference-side façade would fall through to stock
 PhiFlow, INTEGRATION.md section 2).  No CPU fallback.
@@ -25,7 +26,7 @@ from . import scene as _scene
 
 __all__ = ['Scene', 'vec', 'batch', 'iterate', 'jit_compile', 'Box', 'Sphere', 'union', 'geom', 'CenteredGrid', 'StaggeredGrid', 'extrapolation', 'ZERO', 'ONE', 'PERIODIC', 'ZERO_GRADIENT',
            'BOUNDARY', 'combine_sides', 'Solve', 'SolveTape', 'NotConverged', 'Diverged', 'ConvergenceException', 'field',
-           'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read']
+           'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read', 'wave_step']
 
 AXES = 'xyz'
 
@@ -131,6 +132,12 @@ class Box:
         self.lower = {k: float(v[0]) if isinstance(v, (tuple, list)) else 0.0 for k, v in dims.items()}
         self.upper = {k: float(v[1]) if isinstance(v, (tuple, list)) else float(v) for k, v in dims.items()}
 
+    @property
+    def center(self):
+        """Box.center (phi/geom/_box.py:109): (lower + upper) / 2 as a float32 NumPy vector, so that `bounds.center + vector` adds
+        element by element (a `vec` is a tuple here, and tuple + tuple would concatenate)."""
+        return np.array([(self.lower[k] + self.upper[k]) * 0.5 for k in self.names], np.float32)
+
     def lies_inside(self, pts):
         ok = np.ones(pts.shape[:-1], bool)
         for i, k in enumerate(self.names):
@@ -148,10 +155,15 @@ class Box:
 
 
 class Sphere:
-    """Sphere(x=50, y=9.5, radius=5)  (phi/geom/_sphere.py)."""
+    """Sphere(x=50, y=9.5, radius=5) or Sphere(center=vector, radius=1.)  (phi/geom/_sphere.py)."""
 
-    def __init__(self, radius, **center):
-        self.names, self.center, self.radius = tuple(center), tuple(float(v) for v in center.values()), float(radius)
+    def __init__(self, radius=None, center=None, **center_):
+        _require(radius is not None and (center is None) != (not center_), "Sphere without a radius, or with both `center` and axis keywords")
+        if center is not None:
+            center = np.asarray(center, np.float32).reshape(-1)
+            _require(len(center) in (2, 3), f"Sphere centre of {len(center)} components")
+            center_ = dict(zip(AXES, center))
+        self.names, self.center, self.radius = tuple(center_), tuple(float(v) for v in center_.values()), float(radius)
 
     def lies_inside(self, pts):
         return np.sum((pts - np.asarray(self.center, np.float32)) ** 2, -1) <= self.radius ** 2
@@ -285,8 +297,23 @@ class SolveTape:
         return len(self.records)
 
 
+def _sin(x):
+    """math.sin of a plain number: float32, as PhiML's NumPy backend returns it."""
+    _require(isinstance(x, numbers.Real) and not isinstance(x, bool), "math.sin of anything but a plain number")
+    return np.sin(np.float32(x))
+
+
+def rotate_vector(vector, angle):
+    """math.rotate_vector (PhiML/phiml/math/_nd.py:195-215) of a 2-D vector by a plain-number angle: (cos v_x - sin v_y,
+    sin v_x + cos v_y) with sin and cos of the float32 angle, every operation in float32.  Returns a float32 NumPy vector."""
+    v = np.asarray(vector, np.float32).reshape(-1)
+    _require(len(v) == 2 and isinstance(angle, numbers.Real) and not isinstance(angle, bool), "rotate_vector other than 2-D by a plain number")
+    s, c = np.sin(np.float32(angle)), np.cos(np.float32(angle))
+    return np.array([c * v[0] + (-s) * v[1], s * v[0] + c * v[1]], np.float32)
+
+
 math = SimpleNamespace(Solve=Solve, SolveTape=SolveTape, NotConverged=NotConverged, Diverged=Diverged,
-                       ConvergenceException=ConvergenceException, extrapolation=extrapolation)
+                       ConvergenceException=ConvergenceException, extrapolation=extrapolation, sin=_sin, PI=np.pi, rotate_vector=rotate_vector)
 
 
 def jit_compile(f=None, **_):
@@ -387,6 +414,13 @@ class CenteredGrid(_Grid):
         axes = [(np.linspace(0.5 / n, 1 - 0.5 / n, n).astype(np.float32) * np.float32(u - l) + np.float32(l)) for l, u, n in zip(self.lower, self.upper, self.res)]
         return np.stack(np.meshgrid(*axes, indexing='ij'), -1).astype(np.float32)
 
+    def axis_centres(self):
+        """The reference's float32 cell centres along each axis, bit for bit (UniformGrid.center, phi/geom/_grid.py:60-63):
+        PhiML's linspace runs in float32 (its limits arrive as float32 numbers), then lower + local * size.  `points()` forms the
+        linspace in float64 and can differ by one ulp; the disc masks of field.where and wave_step use these."""
+        return [np.linspace(np.float32(0.5 / n), np.float32(1 - 0.5 / n), n, dtype=np.float32) * np.float32(u - l) + np.float32(l)
+                for l, u, n in zip(self.lower, self.upper, self.res)]
+
     @property
     def spec(self):
         return self.boundary.spec(self.axes)
@@ -438,6 +472,10 @@ class CenteredGrid(_Grid):
     def __pow__(self, power):
         _require(isinstance(power, numbers.Real) and not isinstance(power, bool), "a power other than a plain number")
         return self.with_values(self.data ** float(power))
+
+    def laplace(self, order=2):
+        """Field.laplace (phi/field/_field.py:563-573) = field.laplace(self)."""
+        return laplace(self, order)
 
 
 class StaggeredGrid(_Grid):
@@ -638,7 +676,28 @@ def read(file: str):
     return StaggeredGrid(comps, boundary, bounds, batch, **res)
 
 
-field = SimpleNamespace(divergence=divergence, laplace=laplace, spatial_gradient=spatial_gradient, resample=resample,
+def where(mask, field_true, field_false):
+    """field.where (phi/field/_field_math.py:997-1015) on CenteredGrids with a hard mask: mask is a geometry (Box / Sphere / union,
+    sampled at the cell centres: _resample.py:192-210, Sphere.lies_inside, phi/geom/_sphere.py:103-105) or a CenteredGrid (non-zero
+    = True); field_true / field_false are CenteredGrids or plain numbers.  The result carries the extrapolation of the first field
+    among (field_true, field_false, mask), as _auto_resample resamples everything onto it."""
+    fields = [f for f in (field_true, field_false, mask) if isinstance(f, CenteredGrid)]
+    _require(bool(fields), "field.where without a CenteredGrid")
+    ref = fields[0]
+    _require(all(f._same_grid(ref) and f.vector_scale is None for f in fields), "field.where of vector fields or fields on different grids")
+    plain = lambda x: isinstance(x, numbers.Real) and not isinstance(x, bool)
+    _require(all(isinstance(x, CenteredGrid) or plain(x) for x in (field_true, field_false)), "field.where with non-number values")
+    if isinstance(mask, CenteredGrid):
+        m = mask.data != 0
+    else:
+        _require(isinstance(mask, (Box, Sphere, Union)), f"field.where with a {type(mask).__name__} mask")
+        pts = np.stack(np.meshgrid(*ref.axis_centres(), indexing='ij'), -1)
+        m = ref.dom.centered_from_numpy(mask.lies_inside(pts).astype(np.float32)) != 0
+    val = lambda x: x.data if isinstance(x, CenteredGrid) else torch.tensor(np.float32(x), device=ref.data.device)
+    return ref.with_values(torch.where(m, val(field_true), val(field_false)))
+
+
+field = SimpleNamespace(divergence=divergence, laplace=laplace, spatial_gradient=spatial_gradient, resample=resample, where=where,
                         CenteredGrid=CenteredGrid, StaggeredGrid=StaggeredGrid, write=write, read=read)
 
 
@@ -792,6 +851,45 @@ def reaction_diffusion(u: CenteredGrid, v: CenteredGrid, du: float, dv: float, f
              "reaction-diffusion with different boundary kinds for u and v")
     un, vn = ops.reaction_diffusion(u.dom, [su, sv], u.data, v.data, float(du), float(dv), float(f), float(k), float(dt), substeps)
     return u.with_values(un), v.with_values(vn)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# waves  (examples/grids/Waves.ipynb)
+# ----------------------------------------------------------------------------------------------------------------------
+def wave_step(h_c: CenteredGrid, h_p: CenteredGrid, time, dt: float, k_speed: float = 1.0, k_damp: float = 0.0, substeps: int = 1,
+              source=None):
+    """The Waves notebook's step, `substeps` times in one kernel launch.  Per substep, at the substep's time:
+        sphere, value = source(time);  h_c, h_p = [field.where(sphere, value, f) for f in (h_c, h_p)]
+        h_n = 2.0 * h_c - h_p + dt * dt * (k_speed * h_c.laplace() - k_damp * (h_c - h_p));  h_c, h_p, time = h_n, h_c, time + dt
+    with the rounding of the reference's float32 field arithmetic.  `source`: None (no disc) or a callable time -> (Sphere, value),
+    evaluated on the host for every substep; one disc per substep for every batch entry, one radius per call.  Returns (h_n, h_c,
+    time): the newest state, the previous (stamped) one and the advanced time.  h_c and h_p are not modified and may be the same field
+    (the notebook passes h0, h0).  Boundaries: PERIODIC, ZERO_GRADIENT and ZERO per side; a non-zero constant c drifts to 0 under
+    the reference's step (2.0 * h_c keeps h_c's extrapolation) and raises NotImplementedError."""
+    plain = lambda x: isinstance(x, numbers.Real) and not isinstance(x, bool)
+    _require(isinstance(h_c, CenteredGrid) and isinstance(h_p, CenteredGrid), "the wave step of non-centred fields")
+    _require(h_c.vector_scale is None and h_p.vector_scale is None, "the wave step of vector fields")
+    _require(h_c._same_grid(h_p) and h_c.boundary == h_p.boundary, "the wave step of fields on different grids or with different boundaries")
+    _require(all(plain(x) for x in (time, dt, k_speed, k_damp)), "the wave step with Field / per-batch parameters")
+    _require(isinstance(substeps, int) and substeps >= 0, f"substeps = {substeps!r}")
+    _require(all(_fixed_point_side(s) for ax in h_c.spec for s in ax),
+             f"the wave step with a non-zero constant boundary ({h_c.boundary}): the reference's step moves it to c - c = 0")
+    discs, radius = [], None
+    for _ in builtins_range(substeps):
+        if source is None:
+            discs.append(None)
+        else:
+            sphere, value = source(time)
+            _require(isinstance(sphere, Sphere) and sphere.names == h_c.axes, f"a {type(sphere).__name__} source (a Sphere over the grid's axes is on the fast path)")
+            _require(plain(value), "a source value that is not a plain number")
+            _require(radius is None or sphere.radius == radius, "sources of different radii in one call")
+            radius = sphere.radius
+            discs.append((np.asarray(sphere.center, np.float32), np.float32(value)))
+        time = time + dt
+    r2 = np.float32((radius if radius is not None else 0.0) ** 2)
+    hn, hc = ops.wave(h_c.dom, h_c.spec, h_c.data, h_p.data, np.float32(dt * dt), float(k_speed), float(k_damp), discs, r2,
+                      np.concatenate(h_c.axis_centres()), substeps)
+    return h_c.with_values(hn), h_c.with_values(hc), time
 
 
 # ----------------------------------------------------------------------------------------------------------------------
