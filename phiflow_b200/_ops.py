@@ -439,6 +439,16 @@ def diffuse_implicit_varying(dom: Domain, spec, u, k, dt: float, rtol=1e-5, atol
     return x
 
 
+def _cached_scratch(dom: Domain, attr: str, nbytes: int) -> torch.Tensor:
+    """A float32 scratch tensor of at least nbytes bytes, cached on dom as `attr` and replaced by a larger one when a call needs more.
+    Each caller keeps its own attribute: calls of different functions may run on different streams."""
+    s = getattr(dom, attr, None)
+    if s is None or 4 * s.numel() < nbytes:
+        s = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=dom.device)
+        setattr(dom, attr, s)
+    return s
+
+
 def reaction_diffusion(dom: Domain, spec, u, v, du: float, dv: float, f: float, k: float, dt: float, substeps: int = 1):
     """`substeps` Gray-Scott substeps of the Reaction_Diffusion notebook in one launch (include/phicuda.h, N7):
     uvv = u * v**2, u += dt * (du * laplace(u) - uvv + f * (1 - u)), v += dt * (dv * laplace(v) + uvv - (f + k) * v).
@@ -449,10 +459,7 @@ def reaction_diffusion(dom: Domain, spec, u, v, du: float, dv: float, f: float, 
     shape = dom._shape(dom.cext)
     assert tuple(u.shape) == shape and tuple(v.shape) == shape, f"u, v: shapes {tuple(u.shape)}, {tuple(v.shape)} are not centred arrays of the domain"
     un, vn = u.clone(), v.clone()
-    if getattr(dom, '_rd_scratch', None) is None:
-        n = _lib.load().phicuda_reaction_diffusion_scratch_bytes(C.byref(dom.grid))
-        dom._rd_scratch = torch.empty(n // 4, dtype=torch.float32, device=dom.device)
-    s = dom._rd_scratch
+    s = _cached_scratch(dom, '_rd_scratch', _lib.load().phicuda_reaction_diffusion_scratch_bytes(C.byref(dom.grid)))
     _lib.check(_lib.load().phicuda_reaction_diffusion_f32(C.byref(dom.grid), C.byref(make_vbc(spec, 2)), _ptr(un), _ptr(vn), C.c_float(du),
                                                           C.c_float(dv), C.c_float(f), C.c_float(k), C.c_float(dt), C.c_int32(substeps),
                                                           _ptr(s), C.c_size_t(4 * s.numel()), _stream()))
@@ -480,10 +487,7 @@ def wave(dom: Domain, spec, h_c, h_p, dd: float, k_speed: float, k_damp: float, 
     assert coords.size == sum(dom.res), f"{coords.size} cell centres for resolution {dom.res}"
     hc, hp = h_c.clone(), h_p.clone()
     lib = _lib.load()
-    n = lib.phicuda_wave_scratch_bytes(C.byref(dom.grid), substeps)
-    scratch = getattr(dom, '_wave_scratch', None)
-    if scratch is None or 4 * scratch.numel() < n:
-        scratch = dom._wave_scratch = torch.empty((n + 3) // 4, dtype=torch.float32, device=dom.device)
+    scratch = _cached_scratch(dom, '_wave_scratch', lib.phicuda_wave_scratch_bytes(C.byref(dom.grid), substeps))
     _lib.check(lib.phicuda_wave_f32(C.byref(dom.grid), C.byref(make_bc(spec)), _ptr(hc), _ptr(hp), C.c_float(dd), C.c_float(k_speed),
                                     C.c_float(k_damp), table, C.c_float(radius_sq), coords.ctypes.data_as(C.POINTER(C.c_float)),
                                     C.c_int32(substeps), _ptr(scratch), C.c_size_t(4 * scratch.numel()), _stream()))

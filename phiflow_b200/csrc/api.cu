@@ -680,6 +680,19 @@ int phicuda_plume_step_masked_f32(const PhiGrid* g, const PhiVBC* vbc, const Phi
     return plume_step(g, vbc, sbc, v, s, p, inflow, accessible, face_factors, sp, prm, result, scratch, workspace, workspace_bytes, stream);
 }
 
+static bool overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes) { return (const char*)a < (const char*)b + b_bytes && (const char*)b < (const char*)a + a_bytes; }
+
+// a persistent stepper runs on its TMA ring only: refuses PHICUDA_NO_RING and lines longer than the ring takes, naming the widest
+static int ring_only(const char* name, const PhiGrid* g, const DGrid& dg, int kernel)
+{
+    if (!phi_ring_enabled()) { phi_set_error("%s: runs on the TMA ring kernel only, which PHICUDA_NO_RING switches off", name); return PHI_ERR_UNSUPPORTED; }
+    if (!phi_step_ring_fits(dg, kernel)) {
+        phi_set_error("%s: grid lines of %d cells do not fit the TMA ring (%d-D: at most %d cells)", name, g->n[0], g->dim, phi_step_ring_max_width(dg, kernel));
+        return PHI_ERR_UNSUPPORTED;
+    }
+    return 0;
+}
+
 size_t phicuda_reaction_diffusion_scratch_bytes(const PhiGrid* g)
 {
     return g ? 2 * centred_elems(g) * sizeof(float) : 0;
@@ -699,9 +712,8 @@ int phicuda_reaction_diffusion_f32(const PhiGrid* g, const PhiVBC* bc, float* u,
     const size_t n = centred_elems(g);
     const size_t need = phicuda_reaction_diffusion_scratch_bytes(g);
     if (scratch_bytes < need) { phi_set_error("reaction_diffusion: scratch %zu < %zu bytes", scratch_bytes, need); return PHI_ERR_INVALID; }
-    auto overlap = [](const float* a, size_t na, const float* b, size_t nb) { return a < b + nb && b < a + na; };
-    if (overlap(u, n, v, n)) { phi_set_error("reaction_diffusion: u and v must be distinct arrays (they overlap)"); return PHI_ERR_INVALID; }
-    if (overlap(scratch, 2 * n, u, n) || overlap(scratch, 2 * n, v, n)) {
+    if (overlap(u, 4 * n, v, 4 * n)) { phi_set_error("reaction_diffusion: u and v must be distinct arrays (they overlap)"); return PHI_ERR_INVALID; }
+    if (overlap(scratch, need, u, 4 * n) || overlap(scratch, need, v, 4 * n)) {
         phi_set_error("reaction_diffusion: scratch overlaps u or v"); return PHI_ERR_INVALID;
     }
     if (g->halo != 0) { phi_set_error("reaction_diffusion: z-slab grids are not supported"); return PHI_ERR_UNSUPPORTED; }
@@ -717,11 +729,7 @@ int phicuda_reaction_diffusion_f32(const PhiGrid* g, const PhiVBC* bc, float* u,
                 return PHI_ERR_UNSUPPORTED;
             }
     }
-    if (!phi_ring_enabled()) { phi_set_error("reaction_diffusion: runs on the TMA ring kernel only, which PHICUDA_NO_RING switches off"); return PHI_ERR_UNSUPPORTED; }
-    if (!phi_rd_ring_fits(dg)) {
-        phi_set_error("reaction_diffusion: grid lines of %d cells do not fit the TMA ring (%d-D: at most %d cells)", g->n[0], g->dim, phi_rd_ring_max_width(dg));
-        return PHI_ERR_UNSUPPORTED;
-    }
+    CHECK(ring_only("reaction_diffusion", g, dg, PHI_KERNEL_RD_RING));
     if (substeps == 0) return 0;
     RdParams p;
     p.du = du; p.dv = dv; p.f = f; p.fk = f + k; p.dt = dt;
@@ -766,9 +774,6 @@ int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, 
     const size_t n = centred_elems(g);
     const size_t need = phicuda_wave_scratch_bytes(g, substeps);
     if (scratch_bytes < need) { phi_set_error("wave: scratch %zu < %zu bytes", scratch_bytes, need); return PHI_ERR_INVALID; }
-    auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
-        const char* x = (const char*)a; const char* y = (const char*)b; return x < y + nb && y < x + na;
-    };
     if (overlap(h_c, 4 * n, h_p, 4 * n)) { phi_set_error("wave: h_c and h_p must be distinct arrays (they overlap)"); return PHI_ERR_INVALID; }
     if (overlap(scratch, need, h_c, 4 * n) || overlap(scratch, need, h_p, 4 * n)) {
         phi_set_error("wave: scratch overlaps h_c or h_p"); return PHI_ERR_INVALID;
@@ -781,11 +786,7 @@ int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, 
                           "(2.0 * h_c keeps h_c's extrapolation), so its ghosts are not fixed", a);
             return PHI_ERR_UNSUPPORTED;
         }
-    if (!phi_ring_enabled()) { phi_set_error("wave: runs on the TMA ring kernel only, which PHICUDA_NO_RING switches off"); return PHI_ERR_UNSUPPORTED; }
-    if (!phi_wave_ring_fits(dg)) {
-        phi_set_error("wave: grid lines of %d cells do not fit the TMA ring (%d-D: at most %d cells)", g->n[0], g->dim, phi_wave_ring_max_width(dg));
-        return PHI_ERR_UNSUPPORTED;
-    }
+    CHECK(ring_only("wave", g, dg, PHI_KERNEL_WAVE_RING));
     if (substeps == 0) return 0;
     // the disc table: per axis the index range of cells whose own term fl(fl(p - c)^2) is <= r^2 (the float32 operations of the
     // kernel's test), which holds every cell of the disc because a float sum of non-negative terms is no smaller than any term

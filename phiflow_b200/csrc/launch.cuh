@@ -93,10 +93,11 @@ bool phi_cg_ring_fits(const DGrid& g, CgOp op);
 // widest grid line the ring CG takes for g's other extents and batch (host-only; error messages of refused solves)
 int phi_cg_ring_max_width(const DGrid& g, CgOp op, bool adapt);
 int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField* cf, cudaStream_t s);
+// N7 / N8 persistent steppers on the TMA ring (ring_kernels.cu), kernel = PHI_KERNEL_RD_RING or PHI_KERNEL_WAVE_RING; host-only, no CUDA call
+bool phi_step_ring_fits(const DGrid& g, int kernel);
+int phi_step_ring_max_width(const DGrid& g, int kernel);   // widest line (cells) the stepper's ring takes for g's other extents
 // N7 reaction-diffusion on the TMA ring (ring_kernels.cu).  fk = f + k, rounded to float once.  -100: the grid does not fit the ring.
 struct RdParams { float du, dv, f, fk, dt; };
-bool phi_rd_ring_fits(const DGrid& g);                 // host-only, no CUDA call
-int phi_rd_ring_max_width(const DGrid& g);             // widest line (cells) the ring takes for g's other extents; host-only
 int phi_launch_reaction_diffusion(const DGrid& g, const DField& f, float* u, float* v, float* su, float* sv, const RdParams& p,
                                   int substeps, cudaStream_t s);
 // N8 the Waves notebook's wave step on the TMA ring (ring_kernels.cu).  -100: the grid does not fit the ring.
@@ -104,8 +105,6 @@ int phi_launch_reaction_diffusion(const DGrid& g, const DField& f, float* u, flo
 // box that holds every cell of the disc (empty, lo = hi = 0, when the substep has no disc).
 struct WaveDisc { float c[3]; float value; int lo[3], hi[3]; };
 struct WaveParams { float dd, k_speed, k_damp, r2; };
-bool phi_wave_ring_fits(const DGrid& g);               // host-only, no CUDA call
-int phi_wave_ring_max_width(const DGrid& g);           // widest line (cells) the ring takes for g's other extents; host-only
 // discs: `substeps` entries in device memory; coords: per-axis cell centres (n[0] x, then n[1] y, then n[2] z) in device memory;
 // tmp: one centred array, written only for an odd substep count
 int phi_launch_wave(const DGrid& g, const DField& f, float* hc, float* hp, float* tmp, const WaveDisc* discs, const float* coords,

@@ -1854,20 +1854,28 @@ bool phi_cg_ring_fits(const DGrid& g, CgOp op)
     return cg_ring_config(g, op, (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128), 1, &c);
 }
 
+// the widest grid line (cells, a multiple of 4, at most g's own) for which fits(h) holds, h being g with that line; 0: none
+template <class F>
+static int ring_max_width(const DGrid& g, F&& fits)
+{
+    for (int w = g.cext[0] < 4096 ? g.cext[0] / 4 * 4 : 4096; w >= 4; w -= 4) {       // ty * nx4 <= RING_G * 256: no line beyond 4096
+        DGrid h = g; h.n[0] = w; h.cext[0] = w;
+        if (fits(h)) return w;
+    }
+    return 0;
+}
+
 // the widest grid line (cells, a multiple of 4) that phi_launch_cg_ring takes for g's other extents and batch with operator op and
 // solver method adapt; 0: none (host-only, no CUDA call; for the error message of a refused solve)
 int phi_cg_ring_max_width(const DGrid& g, CgOp op, bool adapt)
 {
     if (g.batch > CG_MAX_BATCH || g.halo != 0) return 0;
     const int cgs = (int)((cg_smem_bytes(g.batch) + 127) / 128 * 128);
-    for (int w = g.cext[0] < 4096 ? g.cext[0] / 4 * 4 : 4096; w >= 4; w -= 4) {       // ty * nx4 <= RING_G * 256: no line beyond 4096
-        DGrid h = g; h.n[0] = w; h.cext[0] = w;
+    return ring_max_width(g, [&](const DGrid& h) {
         RingCfg c;
-        if (!cg_ring_config(h, op, cgs, 1, &c)) continue;
-        if (adapt && !cg_op_xslot(op) && c.TY == 1 && !ring_config(h, 4, 3, cgs, h.dim == 3 ? 4 : 2, RING_MAX_STAGES, 1, &c)) continue;
-        return w;
-    }
-    return 0;
+        if (!cg_ring_config(h, op, cgs, 1, &c)) return false;
+        return !(adapt && !cg_op_xslot(op) && c.TY == 1) || ring_config(h, 4, 3, cgs, h.dim == 3 ? 4 : 2, RING_MAX_STAGES, 1, &c);
+    });
 }
 
 // l.pf: boundary kinds with zeroed constants (the value ghosts of L0 / D0); cf[0 .. C-1]: the boundary with its constants of component
@@ -1900,6 +1908,27 @@ int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField* cf, cuda
         m.rhs = yb;
     }
     return phi_launch_cg_ring(m, nullptr, s);
+}
+
+// ---- persistent steppers (N7, N8): every substep of a call in one cooperative launch ------------------------------------------
+// Between two substeps: the generic-proxy stores of one substep must be visible to the TMA (async proxy) loads of the next one, whose
+// halo lines other CTAs wrote - the sequence k_cg_ring uses between passes.
+__device__ __forceinline__ void step_grid_sync(cg::grid_group& grid)
+{
+    fence_proxy_async();
+    grid.sync();
+    fence_proxy_async();
+}
+
+// d0 = s0 and, with TWO, d1 = s1 on every cell of this CTA's units
+template <int DIM, bool TWO>
+__device__ __forceinline__ void step_copy_units(const RingCfg& cfg, const DGrid& g, const DField& f, const ThreadGroups& tg,
+                                                float* d0, const float* s0, float* d1 = nullptr, const float* s1 = nullptr)
+{
+    for (int unit = blockIdx.x; unit < cfg.total_units; unit += gridDim.x)
+        ring_unit_cells<DIM>(cfg, g, f, tg, ring_unit<DIM>(cfg, g, unit), [&](long long off, int nvalid) {
+            for (int j = 0; j < nvalid; ++j) { d0[off + j] = s0[off + j]; if (TWO) d1[off + j] = s1[off + j]; }
+        });
 }
 
 // ---- N7 reaction-diffusion (Gray-Scott, the Reaction_Diffusion notebook) ------------------------------------------------------
@@ -1937,10 +1966,11 @@ struct REpiReactionDiffusion {
     }
 };
 
+// stage of k_rd_ring: u and v with their halo lines
+constexpr int RD_NH = 2, RD_NE = 0;
+
 // All substeps of one call in one cooperative launch.  The state ping-pongs between (u, v) and the scratch (su, sv) so that the last
-// substep writes (u, v); an odd count first copies (u, v) into the scratch.  Between substeps: the generic-proxy stores of this
-// substep must be visible to the TMA (async proxy) loads of the next one, whose halo lines other CTAs wrote - the sequence k_cg_ring
-// uses between passes.
+// substep writes (u, v); an odd count first copies (u, v) into the scratch.
 template <int DIM, bool GENERIC>
 __global__ void __launch_bounds__(RING_THREADS, 1)
 k_rd_ring(DGrid g, DField f, RingCfg cfg, float* u, float* v, float* su, float* sv, RdParams p, int substeps)
@@ -1951,15 +1981,11 @@ k_rd_ring(DGrid g, DField f, RingCfg cfg, float* u, float* v, float* su, float* 
     cg::grid_group grid = cg::this_grid();
     ThreadGroups tg;
     groups_init(tg, cfg, g, f);
-    auto barrier = [&] { fence_proxy_async(); grid.sync(); fence_proxy_async(); };
     float* src[2] = {u, v};
     float* dst[2] = {su, sv};
     if (substeps & 1) {
-        for (int unit = blockIdx.x; unit < cfg.total_units; unit += gridDim.x)
-            ring_unit_cells<DIM>(cfg, g, f, tg, ring_unit<DIM>(cfg, g, unit), [&](long long off, int nvalid) {
-                for (int j = 0; j < nvalid; ++j) { su[off + j] = u[off + j]; sv[off + j] = v[off + j]; }
-            });
-        barrier();
+        step_copy_units<DIM, true>(cfg, g, f, tg, su, u, sv, v);
+        step_grid_sync(grid);
         src[0] = su; src[1] = sv; dst[0] = u; dst[1] = v;
     }
     for (int s = 0; s < substeps; ++s) {
@@ -1968,59 +1994,11 @@ k_rd_ring(DGrid g, DField f, RingCfg cfg, float* u, float* v, float* su, float* 
         REpiReactionDiffusion epi;
         epi.un = dst[0]; epi.vn = dst[1]; epi.p = p;
         for (int unit = blockIdx.x; unit < cfg.total_units; unit += gridDim.x)
-            ring_process_unit<GENERIC, DIM, 2, 0, false>(rg, cfg, g, f, tg, hsrc, esrc, 0.f, ring_unit<DIM>(cfg, g, unit), epi);
-        if (s + 1 < substeps) barrier();
+            ring_process_unit<GENERIC, DIM, RD_NH, RD_NE, false>(rg, cfg, g, f, tg, hsrc, esrc, 0.f, ring_unit<DIM>(cfg, g, unit), epi);
+        if (s + 1 < substeps) step_grid_sync(grid);
         float* t0 = src[0]; float* t1 = src[1];
         src[0] = dst[0]; src[1] = dst[1]; dst[0] = t0; dst[1] = t1;
     }
-}
-
-// stage = u and v with their halo lines: 2 TY + 4 lines; the whole shared memory, one CTA per SM (cooperative launch)
-static bool rd_ring_config(const DGrid& g, int target_units, RingCfg* c)
-{
-    return ring_config(g, 2, 4, 0, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, target_units, c);
-}
-
-int phi_rd_ring_max_width(const DGrid& g)
-{
-    if (g.halo != 0) return 0;
-    for (int w = g.cext[0] < 4096 ? g.cext[0] / 4 * 4 : 4096; w >= 4; w -= 4) {       // ty * nx4 <= RING_G * 256: no line beyond 4096
-        DGrid h = g; h.n[0] = w; h.cext[0] = w;
-        RingCfg c;
-        if (rd_ring_config(h, 1, &c)) return w;
-    }
-    return 0;
-}
-
-bool phi_rd_ring_fits(const DGrid& g)
-{
-    RingCfg c;
-    return g.halo == 0 && rd_ring_config(g, 1, &c);
-}
-
-int phi_launch_reaction_diffusion(const DGrid& g, const DField& f, float* u, float* v, float* su, float* sv, const RdParams& p,
-                                  int substeps, cudaStream_t s)
-{
-    const int sms = phi_sm_count();
-    RingCfg cfg;
-    if (!rd_ring_config(g, sms, &cfg)) return -100;
-    const size_t smem = 128 + (size_t)cfg.R * cfg.stage_floats * 4;
-    const bool generic = !ring_all_fast(g, f, cfg);
-    const void* fn = g.dim == 3 ? (generic ? (const void*)k_rd_ring<3, true> : (const void*)k_rd_ring<3, false>)
-                                : (generic ? (const void*)k_rd_ring<2, true> : (const void*)k_rd_ring<2, false>);
-    int per_sm = 0;
-    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, RING_THREADS, smem);
-    if (e != cudaSuccess) return (int)e;
-    if (per_sm < 1) return -100;
-    int grid = sms * per_sm;
-    if (grid > cfg.total_units) grid = cfg.total_units;
-    DGrid ga = g; DField fa = f; RdParams pa = p; int ns = substeps;
-    void* args[] = {&ga, &fa, &cfg, &u, &v, &su, &sv, &pa, &ns};
-    e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(RING_THREADS), args, smem, s);
-    if (e != cudaSuccess) { phi_set_error("reaction_diffusion: cooperative launch failed: %s", cudaGetErrorString(e)); return (int)e; }
-    note_ring_launch(PHI_KERNEL_RD_RING, cfg, generic, false, false, grid);
-    return 0;
 }
 
 // ---- N8 wave step (the Waves notebook) -------------------------------------------------------------------------------------------
@@ -2092,11 +2070,14 @@ struct REpiWave {
     }
 };
 
+// stage of k_wave_ring: h_c with its halo lines, h_p element-wise
+constexpr int WAVE_NH = 1, WAVE_NE = 1;
+
 // All substeps of one call in one cooperative launch.  Before the loop, disc 0 is stamped on h_c over its box.  Substep s reads the
 // array a (h_c, staged with halo lines) and b (h_p, element-wise) and writes h_n into b; then a and b swap.  After an even count
 // the newest state is in hc and the previous (stamped) one in hp.  For an odd count the last substep writes h_n into the scratch and
 // h_c' into hp, and a final pass copies the scratch into hc.  12 B/cell per substep (+ 12 B/cell once for an odd count, + the box of
-// disc 0).  Between substeps the fence / grid-sync / async-proxy-fence sequence of k_rd_ring.
+// disc 0).
 template <int DIM, bool GENERIC>
 __global__ void __launch_bounds__(RING_THREADS, 1)
 k_wave_ring(DGrid g, DField f, RingCfg cfg, float* hc, float* hp, float* tmp, const WaveDisc* discs, const float* coords, WaveParams p,
@@ -2108,7 +2089,6 @@ k_wave_ring(DGrid g, DField f, RingCfg cfg, float* hc, float* hp, float* tmp, co
     cg::grid_group grid = cg::this_grid();
     ThreadGroups tg;
     groups_init(tg, cfg, g, f);
-    auto barrier = [&] { fence_proxy_async(); grid.sync(); fence_proxy_async(); };
     const bool odd = substeps & 1;
     const WaveCoords pc = {{coords, coords + g.n[0], coords + g.n[0] + g.n[1]}};
     {
@@ -2125,7 +2105,7 @@ k_wave_ring(DGrid g, DField f, RingCfg cfg, float* hc, float* hp, float* tmp, co
                 if (wave_in_disc(d, pc, p.r2, x, y, z, DIM))
                     hc[(long long)b * f.sb + (long long)z * f.sz + (long long)y * f.sy + x] = d.value;
             }
-            barrier();
+            step_grid_sync(grid);
         }
     }
     float* a = hc;
@@ -2145,62 +2125,79 @@ k_wave_ring(DGrid g, DField f, RingCfg cfg, float* hc, float* hp, float* tmp, co
             epi.hit_p = wave_unit_hit<DIM>(epi.dp, cfg, u);
             epi.hit_n = s + 1 < substeps && wave_unit_hit<DIM>(epi.dn, cfg, u);
             epi.bbase = (long long)u.b * f.sb;
-            ring_process_unit<GENERIC, DIM, 1, 1, false>(rg, cfg, g, f, tg, hsrc, esrc, 0.f, u, epi);
+            ring_process_unit<GENERIC, DIM, WAVE_NH, WAVE_NE, false>(rg, cfg, g, f, tg, hsrc, esrc, 0.f, u, epi);
         }
-        if (s + 1 < substeps || last_odd) barrier();
+        if (s + 1 < substeps || last_odd) step_grid_sync(grid);
         float* t = a; a = b; b = t;
     }
-    if (odd)
-        for (int unit = blockIdx.x; unit < cfg.total_units; unit += gridDim.x)
-            ring_unit_cells<DIM>(cfg, g, f, tg, ring_unit<DIM>(cfg, g, unit), [&](long long off, int nvalid) {
-                for (int j = 0; j < nvalid; ++j) hc[off + j] = tmp[off + j];
-            });
+    if (odd) step_copy_units<DIM, false>(cfg, g, f, tg, hc, tmp);
 }
 
-// stage = h_c with its halo lines + h_p: 2 TY + 2 lines; the whole shared memory, one CTA per SM (cooperative launch)
-static bool wave_ring_config(const DGrid& g, int target_units, RingCfg* c)
+// ---- host side of the persistent steppers -----------------------------------------------------------------------------------------
+// The ring of a stepper stages its NH haloed arrays with their halo lines and its NE element-wise arrays: (NH + NE) TY + 2 NH lines per
+// stage; the whole shared memory, one CTA per SM (cooperative launch).  kernel: PHI_KERNEL_RD_RING or PHI_KERNEL_WAVE_RING.
+static bool step_ring_config(const DGrid& g, int kernel, int target_units, RingCfg* c)
 {
-    return ring_config(g, 2, 2, 0, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, target_units, c);
-}
-
-int phi_wave_ring_max_width(const DGrid& g)
-{
-    if (g.halo != 0) return 0;
-    for (int w = g.cext[0] < 4096 ? g.cext[0] / 4 * 4 : 4096; w >= 4; w -= 4) {       // ty * nx4 <= RING_G * 256: no line beyond 4096
-        DGrid h = g; h.n[0] = w; h.cext[0] = w;
-        RingCfg c;
-        if (wave_ring_config(h, 1, &c)) return w;
+    int nh, ne;
+    switch (kernel) {
+    case PHI_KERNEL_RD_RING: nh = RD_NH; ne = RD_NE; break;
+    case PHI_KERNEL_WAVE_RING: nh = WAVE_NH; ne = WAVE_NE; break;
+    default: return false;
     }
-    return 0;
+    return ring_config(g, nh + ne, 2 * nh, 0, g.dim == 3 ? 4 : 2, RING_MAX_STAGES, target_units, c);
 }
 
-bool phi_wave_ring_fits(const DGrid& g)
+bool phi_step_ring_fits(const DGrid& g, int kernel)
 {
     RingCfg c;
-    return g.halo == 0 && wave_ring_config(g, 1, &c);
+    return g.halo == 0 && step_ring_config(g, kernel, 1, &c);
 }
 
-int phi_launch_wave(const DGrid& g, const DField& f, float* hc, float* hp, float* tmp, const WaveDisc* discs, const float* coords,
-                    const WaveParams& p, int substeps, cudaStream_t s)
+int phi_step_ring_max_width(const DGrid& g, int kernel)
 {
-    const int sms = phi_sm_count();
-    RingCfg cfg;
-    if (!wave_ring_config(g, sms, &cfg)) return -100;
+    return ring_max_width(g, [&](const DGrid& h) { return phi_step_ring_fits(h, kernel); });
+}
+
+// Sets the dynamic shared memory of fn, sizes the grid from its occupancy (at most one CTA per unit) and launches it cooperatively
+// with args.  -100: not even one CTA fits on an SM.  name: the stepper, in the error message of a failed launch.
+static int launch_step_ring(const void* fn, const RingCfg& cfg, void** args, int kernel, bool generic, const char* name, cudaStream_t s)
+{
     const size_t smem = 128 + (size_t)cfg.R * cfg.stage_floats * 4;
-    const bool generic = !ring_all_fast(g, f, cfg);
-    const void* fn = g.dim == 3 ? (generic ? (const void*)k_wave_ring<3, true> : (const void*)k_wave_ring<3, false>)
-                                : (generic ? (const void*)k_wave_ring<2, true> : (const void*)k_wave_ring<2, false>);
     int per_sm = 0;
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, RING_THREADS, smem);
     if (e != cudaSuccess) return (int)e;
     if (per_sm < 1) return -100;
-    int grid = sms * per_sm;
+    int grid = phi_sm_count() * per_sm;
     if (grid > cfg.total_units) grid = cfg.total_units;
+    e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(RING_THREADS), args, smem, s);
+    if (e != cudaSuccess) { phi_set_error("%s: cooperative launch failed: %s", name, cudaGetErrorString(e)); return (int)e; }
+    note_ring_launch(kernel, cfg, generic, false, false, grid);
+    return 0;
+}
+
+int phi_launch_reaction_diffusion(const DGrid& g, const DField& f, float* u, float* v, float* su, float* sv, const RdParams& p,
+                                  int substeps, cudaStream_t s)
+{
+    RingCfg cfg;
+    if (!step_ring_config(g, PHI_KERNEL_RD_RING, phi_sm_count(), &cfg)) return -100;
+    const bool generic = !ring_all_fast(g, f, cfg);
+    const void* fn = g.dim == 3 ? (generic ? (const void*)k_rd_ring<3, true> : (const void*)k_rd_ring<3, false>)
+                                : (generic ? (const void*)k_rd_ring<2, true> : (const void*)k_rd_ring<2, false>);
+    DGrid ga = g; DField fa = f; RdParams pa = p; int ns = substeps;
+    void* args[] = {&ga, &fa, &cfg, &u, &v, &su, &sv, &pa, &ns};
+    return launch_step_ring(fn, cfg, args, PHI_KERNEL_RD_RING, generic, "reaction_diffusion", s);
+}
+
+int phi_launch_wave(const DGrid& g, const DField& f, float* hc, float* hp, float* tmp, const WaveDisc* discs, const float* coords,
+                    const WaveParams& p, int substeps, cudaStream_t s)
+{
+    RingCfg cfg;
+    if (!step_ring_config(g, PHI_KERNEL_WAVE_RING, phi_sm_count(), &cfg)) return -100;
+    const bool generic = !ring_all_fast(g, f, cfg);
+    const void* fn = g.dim == 3 ? (generic ? (const void*)k_wave_ring<3, true> : (const void*)k_wave_ring<3, false>)
+                                : (generic ? (const void*)k_wave_ring<2, true> : (const void*)k_wave_ring<2, false>);
     DGrid ga = g; DField fa = f; WaveParams pa = p; int ns = substeps;
     void* args[] = {&ga, &fa, &cfg, &hc, &hp, &tmp, &discs, &coords, &pa, &ns};
-    e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(RING_THREADS), args, smem, s);
-    if (e != cudaSuccess) { phi_set_error("wave: cooperative launch failed: %s", cudaGetErrorString(e)); return (int)e; }
-    note_ring_launch(PHI_KERNEL_WAVE_RING, cfg, generic, false, false, grid);
-    return 0;
+    return launch_step_ring(fn, cfg, args, PHI_KERNEL_WAVE_RING, generic, "wave", s);
 }
