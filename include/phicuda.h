@@ -12,7 +12,9 @@
  *     cudaMalloc + cudaMemset + device synchronisation / CUDA-IPC open / cudaFree - once per run, never inside a step);
  *   - return 0 on success, a negative PHI_ERR_* or a positive cudaError_t otherwise; the message is kept per thread
  *     and read with phicuda_last_error();
- *   - fp32 only.  Other precisions are not part of this path (the reference falls through to its stock backends).
+ *   - fp32 (`_f32`) throughout; fp64 (`_f64`, math.set_global_precision(64)) for the stencils, semi-Lagrangian advection and the
+ *     CG pressure projection (see "fp64" below).  Other precisions are not part of this path (the reference falls through to its
+ *     stock backends).
  *
  * Device layout (one PhiGrid describes every array that lives on a domain):
  *   element (b, z, y, x)  at  ((b*E[2] + z)*E[1] + y)*E[0] + x               (x contiguous, z-slabs contiguous)
@@ -359,6 +361,63 @@ size_t phicuda_wave_scratch_bytes(const PhiGrid* g, int32_t substeps);
 int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, float dd, float k_speed, float k_damp,
                      const PhiWaveDisc* discs, float radius_sq, const float* centers, int32_t substeps, void* scratch,
                      size_t scratch_bytes, void* stream);
+
+/* ---- N9  fp64: the Taylor-Green step of math.set_global_precision(64) -----------------------------------------------------
+ * The same operations as their _f32 counterparts on float64 arrays (same layout, element size 8; x-rows stay padded to multiples of
+ * 4 elements).  PhiGrid and PhiBC / PhiVBC keep describing the layout and the boundary kinds; their float fields hold the exact
+ * values rounded to float, and PhiValues64 carries the exact values: every _f64 call returns PHI_ERR_INVALID unless
+ * (float) values->dx[a] == g->dx[a] and (float) values->clo / chi[c][a] == the boundary's clo / chi[a] on every axis a < dim of
+ * every component c < dim (a PhiBC argument: row c = 0).  The kernels compute in double throughout: 1 / dx is RN(1 / dx) in double,
+ * and CG step sizes, offsets, means, tolerances and |r|^2 are double.
+ * Single GPU: z-slab grids (halo != 0) return PHI_ERR_UNSUPPORTED.  The stencils and advection run one thread per sample; the
+ * solve is the register-marching persistent CG (phicuda_last_launch_info reports PHI_KERNEL_CG_MARCH), two sweeps and 64 B/cell per
+ * iteration.  PHICUDA_NO_RING and PHICUDA_SCALAR_KERNELS do not change this path.  Not offered in fp64: CG-adaptive (ring kernel
+ * only), obstacles, MacCormack, diffuse.implicit, the fused steps and CenteredGrid velocities. */
+typedef struct PhiValues64 {
+    double dx[3];           /* cell size per axis */
+    double clo[3][3];       /* [component][axis] constant of the lower side (unused, but still checked, where the kind is not PHI_BC_CONST) */
+    double chi[3][3];
+} PhiValues64;
+
+typedef struct PhiCgParams64 {
+    double  rtol;
+    double  atol;
+    int32_t max_iter;
+    int32_t balance_rhs;
+    int32_t project_mean;
+    double  matrix_offset;
+    int32_t method;          /* PHI_SOLVER_CG only */
+} PhiCgParams64;
+
+typedef struct PhiCgResult64 {
+    int32_t iterations;
+    int32_t converged;
+    int32_t diverged;
+    double  residual_sq;
+    double  tol_sq;
+    double  initial_residual_sq;
+} PhiCgResult64;
+
+int phicuda_laplace_f64(const PhiGrid* g, const PhiBC* bc, const PhiValues64* values, const double* x, double* y, void* stream);
+int phicuda_laplace_axpy_f64(const PhiGrid* g, const PhiBC* bc, const PhiValues64* values, const double* x, double coeff, double* y,
+                             void* stream);
+int phicuda_divergence_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* values, const double* const v[3], double* div,
+                           void* stream);
+int phicuda_grad_sub_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* values, double* const v[3], const double* p,
+                         void* stream);
+/* vvalues: the velocity's exact values (vbc), fvalues: the advected field's (fbc) */
+int phicuda_advect_centered_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* vvalues, const double* const vel[3],
+                                const PhiBC* fbc, const PhiValues64* fvalues, const double* src, double* dst, double dt, void* stream);
+int phicuda_advect_staggered_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* vvalues, const double* const vel[3],
+                                 const PhiVBC* fbc, const PhiValues64* fvalues, const double* const src[3], double* const dst[3],
+                                 double dt, void* stream);
+size_t phicuda_cg_workspace_bytes_f64(const PhiGrid* g);
+/* result: device array of `batch` PhiCgResult64 */
+int phicuda_cg_poisson_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* values, const double* rhs, double* x,
+                           const PhiCgParams64* prm, PhiCgResult64* result, void* workspace, size_t workspace_bytes, void* stream);
+int phicuda_make_incompressible_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* values, double* const v[3], double* p,
+                                    double* div, const PhiCgParams64* prm, PhiCgResult64* result, void* workspace,
+                                    size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

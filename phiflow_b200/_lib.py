@@ -55,6 +55,20 @@ class PhiPlumeParams(C.Structure):
                 ('cg_start_event', C.c_void_p), ('cg_stop_event', C.c_void_p)]
 
 
+class PhiValues64(C.Structure):
+    _fields_ = [('dx', C.c_double * 3), ('clo', (C.c_double * 3) * 3), ('chi', (C.c_double * 3) * 3)]
+
+
+class PhiCgParams64(C.Structure):
+    _fields_ = [('rtol', C.c_double), ('atol', C.c_double), ('max_iter', C.c_int32), ('balance_rhs', C.c_int32),
+                ('project_mean', C.c_int32), ('matrix_offset', C.c_double), ('method', C.c_int32)]
+
+
+class PhiCgResult64(C.Structure):
+    _fields_ = [('iterations', C.c_int32), ('converged', C.c_int32), ('diverged', C.c_int32),
+                ('residual_sq', C.c_double), ('tol_sq', C.c_double), ('initial_residual_sq', C.c_double)]
+
+
 F3 = C.c_void_p * 3          # float* const v[3]
 _P = C.POINTER
 
@@ -118,6 +132,19 @@ PROTOTYPES = {
     'phicuda_wave_scratch_bytes': (C.c_size_t, [_P(PhiGrid), C.c_int32]),
     'phicuda_wave_f32': (C.c_int, [_P(PhiGrid), _P(PhiBC), C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, _P(PhiWaveDisc),
                                    C.c_float, _P(C.c_float), C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'phicuda_laplace_f64': (C.c_int, [_P(PhiGrid), _P(PhiBC), _P(PhiValues64), C.c_void_p, C.c_void_p, C.c_void_p]),
+    'phicuda_laplace_axpy_f64': (C.c_int, [_P(PhiGrid), _P(PhiBC), _P(PhiValues64), C.c_void_p, C.c_double, C.c_void_p, C.c_void_p]),
+    'phicuda_divergence_f64': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiValues64), F3, C.c_void_p, C.c_void_p]),
+    'phicuda_grad_sub_f64': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiValues64), F3, C.c_void_p, C.c_void_p]),
+    'phicuda_advect_centered_f64': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiValues64), F3, _P(PhiBC), _P(PhiValues64), C.c_void_p,
+                                              C.c_void_p, C.c_double, C.c_void_p]),
+    'phicuda_advect_staggered_f64': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiValues64), F3, _P(PhiVBC), _P(PhiValues64), F3, F3,
+                                               C.c_double, C.c_void_p]),
+    'phicuda_cg_workspace_bytes_f64': (C.c_size_t, [_P(PhiGrid)]),
+    'phicuda_cg_poisson_f64': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiValues64), C.c_void_p, C.c_void_p, _P(PhiCgParams64), C.c_void_p,
+                                         C.c_void_p, C.c_size_t, C.c_void_p]),
+    'phicuda_make_incompressible_f64': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiValues64), F3, C.c_void_p, C.c_void_p,
+                                                  _P(PhiCgParams64), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 

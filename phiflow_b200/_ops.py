@@ -12,11 +12,14 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import PhiGrid, PhiBC, PhiVBC, PhiCgParams, PhiCgResult, PhiPlumeParams, F3
+from ._lib import PhiGrid, PhiBC, PhiVBC, PhiCgParams, PhiCgParams64, PhiCgResult, PhiPlumeParams, PhiValues64, F3
 
 PERIODIC, ZG, HALO = 'periodic', 'zg', 'halo'
 _RESULT_DTYPE = np.dtype([('iterations', np.int32), ('converged', np.int32), ('diverged', np.int32),
                           ('residual_sq', np.float32), ('tol_sq', np.float32), ('initial_residual_sq', np.float32)])
+_RESULT_DTYPE64 = np.dtype({'names': ['iterations', 'converged', 'diverged', 'residual_sq', 'tol_sq', 'initial_residual_sq'],
+                            'formats': [np.int32, np.int32, np.int32, np.float64, np.float64, np.float64],
+                            'offsets': [0, 4, 8, 16, 24, 32], 'itemsize': 40})          # PhiCgResult64
 
 
 def _kind(side):
@@ -36,6 +39,23 @@ def make_bc(spec) -> PhiBC:
         bc.clo[a] = float(lo) if not isinstance(lo, str) else 0.0
         bc.chi[a] = float(hi) if not isinstance(hi, str) else 0.0
     return bc
+
+
+def _dtype_of(dom, *ts) -> torch.dtype:
+    """The one dtype of a call's arrays: float32 selects the _f32 entry point, float64 the _f64 one.  Arrays never mix, and they have
+    the domain's dtype: the domain's CG workspace and result records are sized and read for its dtype."""
+    dts = {t.dtype for t in ts if t is not None}
+    assert len(dts) == 1, f"the arrays of one call must share a dtype, got {sorted(str(d) for d in dts)}"
+    dt = dts.pop()
+    assert dt == dom.dtype, f"{dt} arrays on a {dom.dtype} domain (the domain's dtype decides its workspace and result records)"
+    return dt
+
+
+def _f32_only(what: str, dom, *ts):
+    """Entry points without an fp64 kernel refuse float64 arrays and float64 domains instead of reading them as float32."""
+    if dom.dtype == torch.float64 or any(t is not None and t.dtype == torch.float64 for t in ts):
+        raise _lib.Unsupported(_lib.ERR_UNSUPPORTED, f"{what}: float64 arrays are not supported (fp32 only; the fp64 path covers laplace, "
+                                                     f"divergence, grad_sub, semi-Lagrangian advection and the CG projection)")
 
 
 def make_vbc(spec, dim) -> PhiVBC:
@@ -78,7 +98,13 @@ def _stream():
 class Domain:
     """Resolution, cell size, batch size and the allocation extents of centred / staggered arrays (include/phicuda.h)."""
 
-    def __init__(self, resolution: Sequence[int], dx: Sequence[float], batch: int = 1, vbc=None, device='cuda', halo: int = 0):
+    def __init__(self, resolution: Sequence[int], dx: Sequence[float], batch: int = 1, vbc=None, device='cuda', halo: int = 0,
+                 dtype=torch.float32):
+        assert dtype in (torch.float32, torch.float64), f"dtype must be torch.float32 or torch.float64, got {dtype}"
+        assert dtype == torch.float32 or int(halo) == 0, "the fp64 path runs on one GPU (no z-slabs)"
+        self.dtype = dtype                    # of what alloc_* and *_from_numpy make; the array functions follow their arrays' dtype
+        self.np_dtype = np.float64 if dtype == torch.float64 else np.float32
+        esize = 8 if dtype == torch.float64 else 4
         self.dim = len(resolution)
         assert self.dim in (2, 3), "only 2-D and 3-D grids"
         self.res = tuple(int(r) for r in resolution)
@@ -92,8 +118,8 @@ class Domain:
         pad = lambda a: 2 * self.halo if a == 2 else 0
         self.cext = (r4(self.res[0]),) + tuple(self.res[a] + pad(a) for a in range(1, self.dim))
         self.fext = (r4(self.res[0] + int(self.upper[0])),) + tuple(self.res[a] + int(self.upper[a]) + pad(a) for a in range(1, self.dim))
-        self.coff = 4 * self.halo * self.cext[0] * self.cext[1]       # byte offset of the first owned plane
-        self.foff = 4 * self.halo * self.fext[0] * self.fext[1]
+        self.coff = esize * self.halo * self.cext[0] * self.cext[1]   # byte offset of the first owned plane
+        self.foff = esize * self.halo * self.fext[0] * self.fext[1]
         g = PhiGrid()
         g.dim, g.batch = self.dim, self.batch
         for a in range(3):
@@ -112,22 +138,36 @@ class Domain:
         return (self.batch,) + tuple(reversed(ext))
 
     def alloc_centered(self) -> torch.Tensor:
-        return torch.zeros(self._shape(self.cext), dtype=torch.float32, device=self.device)
+        return torch.zeros(self._shape(self.cext), dtype=self.dtype, device=self.device)
 
     def alloc_faces(self) -> List[torch.Tensor]:
-        return [torch.zeros(self._shape(self.fext), dtype=torch.float32, device=self.device) for _ in range(self.dim)]
+        return [torch.zeros(self._shape(self.fext), dtype=self.dtype, device=self.device) for _ in range(self.dim)]
 
     def workspace(self):
         if self._ws is None:
-            n = _lib.load().phicuda_cg_workspace_bytes(C.byref(self.grid))
+            lib = _lib.load()
+            n = (lib.phicuda_cg_workspace_bytes_f64 if self.dtype == torch.float64 else lib.phicuda_cg_workspace_bytes)(C.byref(self.grid))
             self._ws = torch.zeros(n, dtype=torch.uint8, device=self.device)
         return self._ws, self.results()
 
     def results(self):
-        """Device buffer of one PhiCgResult per batch entry (what read_results returns)."""
+        """Device buffer of one PhiCgResult (PhiCgResult64 on a float64 domain) per batch entry (what read_results returns)."""
         if self._result is None:
-            self._result = torch.zeros(self.batch * 6, dtype=torch.int32, device=self.device)
+            self._result = torch.zeros(self.batch * (10 if self.dtype == torch.float64 else 6), dtype=torch.int32, device=self.device)
         return self._result
+
+    def values64(self, spec, ncomp: int = 1) -> PhiValues64:
+        """The exact (float64) cell sizes and boundary constants of an _f64 call: `spec` is one boundary spec for `ncomp` components
+        or a list of per-component specs; self.grid.dx and make_bc / make_vbc carry the same values rounded to float."""
+        v = PhiValues64()
+        for a, d in enumerate(self.dx):
+            v.dx[a] = d
+        per_comp = spec if isinstance(spec, list) else [spec] * ncomp
+        for c in range(ncomp):
+            for a, (lo, hi) in enumerate(per_comp[c]):
+                v.clo[c][a] = float(lo) if not isinstance(lo, str) else 0.0
+                v.chi[c][a] = float(hi) if not isinstance(hi, str) else 0.0
+        return v
 
     def scratch(self):
         if self._scratch is None:
@@ -137,13 +177,13 @@ class Domain:
 
     # ---- conversions: reference layout (x, y[, z]) <-> device layout (b, [z,] y, x) ------------------------------------
     def _to_dev(self, a: np.ndarray, ext, offset_axis=None, offset=0) -> torch.Tensor:
-        a = np.asarray(a, dtype=np.float32)
+        a = np.asarray(a, dtype=self.np_dtype)
         if a.ndim == self.dim:
             a = a[None]
         assert a.ndim == self.dim + 1 and a.shape[0] in (1, self.batch), f"bad array shape {a.shape}"
         if a.shape[0] != self.batch:
             a = np.broadcast_to(a, (self.batch,) + a.shape[1:])
-        t = torch.zeros(self._shape(ext), dtype=torch.float32, device=self.device)
+        t = torch.zeros(self._shape(ext), dtype=self.dtype, device=self.device)
         src = torch.from_numpy(np.ascontiguousarray(np.transpose(a, (0,) + tuple(range(self.dim, 0, -1)))))
         idx = [slice(None)]
         for ax in range(self.dim - 1, -1, -1):               # device axis order: z, y, x
@@ -179,7 +219,7 @@ class Domain:
         shapes, offsets = self.face_shapes(vspec)
         out = []
         for c in range(self.dim):
-            a = np.asarray(comps[c], dtype=np.float32)
+            a = np.asarray(comps[c], dtype=self.np_dtype)
             assert tuple(a.shape[-self.dim:]) == shapes[c], f"component {c}: shape {a.shape} != stored faces {shapes[c]}"
             out.append(self._to_dev(a, self.fext, c, offsets[c]))
         return out
@@ -199,6 +239,9 @@ def laplace(dom: Domain, bc, x: torch.Tensor, out: torch.Tensor = None) -> torch
     """field.laplace order 2 (phi/field/_field_math.py:118-145)."""
     require_cuda()
     out = dom.alloc_centered() if out is None else out
+    if _dtype_of(dom, x, out) == torch.float64:
+        _lib.check(_lib.load().phicuda_laplace_f64(C.byref(dom.grid), C.byref(make_bc(bc)), C.byref(dom.values64(bc)), _ptr(x), _ptr(out), _stream()))
+        return out
     _lib.check(_lib.load().phicuda_laplace_f32(C.byref(dom.grid), C.byref(make_bc(bc)), _ptr(x, dom.coff), _ptr(out, dom.coff), _stream()))
     return out
 
@@ -207,6 +250,10 @@ def laplace_axpy(dom: Domain, bc, x, coeff: float, out=None):
     """x + coeff * laplace(x): one explicit diffusion sub-step (phi/physics/diffuse.py:13-60)."""
     require_cuda()
     out = dom.alloc_centered() if out is None else out
+    if _dtype_of(dom, x, out) == torch.float64:
+        _lib.check(_lib.load().phicuda_laplace_axpy_f64(C.byref(dom.grid), C.byref(make_bc(bc)), C.byref(dom.values64(bc)), _ptr(x), C.c_double(coeff),
+                                                        _ptr(out), _stream()))
+        return out
     _lib.check(_lib.load().phicuda_laplace_axpy_f32(C.byref(dom.grid), C.byref(make_bc(bc)), _ptr(x, dom.coff), C.c_float(coeff), _ptr(out, dom.coff), _stream()))
     return out
 
@@ -223,7 +270,7 @@ def laplace_axpy_faces(dom: Domain, vbc, v: List[torch.Tensor], coeff: float, su
     shapes, offsets = dom.face_shapes(vbc)
     out = []
     for c in range(dom.dim):
-        sub = Domain(shapes[c], dom.dx, dom.batch, device=dom.device)
+        sub = Domain(shapes[c], dom.dx, dom.batch, device=dom.device, dtype=dom.dtype)
         spec = vbc[c] if isinstance(vbc, list) else vbc
         src = (slice(None),) + tuple(slice(offsets[c] if a == c else 0, (offsets[c] if a == c else 0) + shapes[c][a]) for a in range(dom.dim - 1, -1, -1))
         dst = (slice(None),) + tuple(slice(0, shapes[c][a]) for a in range(dom.dim - 1, -1, -1))
@@ -242,6 +289,12 @@ def divergence(dom: Domain, vbc, v: List[torch.Tensor], out=None, accessible=Non
     """field.divergence of a staggered grid (phi/field/_field_math.py:617-626); accessible: div *= active mask (fluid.py:138-141)."""
     require_cuda()
     out = dom.alloc_centered() if out is None else out
+    if _dtype_of(dom, *v, out, accessible) == torch.float64:
+        if accessible is not None:
+            _f32_only("divergence with obstacles", dom, accessible)
+        _lib.check(_lib.load().phicuda_divergence_f64(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(dom.values64(vbc, dom.dim)),
+                                                      _f3(v), _ptr(out), _stream()))
+        return out
     if accessible is not None:
         _lib.check(_lib.load().phicuda_divergence_masked_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _f3(v, dom.foff),
                                                             _ptr(accessible, dom.coff), _ptr(out, dom.coff), _stream()))
@@ -253,6 +306,12 @@ def divergence(dom: Domain, vbc, v: List[torch.Tensor], out=None, accessible=Non
 def grad_sub(dom: Domain, vbc, v: List[torch.Tensor], p: torch.Tensor, accessible=None):
     """v -= spatial_gradient(p, at='face') in place (phi/physics/fluid.py:158-161); accessible: gradient *= hard_bcs (:159-160)."""
     require_cuda()
+    if _dtype_of(dom, *v, p, accessible) == torch.float64:
+        if accessible is not None:
+            _f32_only("grad_sub with obstacles", dom, accessible)
+        _lib.check(_lib.load().phicuda_grad_sub_f64(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(dom.values64(vbc, dom.dim)), _f3(v),
+                                                    _ptr(p), _stream()))
+        return v
     if accessible is not None:
         _lib.check(_lib.load().phicuda_grad_sub_masked_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _f3(v, dom.foff), _ptr(p, dom.coff),
                                                           _ptr(accessible, dom.coff), _stream()))
@@ -265,6 +324,11 @@ def advect_centered(dom: Domain, vbc, vel, fbc, src, dt: float, out=None):
     """advect.semi_lagrangian of a centred field (phi/physics/advect.py:156-179)."""
     require_cuda()
     out = dom.alloc_centered() if out is None else out
+    if _dtype_of(dom, *vel, src, out) == torch.float64:
+        _lib.check(_lib.load().phicuda_advect_centered_f64(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(dom.values64(vbc, dom.dim)),
+                                                           _f3(vel), C.byref(make_bc(fbc)), C.byref(dom.values64(fbc)), _ptr(src), _ptr(out),
+                                                           C.c_double(dt), _stream()))
+        return out
     _lib.check(_lib.load().phicuda_advect_centered_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _f3(vel, dom.foff),
                                                        C.byref(make_bc(fbc)), _ptr(src, dom.coff), _ptr(out, dom.coff), C.c_float(dt), _stream()))
     return out
@@ -274,6 +338,11 @@ def advect_staggered(dom: Domain, vbc, vel, fbc, src, dt: float, out=None):
     """advect.semi_lagrangian of a staggered field (self-advection when src is vel)."""
     require_cuda()
     out = dom.alloc_faces() if out is None else out
+    if _dtype_of(dom, *vel, *src, *out) == torch.float64:
+        _lib.check(_lib.load().phicuda_advect_staggered_f64(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(dom.values64(vbc, dom.dim)),
+                                                            _f3(vel), C.byref(make_vbc(fbc, dom.dim)), C.byref(dom.values64(fbc, dom.dim)),
+                                                            _f3(src), _f3(out), C.c_double(dt), _stream()))
+        return out
     _lib.check(_lib.load().phicuda_advect_staggered_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _f3(vel, dom.foff),
                                                         C.byref(make_vbc(fbc, dom.dim)), _f3(src, dom.foff), _f3(out, dom.foff), C.c_float(dt), _stream()))
     return out
@@ -283,6 +352,7 @@ def grid_sample(dom: Domain, bc, grid: torch.Tensor, coords: torch.Tensor, out: 
     """math.grid_sample (PhiML/phiml/math/_ops.py:936-1015): grid = centred array in device layout, coords = float32 tensor
     (batch, npoints, dim) of index-space positions (x first, 0 = first cell centre).  Returns (batch, npoints)."""
     require_cuda()
+    _f32_only("grid_sample", dom, grid)
     assert coords.dtype == torch.float32 and coords.is_contiguous() and coords.shape[0] == dom.batch and coords.shape[-1] == dom.dim
     npoints = coords.shape[1]
     out = torch.empty((dom.batch, npoints), dtype=torch.float32, device=dom.device) if out is None else out
@@ -294,6 +364,7 @@ def grid_sample(dom: Domain, bc, grid: torch.Tensor, coords: torch.Tensor, out: 
 def mac_cormack_centered(dom: Domain, vbc, vel, fbc, src, dt: float, correction_strength=1.0, out=None):
     """advect.mac_cormack of a centred field (phi/physics/advect.py:182-215)."""
     require_cuda()
+    _f32_only("mac_cormack", dom, *vel, src, out)
     out = dom.alloc_centered() if out is None else out
     tmp = dom.alloc_centered()
     _lib.check(_lib.load().phicuda_mac_cormack_centered_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _f3(vel, dom.foff),
@@ -304,6 +375,7 @@ def mac_cormack_centered(dom: Domain, vbc, vel, fbc, src, dt: float, correction_
 
 def axpy_centered(dom: Domain, a: float, x, y):
     require_cuda()
+    _f32_only("axpy_centered", dom, x, y)
     _lib.check(_lib.load().phicuda_axpy_centered_f32(C.byref(dom.grid), C.c_float(a), _ptr(x, dom.coff), _ptr(y, dom.coff), _stream()))
     return y
 
@@ -312,6 +384,7 @@ def add_buoyancy(dom: Domain, vbc, sbc, s, factor: Sequence[float], dt: float, v
     """v += dt * resample(s * factor, to=v) in place (phi/field/_resample.py:272-276).  The product keeps the boundary of s
     (phi/field/_field.py:809): faces next to a constant side c of s average c itself, unscaled, also where factor is 0."""
     require_cuda()
+    _f32_only("add_buoyancy (resample of a centred field to faces)", dom, s, *v)
     b = (C.c_float * 3)(*[float(factor[i]) if i < len(factor) else 0.0 for i in range(3)])
     _lib.check(_lib.load().phicuda_add_buoyancy_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(make_bc(sbc)),
                                                     _ptr(s, dom.coff), b, C.c_float(dt), _f3(v, dom.foff), _stream()))
@@ -322,6 +395,7 @@ def max_abs_velocity(dom: Domain, vbc, v, out: torch.Tensor = None) -> torch.Ten
     """Device tensor of 3 floats: max |v_c| per component over the stored faces of the owned planes (CFL number of the
     unbounded semi-Lagrangian back-trace, phi/physics/advect.py:20-24)."""
     require_cuda()
+    _f32_only("max_abs_velocity", dom, *v)
     out = torch.zeros(3, dtype=torch.float32, device=dom.device) if out is None else out
     _lib.check(_lib.load().phicuda_max_abs_velocity_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _f3(v, dom.foff), _ptr(out), _stream()))
     return out
@@ -350,11 +424,12 @@ def _is_flexible(vspec) -> bool:
     return any(side == ZG for ax in spec for side in ax)
 
 
-def cg_params(vbc, rtol=1e-5, atol=1e-5, max_iter=1000, matrix_offset=0.0, balance=None, method='CG') -> PhiCgParams:
+def cg_params(vbc, rtol=1e-5, atol=1e-5, max_iter=1000, matrix_offset=0.0, balance=None, method='CG', dtype=torch.float32):
     """Solver parameters with the defaults of fluid.make_incompressible (phi/physics/fluid.py:145-148):
-    non-flexible velocity boundaries (closed / periodic) -> balanced right-hand side and rank deficiency 1."""
+    non-flexible velocity boundaries (closed / periodic) -> balanced right-hand side and rank deficiency 1.
+    dtype float64: a PhiCgParams64 for the fp64 solve (tolerances and offset in double)."""
     rank_def = not _is_flexible(vbc)
-    prm = PhiCgParams()
+    prm = PhiCgParams64() if dtype == torch.float64 else PhiCgParams()
     prm.rtol, prm.atol, prm.max_iter = rtol, atol, int(max_iter)
     prm.balance_rhs = int(rank_def if balance is None else balance)
     prm.project_mean = int(rank_def)
@@ -367,7 +442,7 @@ def read_results(dom: Domain, components: int = 1) -> np.ndarray:
     """Synchronises and returns the per-batch solve results as a structured array.  components = C > 1: the records of the last
     diffuse_implicit of C components on `dom`, one per (batch entry, component), entry b * C + c."""
     d = dom if components == 1 else dom._stacked[components]
-    return d.results().cpu().numpy().view(_RESULT_DTYPE)
+    return d.results().cpu().numpy().view(_RESULT_DTYPE64 if d.dtype == torch.float64 else _RESULT_DTYPE)
 
 
 def cg_poisson(dom: Domain, vbc, rhs, x0=None, prm: PhiCgParams = None):
@@ -375,6 +450,12 @@ def cg_poisson(dom: Domain, vbc, rhs, x0=None, prm: PhiCgParams = None):
     require_cuda()
     ws, res = dom.workspace()
     x = dom.alloc_centered() if x0 is None else x0
+    if _dtype_of(dom, rhs, x) == torch.float64:
+        prm = prm or cg_params(vbc, rtol=1e-12, atol=1e-12, dtype=torch.float64)
+        assert isinstance(prm, PhiCgParams64), "float64 arrays take PhiCgParams64 (cg_params(..., dtype=torch.float64))"
+        _lib.check(_lib.load().phicuda_cg_poisson_f64(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(dom.values64(vbc, dom.dim)), _ptr(rhs),
+                                                      _ptr(x), C.byref(prm), _ptr(res), _ptr(ws), C.c_size_t(ws.numel()), _stream()))
+        return x
     prm = prm or cg_params(vbc)
     _lib.check(_lib.load().phicuda_cg_poisson_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _ptr(rhs, dom.coff), _ptr(x, dom.coff), C.byref(prm),
                                                   _ptr(res), _ptr(ws), C.c_size_t(ws.numel()), _stream()))
@@ -390,6 +471,7 @@ def diffuse_implicit(dom: Domain, spec, u, amount: float, rtol=1e-5, atol=1e-5, 
     read_results(dom, components=C) then holds one record per system, entry b * C + c = component c of batch entry b."""
     require_cuda()
     comps = list(u) if isinstance(u, (list, tuple)) else [u]
+    _f32_only("diffuse_implicit", dom, *comps)
     n = len(comps)
     assert 1 <= n <= 3 and all(c.shape == comps[0].shape for c in comps), "1 to 3 components of the same shape"
     assert dom.halo == 0, "implicit diffusion is not offered on z-slabs"
@@ -425,6 +507,7 @@ def diffuse_implicit_varying(dom: Domain, spec, u, k, dt: float, rtol=1e-5, atol
     u: centred array of `dom`; k: centred array with 1 (shared by every entry) or dom.batch entries.  x0: start value, default u.
     Returns a new array; the inputs are not modified.  read_results(dom) then holds one record per batch entry."""
     require_cuda()
+    _f32_only("diffuse_implicit_varying", dom, u, k)
     assert dom.halo == 0, "implicit diffusion is not offered on z-slabs"
     assert tuple(u.shape) == dom._shape(dom.cext), f"u: shape {tuple(u.shape)} is not a centred array of the domain"
     assert k.dtype == torch.float32 and k.is_contiguous() and tuple(k.shape[1:]) == tuple(u.shape[1:]) and k.shape[0] in (1, dom.batch), \
@@ -455,6 +538,7 @@ def reaction_diffusion(dom: Domain, spec, u, v, du: float, dv: float, f: float, 
     u, v: centred arrays of `dom`; spec: one boundary spec for both, or [spec_u, spec_v] (same kinds, constants 0).
     Returns new arrays (u', v'); the inputs are not modified and may be the same tensor."""
     require_cuda()
+    _f32_only("reaction_diffusion", dom, u, v)
     assert dom.halo == 0, "reaction-diffusion is not offered on z-slabs"
     shape = dom._shape(dom.cext)
     assert tuple(u.shape) == shape and tuple(v.shape) == shape, f"u, v: shapes {tuple(u.shape)}, {tuple(v.shape)} are not centred arrays of the domain"
@@ -472,6 +556,7 @@ def wave(dom: Domain, spec, h_c, h_p, dd: float, k_speed: float, k_damp: float, 
     discs: `substeps` entries (center, value), or None for a substep without a disc; radius_sq: float32 r^2; centers: per-axis cell
     centres (x, then y[, z]) as float32.  Returns new arrays (h_c', h_p'); the inputs are not modified and may be the same tensor."""
     require_cuda()
+    _f32_only("wave", dom, h_c, h_p)
     assert dom.halo == 0, "the wave step is not offered on z-slabs"
     shape = dom._shape(dom.cext)
     assert tuple(h_c.shape) == shape and tuple(h_p.shape) == shape, f"h_c, h_p: shapes {tuple(h_c.shape)}, {tuple(h_p.shape)} are not centred arrays of the domain"
@@ -497,6 +582,7 @@ def wave(dom: Domain, spec, h_c, h_p, dd: float, k_speed: float, k_damp: float, 
 def mul_faces(dom: Domain, vbc, v, mask):
     """v_c *= mask_c on the stored faces (apply_boundary_conditions for stationary obstacles, fluid.py:212-240)."""
     require_cuda()
+    _f32_only("mul_faces (obstacles)", dom, *v, *mask)
     _lib.check(_lib.load().phicuda_mul_faces_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _f3(v, dom.foff), _f3(mask, dom.foff), _stream()))
     return v
 
@@ -507,6 +593,15 @@ def make_incompressible(dom: Domain, vbc, v, p=None, prm: PhiCgParams = None, ac
     ws, res = dom.workspace()
     p = dom.alloc_centered() if p is None else p
     div = dom.alloc_centered()
+    if _dtype_of(dom, *v, p, div, accessible) == torch.float64:
+        if accessible is not None:
+            _f32_only("make_incompressible with obstacles", dom, accessible)
+        prm = prm or cg_params(vbc, rtol=1e-12, atol=1e-12, dtype=torch.float64)
+        assert isinstance(prm, PhiCgParams64), "float64 arrays take PhiCgParams64 (cg_params(..., dtype=torch.float64))"
+        _lib.check(_lib.load().phicuda_make_incompressible_f64(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), C.byref(dom.values64(vbc, dom.dim)),
+                                                               _f3(v), _ptr(p), _ptr(div), C.byref(prm), _ptr(res), _ptr(ws), C.c_size_t(ws.numel()),
+                                                               _stream()))
+        return v, p
     prm = prm or cg_params(vbc)
     if accessible is not None:
         _lib.check(_lib.load().phicuda_make_incompressible_masked_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _f3(v, dom.foff),
@@ -529,6 +624,7 @@ def wide_laplace(dom: Domain, vbc, x: torch.Tensor, out: torch.Tensor = None) ->
     """fluid.masked_laplace(wide_stencil=True) without obstacles (phi/physics/fluid.py:197-202): centred divergence of the centred
     gradient, the pressure operator of CenteredGrid velocities."""
     require_cuda()
+    _f32_only("wide_laplace (CenteredGrid velocities)", dom, x, out)
     out = dom.alloc_centered() if out is None else out
     ws = _collocated_workspace(dom)
     _lib.check(_lib.load().phicuda_wide_laplace_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _ptr(x), _ptr(out), _ptr(ws),
@@ -554,6 +650,7 @@ def make_incompressible_centered(dom: Domain, vbc, v: List[torch.Tensor], p: tor
     CENTRED arrays, updated in place; returns (v, p).  Solver: CG-adaptive, what the reference's default Solve() runs.
     Synchronises the stream (the iteration loop polls the stopping flags from the host)."""
     require_cuda()
+    _f32_only("make_incompressible of CenteredGrid velocities", dom, *v, p)
     res = dom.results()
     ws = _collocated_workspace(dom)
     p = dom.alloc_centered() if p is None else p
@@ -575,6 +672,7 @@ def plume_step(dom: Domain, vbc, sbc, v, s, p, inflow, dt, inflow_rate, buoyancy
     of apply_boundary_conditions (flow._obstacle_masks), both with the full batch (one obstacle per entry); v* is multiplied by the
     factors and projected with the masked operator (phicuda_plume_step_masked_f32)."""
     require_cuda()
+    _f32_only("plume_step (incompressible_step)", dom, *v, s, p)
     assert dom.halo == 0, "plume_step is the single-GPU fused call; z-slab runs sequence the step in phiflow_b200.dist"
     assert (accessible is None) == (factors is None), "obstacles need both the accessible mask and the face factors"
     ws, res = dom.workspace()

@@ -139,7 +139,8 @@ int phi_pressure_bc(const PhiVBC* vbc, int dim, PhiBC* o)
     return 0;
 }
 
-UnitMap phi_make_unit_map(const DGrid& g, int target_units)
+template <class T>
+UnitMap phi_make_unit_map(const DGridT<T>& g, int target_units)
 {
     UnitMap um;
     um.nxt = (g.n[0] + PHI_TILE_X - 1) / PHI_TILE_X;
@@ -163,6 +164,9 @@ UnitMap phi_make_unit_map(const DGrid& g, int target_units)
     }
     return um;
 }
+
+template UnitMap phi_make_unit_map<float>(const DGrid& g, int target_units);
+template UnitMap phi_make_unit_map<double>(const DGridT<double>& g, int target_units);
 
 static int make_vec(const PhiGrid* g, const PhiVBC* vbc, const float* const v[3], DVec* o)
 {
@@ -822,6 +826,216 @@ int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, 
                                   reinterpret_cast<const float*>(dtab + (size_t)substeps * sizeof(WaveDisc)), wp, substeps, (cudaStream_t)stream);
     if (e == -100) { phi_set_error("wave: the grid does not fit the TMA ring on this device"); return PHI_ERR_UNSUPPORTED; }
     return cuda_fail(e, "wave");
+}
+
+}  // extern "C"
+
+// ---- N9: fp64 ------------------------------------------------------------------------------------------------------------
+// The float fields of PhiGrid / PhiBC describe the layout and kinds and must equal the exact values rounded to float; the kernels
+// take the exact values from PhiValues64.  Every check runs before the first CUDA call.
+static const double kZero3[3] = {0.0, 0.0, 0.0};
+
+static int check_values64(const PhiGrid* g, const PhiBC* bcs, int ncomp, const PhiValues64* val, const char* what)
+{
+    if (!val) { phi_set_error("%s: values (PhiValues64) is NULL", what); return PHI_ERR_INVALID; }
+    if (g->halo != 0) { phi_set_error("%s: z-slab grids (halo %d) are not supported; the fp64 path runs on one GPU", what, g->halo); return PHI_ERR_UNSUPPORTED; }
+    for (int a = 0; a < g->dim; ++a)
+        if (!((float)val->dx[a] == g->dx[a])) {
+            phi_set_error("%s: values.dx[%d] = %.17g does not round to grid.dx[%d] = %.9g", what, a, val->dx[a], a, (double)g->dx[a]);
+            return PHI_ERR_INVALID;
+        }
+    for (int c = 0; c < ncomp; ++c)
+        for (int a = 0; a < g->dim; ++a)
+            if (!((float)val->clo[c][a] == bcs[c].clo[a]) || !((float)val->chi[c][a] == bcs[c].chi[a])) {
+                phi_set_error("%s: values.clo/chi[%d][%d] = %.17g / %.17g do not round to the boundary's %.9g / %.9g", what, c, a,
+                              val->clo[c][a], val->chi[c][a], (double)bcs[c].clo[a], (double)bcs[c].chi[a]);
+                return PHI_ERR_INVALID;
+            }
+    return 0;
+}
+
+// after check_values64: the grid with the exact cell sizes, 1 / dx = RN(1 / dx) in double
+static DGridT<double> dgrid64(const DGrid& f, const PhiValues64* val)
+{
+    DGridT<double> o;
+    o.dim = f.dim; o.batch = f.batch; o.halo = f.halo;
+    for (int a = 0; a < 3; ++a) {
+        const bool used = a < f.dim;
+        o.n[a] = f.n[a]; o.cext[a] = f.cext[a]; o.fext[a] = f.fext[a];
+        o.dx[a] = used ? val->dx[a] : 1.0;
+        o.inv_dx[a] = used ? 1.0 / val->dx[a] : 0.0;
+        o.inv_dx2[a] = used ? 1.0 / (val->dx[a] * val->dx[a]) : 0.0;
+    }
+    return o;
+}
+
+static DFieldT<double> field64(const DField& f, const double clo[3], const double chi[3], int dim)
+{
+    DFieldT<double> o;
+    for (int a = 0; a < 3; ++a) {
+        o.lo[a] = f.lo[a]; o.hi[a] = f.hi[a]; o.klo[a] = f.klo[a]; o.khi[a] = f.khi[a];
+        o.clo[a] = a < dim ? clo[a] : 0.0; o.chi[a] = a < dim ? chi[a] : 0.0;
+    }
+    o.sy = f.sy; o.sz = f.sz; o.sb = f.sb; o.halo = f.halo;
+    return o;
+}
+
+static int make_vec64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* val, const double* const v[3], DVecT<double>* o)
+{
+    DVec f;
+    if (!v) { phi_set_error("vector field / boundary is NULL"); return PHI_ERR_INVALID; }
+    const float* vp[3] = {(const float*)v[0], (const float*)v[1], (const float*)v[2]};     // make_vec checks and keeps the addresses
+    CHECK(make_vec(g, vbc, vp, &f));
+    for (int c = 0; c < 3; ++c) {
+        o->p[c] = c < g->dim ? v[c] : nullptr;
+        o->f[c] = c < g->dim ? field64(f.f[c], val->clo[c], val->chi[c], g->dim) : field64(f.f[c], kZero3, kZero3, 0);
+    }
+    return 0;
+}
+
+// Every check of an fp64 pressure solve: fills l without a CUDA call.
+static int cg_setup64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* val, const double* rhs, double* x, const PhiCgParams64* prm,
+                      PhiCgResult64* result, void* workspace, size_t workspace_bytes, CgLaunch64* l)
+{
+    DGrid dg; PhiBC pbc; DField pf;
+    CHECK(phi_make_dgrid(g, &dg));
+    if (!vbc || !rhs || !x || !prm || !result || !workspace) { phi_set_error("cg_f64: NULL argument"); return PHI_ERR_INVALID; }
+    for (int a = 0; a < g->dim; ++a) CHECK(check_bc(&vbc->comp[a], g->dim));
+    CHECK(check_values64(g, vbc->comp, g->dim, val, "cg_f64"));
+    if (prm->method == PHI_SOLVER_CG_ADAPTIVE) { phi_set_error("cg_f64: CG-adaptive runs on the fp32 TMA ring kernel only; fp64 solves take PHI_SOLVER_CG"); return PHI_ERR_UNSUPPORTED; }
+    if (prm->method != PHI_SOLVER_CG) { phi_set_error("cg_f64: unknown solver method %d", prm->method); return PHI_ERR_INVALID; }
+    if (g->batch > CG_MAX_BATCH) { phi_set_error("cg_f64: batch %d exceeds %d (split the batch)", g->batch, CG_MAX_BATCH); return PHI_ERR_UNSUPPORTED; }
+    CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &pf));
+    l->g = dgrid64(dg, val);
+    l->pf = field64(pf, kZero3, kZero3, g->dim);              // the pressure boundary has no constants
+    const size_t need = phi_cg_workspace_bytes_f64(l->g);
+    if (workspace_bytes < need) { phi_set_error("cg_f64: workspace %zu < %zu bytes", workspace_bytes, need); return PHI_ERR_WORKSPACE; }
+    l->rhs = rhs; l->x = x; l->prm = *prm; l->result = result; l->workspace = workspace; l->workspace_bytes = workspace_bytes;
+    return 0;
+}
+
+extern "C" {
+
+static int laplace64(const PhiGrid* g, const PhiBC* bc, const PhiValues64* val, const double* x, double coeff, double* y, bool axpy,
+                     void* stream, const char* what)
+{
+    DGrid dg; DField f;
+    CHECK(phi_make_dgrid(g, &dg)); CHECK(phi_make_centered(g, bc, &f));
+    CHECK(check_values64(g, bc, 1, val, what));
+    if (!x || !y || x == y) { phi_set_error("%s: x and y must be distinct non-NULL arrays", what); return PHI_ERR_INVALID; }
+    return cuda_fail(phi_launch_laplace(dgrid64(dg, val), field64(f, val->clo[0], val->chi[0], g->dim), x, y, coeff, axpy,
+                                        (cudaStream_t)stream), what);
+}
+
+int phicuda_laplace_f64(const PhiGrid* g, const PhiBC* bc, const PhiValues64* values, const double* x, double* y, void* stream)
+{
+    return laplace64(g, bc, values, x, 0.0, y, false, stream, "laplace_f64");
+}
+
+int phicuda_laplace_axpy_f64(const PhiGrid* g, const PhiBC* bc, const PhiValues64* values, const double* x, double coeff, double* y,
+                             void* stream)
+{
+    return laplace64(g, bc, values, x, coeff, y, true, stream, "laplace_axpy_f64");
+}
+
+int phicuda_divergence_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* values, const double* const v[3], double* div,
+                           void* stream)
+{
+    DGrid dg; DVecT<double> dv; DField cf; PhiBC none; memset(&none, 0, sizeof(none));
+    CHECK(phi_make_dgrid(g, &dg));
+    if (!vbc) { phi_set_error("divergence_f64: boundary is NULL"); return PHI_ERR_INVALID; }
+    CHECK(check_values64(g, vbc->comp, g->dim, values, "divergence_f64"));
+    CHECK(make_vec64(g, vbc, values, v, &dv)); CHECK(phi_make_centered(g, &none, &cf));
+    if (!div) { phi_set_error("divergence_f64: div is NULL"); return PHI_ERR_INVALID; }
+    return cuda_fail(phi_launch_divergence(dgrid64(dg, values), dv, field64(cf, kZero3, kZero3, g->dim), div, (cudaStream_t)stream),
+                     "divergence_f64");
+}
+
+int phicuda_grad_sub_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* values, double* const v[3], const double* p,
+                         void* stream)
+{
+    DGrid dg; DVecT<double> dv; DVecOutT<double> out; PhiBC pbc; DField pf;
+    CHECK(phi_make_dgrid(g, &dg));
+    if (!vbc) { phi_set_error("grad_sub_f64: boundary is NULL"); return PHI_ERR_INVALID; }
+    CHECK(check_values64(g, vbc->comp, g->dim, values, "grad_sub_f64"));
+    CHECK(make_vec64(g, vbc, values, v, &dv));
+    CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &pf));
+    if (!p) { phi_set_error("grad_sub_f64: p is NULL"); return PHI_ERR_INVALID; }
+    for (int c = 0; c < 3; ++c) out.p[c] = c < g->dim ? v[c] : nullptr;
+    return cuda_fail(phi_launch_grad_sub(dgrid64(dg, values), dv, out, field64(pf, kZero3, kZero3, g->dim), p, (cudaStream_t)stream),
+                     "grad_sub_f64");
+}
+
+int phicuda_advect_centered_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* vvalues, const double* const vel[3],
+                                const PhiBC* fbc, const PhiValues64* fvalues, const double* src, double* dst, double dt, void* stream)
+{
+    DGrid dg; DVecT<double> dv; DField ff;
+    CHECK(phi_make_dgrid(g, &dg));
+    if (!vbc) { phi_set_error("advect_centered_f64: boundary is NULL"); return PHI_ERR_INVALID; }
+    CHECK(check_values64(g, vbc->comp, g->dim, vvalues, "advect_centered_f64"));
+    CHECK(make_vec64(g, vbc, vvalues, vel, &dv)); CHECK(phi_make_centered(g, fbc, &ff));
+    CHECK(check_values64(g, fbc, 1, fvalues, "advect_centered_f64"));
+    if (!src || !dst || src == dst) { phi_set_error("advect_centered_f64: src and dst must be distinct non-NULL arrays"); return PHI_ERR_INVALID; }
+    return cuda_fail(phi_launch_advect(dgrid64(dg, vvalues), dv, field64(ff, fvalues->clo[0], fvalues->chi[0], g->dim), -1, src, dst, dt,
+                                       (cudaStream_t)stream), "advect_centered_f64");
+}
+
+int phicuda_advect_staggered_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* vvalues, const double* const vel[3],
+                                 const PhiVBC* fbc, const PhiValues64* fvalues, const double* const src[3], double* const dst[3],
+                                 double dt, void* stream)
+{
+    DGrid dg; DVecT<double> dv, df;
+    CHECK(phi_make_dgrid(g, &dg));
+    if (!vbc || !fbc || !dst) { phi_set_error("advect_staggered_f64: NULL argument"); return PHI_ERR_INVALID; }
+    CHECK(check_values64(g, vbc->comp, g->dim, vvalues, "advect_staggered_f64"));
+    CHECK(check_values64(g, fbc->comp, g->dim, fvalues, "advect_staggered_f64"));
+    CHECK(make_vec64(g, vbc, vvalues, vel, &dv)); CHECK(make_vec64(g, fbc, fvalues, src, &df));
+    for (int c = 0; c < g->dim; ++c) {
+        if (!dst[c]) { phi_set_error("advect_staggered_f64: dst[%d] is NULL", c); return PHI_ERR_INVALID; }
+        for (int k = 0; k < g->dim; ++k) if (dst[c] == src[k] || dst[c] == vel[k]) { phi_set_error("advect_staggered_f64: dst must not alias src or vel"); return PHI_ERR_INVALID; }
+    }
+    const DGridT<double> dg64 = dgrid64(dg, vvalues);
+    for (int c = 0; c < g->dim; ++c)
+        CHECK(cuda_fail(phi_launch_advect(dg64, dv, df.f[c], c, src[c], dst[c], dt, (cudaStream_t)stream), "advect_staggered_f64"));
+    return 0;
+}
+
+size_t phicuda_cg_workspace_bytes_f64(const PhiGrid* g)
+{
+    DGrid dg;
+    if (phi_make_dgrid(g, &dg)) return 0;
+    const PhiValues64 unit = {{1.0, 1.0, 1.0}, {}, {}};          // the size depends on the extents and the batch only
+    return phi_cg_workspace_bytes_f64(dgrid64(dg, &unit));
+}
+
+int phicuda_cg_poisson_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* values, const double* rhs, double* x,
+                           const PhiCgParams64* prm, PhiCgResult64* result, void* workspace, size_t workspace_bytes, void* stream)
+{
+    CgLaunch64 l;
+    CHECK(cg_setup64(g, vbc, values, rhs, x, prm, result, workspace, workspace_bytes, &l));
+    return cuda_fail(phi_launch_cg(l, (cudaStream_t)stream), "cg_f64");
+}
+
+int phicuda_make_incompressible_f64(const PhiGrid* g, const PhiVBC* vbc, const PhiValues64* values, double* const v[3], double* p,
+                                    double* div, const PhiCgParams64* prm, PhiCgResult64* result, void* workspace,
+                                    size_t workspace_bytes, void* stream)
+{
+    // every check of the projection and its solve runs before the first CUDA call
+    CgLaunch64 l; DGrid dg; DVecT<double> dv; DVecOutT<double> out; DField cf, pf; PhiBC none, pbc; memset(&none, 0, sizeof(none));
+    CHECK(cg_setup64(g, vbc, values, div, p, prm, result, workspace, workspace_bytes, &l));
+    CHECK(phi_make_dgrid(g, &dg));
+    CHECK(make_vec64(g, vbc, values, v, &dv)); CHECK(phi_make_centered(g, &none, &cf));
+    CHECK(phi_pressure_bc(vbc, g->dim, &pbc)); CHECK(phi_make_centered(g, &pbc, &pf));
+    if (div == p) { phi_set_error("make_incompressible_f64: div and p must be distinct arrays"); return PHI_ERR_INVALID; }
+    for (int c = 0; c < g->dim; ++c) {                // divergence reads v while it writes div, grad_sub writes v while it reads p
+        if (v[c] == div || v[c] == p) { phi_set_error("make_incompressible_f64: div and p must not alias v[%d]", c); return PHI_ERR_INVALID; }
+        for (int k = 0; k < c; ++k) if (v[k] == v[c]) { phi_set_error("make_incompressible_f64: v[%d] and v[%d] are the same array", k, c); return PHI_ERR_INVALID; }
+    }
+    for (int c = 0; c < 3; ++c) out.p[c] = c < g->dim ? v[c] : nullptr;
+    cudaStream_t st = (cudaStream_t)stream;
+    CHECK(cuda_fail(phi_launch_divergence(l.g, dv, field64(cf, kZero3, kZero3, g->dim), div, st), "make_incompressible_f64 divergence"));
+    CHECK(cuda_fail(phi_launch_cg(l, st), "make_incompressible_f64 cg"));
+    return cuda_fail(phi_launch_grad_sub(l.g, dv, out, l.pf, p, st), "make_incompressible_f64 grad_sub");
 }
 
 }  // extern "C"

@@ -18,6 +18,14 @@ int phi_launch_advect(const DGrid& g, const DVec& vel, const DField& ff, int tar
 int phi_launch_mac_cormack(const DGrid& g, const DVec& vel, const DField& ff, const float* src, float* dst, float* tmp,
                            float dt, float strength, cudaStream_t s);
 
+// fp64 (N9): the one-thread-per-sample stencils and advection and the register-marching laplace, no obstacle masks
+int phi_launch_laplace(const DGridT<double>& g, const DFieldT<double>& f, const double* x, double* y, double coeff, bool axpy, cudaStream_t s);
+int phi_launch_divergence(const DGridT<double>& g, const DVecT<double>& v, const DFieldT<double>& cf, double* div, cudaStream_t s);
+int phi_launch_grad_sub(const DGridT<double>& g, const DVecT<double>& vin, const DVecOutT<double>& v, const DFieldT<double>& pf,
+                        const double* p, cudaStream_t s);
+int phi_launch_advect(const DGridT<double>& g, const DVecT<double>& vel, const DFieldT<double>& ff, int target_comp, const double* src,
+                      double* dst, double dt, cudaStream_t s);
+
 // vectorised / fused variants (fused_kernels.cu); acc / af / faces: static obstacle masks (N4), nullptr = none
 int phi_launch_divergence_vec(const DGrid& g, const DVec& v, const DField& cf, float* div, const float* acc, cudaStream_t s);
 int phi_launch_grad_sub_vec(const DGrid& g, const DVec& vin, const DVecOut& vout, const DField& pf, const float* p,
@@ -86,6 +94,16 @@ struct CommDev {                      // device view of the multi-GPU communicat
 int phi_launch_cg_ring(const CgLaunch& a, const CommDev* cm, cudaStream_t s);
 bool phi_ring_enabled();
 int phi_launch_cg(const CgLaunch& a, cudaStream_t s);
+// fp64 pressure solve (N9): the register-marching persistent CG on the Poisson operator, workspace r | d0 | d1 | partials.  The caller
+// has checked the solve (batch <= CG_MAX_BATCH, no z-slabs, PHI_SOLVER_CG, workspace_bytes >= phi_cg_workspace_bytes_f64).
+struct CgLaunch64 {
+    DGridT<double> g; DFieldT<double> pf;
+    const double* rhs; double* x;
+    PhiCgParams64 prm; PhiCgResult64* result;
+    void* workspace; size_t workspace_bytes;
+};
+size_t phi_cg_workspace_bytes_f64(const DGridT<double>& g);
+int phi_launch_cg(const CgLaunch64& a, cudaStream_t s);
 // diffuse.implicit on the ring CG (ring_kernels.cu): host-only fit test, and the solve (bias pre-pass + k_cg_ring with the
 // Helmholtz operator l.op); cf[0 .. C-1] = boundary with constants of component c (batch entry b is component b % C; C = 1 for a varying
 // diffusivity).  -100: the grid does not fit the ring.

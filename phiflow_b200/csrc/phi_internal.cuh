@@ -10,38 +10,56 @@
 // ---------------------------------------------------------------------------------------------------------
 // Device views of the C-ABI structs
 // ---------------------------------------------------------------------------------------------------------
-struct DGrid {
+// T = float on every fp32 path; T = double on the fp64 path (the one-thread-per-sample stencils, advection and the
+// register-marching CG).  The float aliases below are what every other kernel uses.
+template <class T>
+struct DGridT {
     int dim, batch;
     int n[3];
     int cext[3], fext[3];          // allocated extents of centred arrays / staggered components
     int halo;                      // z-slab halo planes on each side of the owned range (0 on one GPU)
-    float dx[3], inv_dx[3], inv_dx2[3];
+    T dx[3], inv_dx[3], inv_dx2[3];
 };
+using DGrid = DGridT<float>;
 
 // One scalar array: valid index range per axis + what lies outside it.
 //   centred array:           [0, n-1] on every axis
 //   staggered component c:   along c the stored faces [1-lo_stored, n-1+hi_stored]  (SURVEY.md Appendix A/B)
-struct DField {
+template <class T>
+struct DFieldT {
     int lo[3], hi[3];
     unsigned char klo[3], khi[3];
-    float clo[3], chi[3];
+    T clo[3], chi[3];
     long long sy, sz, sb;          // strides (elements) of y, z, batch of this array
     int halo;                      // planes readable beyond [lo, hi] on the last axis (PHI_BC_HALO)
 };
+using DField = DFieldT<float>;
 
-struct DVec {                      // a staggered vector field
-    DField f[3];
-    const float* p[3];
+template <class T>
+struct DVecT {                     // a staggered vector field
+    DFieldT<T> f[3];
+    const T* p[3];
 };
-struct DVecOut {
-    float* p[3];
+template <class T>
+struct DVecOutT {
+    T* p[3];
 };
+using DVec = DVecT<float>;
+using DVecOut = DVecOutT<float>;
+
+// four consecutive cells of a row: one 16-byte load in fp32, two in fp64 (rows stay 4-element padded, so a double row is
+// 32-byte aligned)
+template <class T> struct Vec4Of;
+template <> struct Vec4Of<float> { using type = float4; };
+template <> struct Vec4Of<double> { using type = double4; };
+template <class T> using Vec4 = typename Vec4Of<T>::type;
 
 // ---------------------------------------------------------------------------------------------------------
 // Boundary resolution: maps an arbitrary index onto the stored range or yields the constant outside value.
 // PERIODIC: index % n (extrapolation.py:668-669); ZERO_GRADIENT: clamp (:160-176); constant c: c (ring of c, _ops.py:912-918)
 // ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool phi_resolve(int& i, const DField& f, int a, float& cval)
+template <class T>
+__device__ __forceinline__ bool phi_resolve(int& i, const DFieldT<T>& f, int a, T& cval)
 {
     const int lo = f.lo[a], hi = f.hi[a];
     if (i < lo) {
@@ -61,12 +79,12 @@ __device__ __forceinline__ bool phi_resolve(int& i, const DField& f, int a, floa
     return true;
 }
 
-template <int DIM>
-__device__ __forceinline__ float phi_fetch(const float* __restrict__ a, const DGrid& g, const DField& f, int b, int x, int y, int z)
+template <int DIM, class T>
+__device__ __forceinline__ T phi_fetch(const T* __restrict__ a, const DGridT<T>& g, const DFieldT<T>& f, int b, int x, int y, int z)
 {
     // Outside in more than one axis: the reference pads axis by axis (math.pad, _ops.py:791-838), so a corner ghost cell holds what
     // the axis padded LAST put there - resolve the last axis first.  (Only visible when two axes carry different constants.)
-    float c = 0.f;
+    T c = 0;
     if (DIM == 3) { if (!phi_resolve(z, f, 2, c)) return c; } else z = 0;
     if (!phi_resolve(y, f, 1, c)) return c;
     if (!phi_resolve(x, f, 0, c)) return c;
@@ -90,17 +108,34 @@ __device__ __forceinline__ float phi_fetch_scaled(const float* __restrict__ a, c
 // correction q = RN(a * inv_b); r = a - q * b (exact in the FMA); q' = RN(q + r * inv_b) gives the correctly rounded quotient -
 // the value the reference's `/ dx` produces (spatial_gradient, PhiML/phiml/math/_nd.py:813-815) - in 3 instructions instead of
 // the ~35 of the IEEE division subroutine (ncu: the divisions were 75 % of the instructions of the stencil kernels).
-// Exceptions (no overflow / denormal handling, significand of b all ones) do not occur for cell sizes.
-__device__ __forceinline__ float phi_div(float a, float b, float inv_b)
+// Exceptions (no overflow / denormal handling, significand of b all ones) do not occur for cell sizes.  The same correction
+// gives the correctly rounded quotient in binary64 with FMA; the host then computes inv_dx = RN(1 / dx) in double.
+__device__ __forceinline__ float phi_fma(float a, float b, float c) { return fmaf(a, b, c); }
+__device__ __forceinline__ double phi_fma(double a, double b, double c) { return fma(a, b, c); }
+template <class T>
+__device__ __forceinline__ T phi_div(T a, T b, T inv_b)
 {
-    const float q = a * inv_b;
-    const float r = fmaf(-q, b, a);
-    return fmaf(r, inv_b, q);
+    const T q = a * inv_b;
+    const T r = phi_fma(-q, b, a);
+    return phi_fma(r, inv_b, q);
 }
+__device__ __forceinline__ float phi_abs(float a) { return fabsf(a); }
+__device__ __forceinline__ double phi_abs(double a) { return fabs(a); }
+__device__ __forceinline__ float phi_min(float a, float b) { return fminf(a, b); }
+__device__ __forceinline__ double phi_min(double a, double b) { return fmin(a, b); }
+__device__ __forceinline__ float phi_max(float a, float b) { return fmaxf(a, b); }
+__device__ __forceinline__ double phi_max(double a, double b) { return fmax(a, b); }
+__device__ __forceinline__ float phi_floor(float a) { return floorf(a); }
+__device__ __forceinline__ double phi_floor(double a) { return floor(a); }
 
 __device__ __forceinline__ float4 f4_splat(float c) { return make_float4(c, c, c, c); }
 __device__ __forceinline__ float f4_get(const float4& v, int j) { return j == 0 ? v.x : (j == 1 ? v.y : (j == 2 ? v.z : v.w)); }
 __device__ __forceinline__ void f4_set(float4& v, int j, float s) { if (j == 0) v.x = s; else if (j == 1) v.y = s; else if (j == 2) v.z = s; else v.w = s; }
+__device__ __forceinline__ double4 f4_splat(double c) { return make_double4(c, c, c, c); }
+__device__ __forceinline__ double f4_get(const double4& v, int j) { return j == 0 ? v.x : (j == 1 ? v.y : (j == 2 ? v.z : v.w)); }
+__device__ __forceinline__ void f4_set(double4& v, int j, double s) { if (j == 0) v.x = s; else if (j == 1) v.y = s; else if (j == 2) v.z = s; else v.w = s; }
+__device__ __forceinline__ float4 f4_make(float a, float b, float c, float d) { return make_float4(a, b, c, d); }
+__device__ __forceinline__ double4 f4_make(double a, double b, double c, double d) { return make_double4(a, b, c, d); }
 
 // ---------------------------------------------------------------------------------------------------------
 // Reductions
@@ -123,16 +158,16 @@ __device__ __forceinline__ double warp_sum(double v)
 //
 //   q = sum_axis (left + right - 2*centre) * inv_dx2[axis]          (PhiML/phiml/math/_nd.py:855-856)
 // ---------------------------------------------------------------------------------------------------------
-template <int DIM>
+template <int DIM, class T = float>
 struct RowRef {            // a resolved grid line: either memory (off >= 0) or a constant
     long long off;         // element offset of x = 0 of the line, -1 if constant
-    float cval;
+    T cval;
 };
 
-template <int DIM>
-__device__ __forceinline__ RowRef<DIM> phi_row(const DGrid& g, const DField& f, int b, int y, int z)
+template <int DIM, class T>
+__device__ __forceinline__ RowRef<DIM, T> phi_row(const DGridT<T>& g, const DFieldT<T>& f, int b, int y, int z)
 {
-    RowRef<DIM> r; r.cval = 0.f; r.off = -1;
+    RowRef<DIM, T> r; r.cval = 0; r.off = -1;
     if (DIM == 3) { if (!phi_resolve(z, f, 2, r.cval)) return r; } else z = 0;
     if (!phi_resolve(y, f, 1, r.cval)) return r;
     r.off = (long long)b * f.sb + (long long)z * f.sz + (long long)y * f.sy;
@@ -140,8 +175,8 @@ __device__ __forceinline__ RowRef<DIM> phi_row(const DGrid& g, const DField& f, 
 }
 
 // value of the ghost cells at x = -1 / x = n for a resolved line
-template <int DIM, class Src>
-__device__ __forceinline__ float phi_ghost_x(const Src& src, const DField& f, const RowRef<DIM>& row, bool upper)
+template <int DIM, class Src, class T>
+__device__ __forceinline__ T phi_ghost_x(const Src& src, const DFieldT<T>& f, const RowRef<DIM, T>& row, bool upper)
 {
     if (row.off < 0) return row.cval;
     const int k = upper ? f.khi[0] : f.klo[0];
@@ -150,65 +185,67 @@ __device__ __forceinline__ float phi_ghost_x(const Src& src, const DField& f, co
     return upper ? f.chi[0] : f.clo[0];
 }
 
-template <int DIM, class Src>
-__device__ __forceinline__ float4 phi_load_row4(const Src& src, const RowRef<DIM>& row, int x0, bool active)
+template <int DIM, class Src, class T>
+__device__ __forceinline__ Vec4<T> phi_load_row4(const Src& src, const RowRef<DIM, T>& row, int x0, bool active)
 {
-    if (!active) return f4_splat(0.f);
+    if (!active) return f4_splat(T(0));
     if (row.off < 0) return f4_splat(row.cval);
     return src.load4(row.off + x0);
 }
 
-template <int DIM, class Src, class Epi>
-__device__ __forceinline__ void phi_march(const DGrid& g, const DField& f, const Src& src, Epi& epi,
+template <int DIM, class Src, class Epi, class T>
+__device__ __forceinline__ void phi_march(const DGridT<T>& g, const DFieldT<T>& f, const Src& src, Epi& epi,
                                           int b, int xt0, int t, int m0, int m1)
 {
+    using V = Vec4<T>;
     const int lane = threadIdx.x & 31;
     const int x0 = xt0 + lane * 4;
     const int nx = g.n[0];
     const bool active = x0 < nx;
     const int nvalid = active ? min(4, nx - x0) : 0;
-    const float ix2 = g.inv_dx2[0], iy2 = g.inv_dx2[1], iz2 = g.inv_dx2[2];
+    const T ix2 = g.inv_dx2[0], iy2 = g.inv_dx2[1], iz2 = g.inv_dx2[2];
+    const T two = 2;
 
     auto rowAt = [&](int tt, int mm) { return DIM == 3 ? phi_row<DIM>(g, f, b, tt, mm) : phi_row<DIM>(g, f, b, mm, 0); };
 
-    float4 vm = phi_load_row4<DIM>(src, rowAt(t, m0 - 1), x0, active);
-    RowRef<DIM> rc = rowAt(t, m0);
-    float4 vc = phi_load_row4<DIM>(src, rc, x0, active);
+    V vm = phi_load_row4<DIM>(src, rowAt(t, m0 - 1), x0, active);
+    RowRef<DIM, T> rc = rowAt(t, m0);
+    V vc = phi_load_row4<DIM>(src, rc, x0, active);
     for (int m = m0; m < m1; ++m) {
-        const float4 vp = phi_load_row4<DIM>(src, rowAt(t, m + 1), x0, active);
-        float4 tl, th;
+        const V vp = phi_load_row4<DIM>(src, rowAt(t, m + 1), x0, active);
+        V tl, th;
         if (DIM == 3) {
             tl = phi_load_row4<DIM>(src, rowAt(t - 1, m), x0, active);
             th = phi_load_row4<DIM>(src, rowAt(t + 1, m), x0, active);
         }
         // x neighbours
-        float left = __shfl_up_sync(0xffffffffu, vc.w, 1);
-        float right = __shfl_down_sync(0xffffffffu, vc.x, 1);
+        T left = __shfl_up_sync(0xffffffffu, vc.w, 1);
+        T right = __shfl_down_sync(0xffffffffu, vc.x, 1);
         if (active) {
             if (x0 == 0) left = phi_ghost_x<DIM>(src, f, rc, false);
             else if (lane == 0) left = src.load1(rc.off + x0 - 1);
             if (x0 + 4 >= nx) right = phi_ghost_x<DIM>(src, f, rc, true);
             else if (lane == 31) right = src.load1(rc.off + x0 + 4);
         }
-        float4 xl = make_float4(left, vc.x, vc.y, vc.z);
-        float4 xr = make_float4(vc.y, vc.z, vc.w, right);
+        V xl = f4_make(left, vc.x, vc.y, vc.z);
+        V xr = f4_make(vc.y, vc.z, vc.w, right);
         if (nvalid > 0 && nvalid < 4) f4_set(xr, nvalid - 1, right);      // row ends inside this float4
-        float4 q;
-        q.x = (xl.x + xr.x - 2.f * vc.x) * ix2;
-        q.y = (xl.y + xr.y - 2.f * vc.y) * ix2;
-        q.z = (xl.z + xr.z - 2.f * vc.z) * ix2;
-        q.w = (xl.w + xr.w - 2.f * vc.w) * ix2;
+        V q;
+        q.x = (xl.x + xr.x - two * vc.x) * ix2;
+        q.y = (xl.y + xr.y - two * vc.y) * ix2;
+        q.z = (xl.z + xr.z - two * vc.z) * ix2;
+        q.w = (xl.w + xr.w - two * vc.w) * ix2;
         if (DIM == 3) {
-            q.x += (tl.x + th.x - 2.f * vc.x) * iy2;
-            q.y += (tl.y + th.y - 2.f * vc.y) * iy2;
-            q.z += (tl.z + th.z - 2.f * vc.z) * iy2;
-            q.w += (tl.w + th.w - 2.f * vc.w) * iy2;
+            q.x += (tl.x + th.x - two * vc.x) * iy2;
+            q.y += (tl.y + th.y - two * vc.y) * iy2;
+            q.z += (tl.z + th.z - two * vc.z) * iy2;
+            q.w += (tl.w + th.w - two * vc.w) * iy2;
         }
-        const float im2 = (DIM == 3) ? iz2 : iy2;
-        q.x += (vm.x + vp.x - 2.f * vc.x) * im2;
-        q.y += (vm.y + vp.y - 2.f * vc.y) * im2;
-        q.z += (vm.z + vp.z - 2.f * vc.z) * im2;
-        q.w += (vm.w + vp.w - 2.f * vc.w) * im2;
+        const T im2 = (DIM == 3) ? iz2 : iy2;
+        q.x += (vm.x + vp.x - two * vc.x) * im2;
+        q.y += (vm.y + vp.y - two * vc.y) * im2;
+        q.z += (vm.z + vp.z - two * vc.z) * im2;
+        q.w += (vm.w + vp.w - two * vc.w) * im2;
         if (active) epi(rc.off + x0, vc, q, nvalid);
         vm = vc; vc = vp;
         rc = rowAt(t, m + 1);
@@ -288,11 +325,13 @@ __device__ __forceinline__ void phi_march_masked(const DGrid& g, const DField& f
 }
 
 // Plain array source
-struct SrcArray {
-    const float* a;
-    __device__ __forceinline__ float4 load4(long long off) const { return *reinterpret_cast<const float4*>(a + off); }
-    __device__ __forceinline__ float load1(long long off) const { return a[off]; }
+template <class T>
+struct SrcArrayT {
+    const T* a;
+    __device__ __forceinline__ Vec4<T> load4(long long off) const { return *reinterpret_cast<const Vec4<T>*>(a + off); }
+    __device__ __forceinline__ T load1(long long off) const { return a[off]; }
 };
+using SrcArray = SrcArrayT<float>;
 
 // ---------------------------------------------------------------------------------------------------------
 // Decomposition of a grid into CTA units for the marching kernels
@@ -315,8 +354,8 @@ struct WarpUnit {
     bool valid;
 };
 
-template <int DIM>
-__device__ __forceinline__ WarpUnit phi_warp_unit(const DGrid& g, const UnitMap& um, int unit, int warp)
+template <int DIM, class T>
+__device__ __forceinline__ WarpUnit phi_warp_unit(const DGridT<T>& g, const UnitMap& um, int unit, int warp)
 {
     WarpUnit w;
     w.b = unit / um.units_per_batch;
@@ -345,7 +384,8 @@ int phi_make_dgrid(const PhiGrid* g, DGrid* out);
 int phi_make_centered(const PhiGrid* g, const PhiBC* bc, DField* out);
 int phi_make_component(const PhiGrid* g, const PhiBC* bc, int c, DField* out);
 int phi_pressure_bc(const PhiVBC* vbc, int dim, PhiBC* out);
-UnitMap phi_make_unit_map(const DGrid& g, int target_units);
+template <class T>
+UnitMap phi_make_unit_map(const DGridT<T>& g, int target_units);    // instantiated for float and double in api.cu
 int phi_sm_count();                      // SMs of the current device
 void phi_set_error(const char* fmt, ...);
 void phi_note_launch(const PhiLaunchInfo& info);

@@ -6,30 +6,48 @@
 // ---------------------------------------------------------------------------------------------------------
 // A7  laplace  --  marching stencil, 8 B/cell (read x once, write y once)
 // ---------------------------------------------------------------------------------------------------------
-template <bool AXPY>
+template <bool AXPY, class T>
 struct EpiLaplace {
-    float* y; float coeff;
-    __device__ __forceinline__ void operator()(long long off, const float4& c, const float4& q, int nvalid)
+    T* y; T coeff;
+    __device__ __forceinline__ void operator()(long long off, const Vec4<T>& c, const Vec4<T>& q, int nvalid)
     {
-        float4 o = q;
+        Vec4<T> o = q;
         if (AXPY) { o.x = c.x + coeff * q.x; o.y = c.y + coeff * q.y; o.z = c.z + coeff * q.z; o.w = c.w + coeff * q.w; }
-        if (nvalid == 4) { *reinterpret_cast<float4*>(y + off) = o; }
+        if (nvalid == 4) { *reinterpret_cast<Vec4<T>*>(y + off) = o; }
         else { for (int j = 0; j < nvalid; ++j) y[off + j] = f4_get(o, j); }
     }
 };
 
-template <int DIM, bool AXPY>
+template <int DIM, bool AXPY, class T>
 __global__ void __launch_bounds__(PHI_WARPS_PER_CTA * 32)
-k_laplace(DGrid g, DField f, UnitMap um, const float* __restrict__ x, float* __restrict__ y, float coeff)
+k_laplace(DGridT<T> g, DFieldT<T> f, UnitMap um, const T* __restrict__ x, T* __restrict__ y, T coeff)
 {
     const int warp = threadIdx.x >> 5;
     for (int unit = blockIdx.x; unit < um.total_units; unit += gridDim.x) {
         const WarpUnit w = phi_warp_unit<DIM>(g, um, unit, warp);
         if (!w.valid) continue;
-        SrcArray src{x};
-        EpiLaplace<AXPY> epi{y, coeff};
+        SrcArrayT<T> src{x};
+        EpiLaplace<AXPY, T> epi{y, coeff};
         phi_march<DIM>(g, f, src, epi, w.b, w.xt0, w.t, w.m0, w.m1);
     }
+}
+
+template <class T>
+static int launch_laplace_march(const DGridT<T>& g, const DFieldT<T>& f, const T* x, T* y, T coeff, bool axpy, cudaStream_t s)
+{
+    UnitMap um = phi_make_unit_map(g, phi_sm_count() * 16);
+    const int blocks = um.total_units;
+    dim3 block(PHI_WARPS_PER_CTA * 32);
+    if (g.dim == 3) {
+        if (axpy) k_laplace<3, true, T><<<blocks, block, 0, s>>>(g, f, um, x, y, coeff);
+        else      k_laplace<3, false, T><<<blocks, block, 0, s>>>(g, f, um, x, y, coeff);
+    } else {
+        if (axpy) k_laplace<2, true, T><<<blocks, block, 0, s>>>(g, f, um, x, y, coeff);
+        else      k_laplace<2, false, T><<<blocks, block, 0, s>>>(g, f, um, x, y, coeff);
+    }
+    PhiLaunchInfo li = {}; li.kernel = PHI_KERNEL_LAPLACE_MARCH; li.generic = 1; li.total_units = um.total_units; li.grid_ctas = blocks;
+    phi_note_launch(li);
+    return (int)cudaGetLastError();
 }
 
 int phi_launch_laplace(const DGrid& g, const DField& f, const float* x, float* y, float coeff, bool axpy, cudaStream_t s)
@@ -38,19 +56,12 @@ int phi_launch_laplace(const DGrid& g, const DField& f, const float* x, float* y
         const int e = phi_launch_laplace_ring(g, f, x, y, coeff, axpy, s);
         if (e != -100) return e;
     }
-    UnitMap um = phi_make_unit_map(g, phi_sm_count() * 16);
-    const int blocks = um.total_units;
-    dim3 block(PHI_WARPS_PER_CTA * 32);
-    if (g.dim == 3) {
-        if (axpy) k_laplace<3, true><<<blocks, block, 0, s>>>(g, f, um, x, y, coeff);
-        else      k_laplace<3, false><<<blocks, block, 0, s>>>(g, f, um, x, y, coeff);
-    } else {
-        if (axpy) k_laplace<2, true><<<blocks, block, 0, s>>>(g, f, um, x, y, coeff);
-        else      k_laplace<2, false><<<blocks, block, 0, s>>>(g, f, um, x, y, coeff);
-    }
-    PhiLaunchInfo li = {}; li.kernel = PHI_KERNEL_LAPLACE_MARCH; li.generic = 1; li.total_units = um.total_units; li.grid_ctas = blocks;
-    phi_note_launch(li);
-    return (int)cudaGetLastError();
+    return launch_laplace_march<float>(g, f, x, y, coeff, axpy, s);
+}
+
+int phi_launch_laplace(const DGridT<double>& g, const DFieldT<double>& f, const double* x, double* y, double coeff, bool axpy, cudaStream_t s)
+{
+    return launch_laplace_march<double>(g, f, x, y, coeff, axpy, s);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -58,8 +69,8 @@ int phi_launch_laplace(const DGrid& g, const DField& f, const float* x, float* y
 // ---------------------------------------------------------------------------------------------------------
 struct Idx { int b, x, y, z; };
 
-template <int DIM>
-__device__ __forceinline__ bool phi_thread_index(const DGrid& g, Idx& i)
+template <int DIM, class T>
+__device__ __forceinline__ bool phi_thread_index(const DGridT<T>& g, Idx& i)
 {
     i.x = blockIdx.x * blockDim.x + threadIdx.x;
     i.y = blockIdx.y;
@@ -68,32 +79,34 @@ __device__ __forceinline__ bool phi_thread_index(const DGrid& g, Idx& i)
     return i.x < g.fext[0];
 }
 
-__device__ __forceinline__ bool phi_in_range(const DField& f, int dim, int x, int y, int z)
+template <class T>
+__device__ __forceinline__ bool phi_in_range(const DFieldT<T>& f, int dim, int x, int y, int z)
 {
     bool ok = x >= f.lo[0] && x <= f.hi[0] && y >= f.lo[1] && y <= f.hi[1];
     if (dim == 3) ok = ok && z >= f.lo[2] && z <= f.hi[2];
     return ok;
 }
 
-__device__ __forceinline__ long long phi_off(const DField& f, const Idx& i)
+template <class T>
+__device__ __forceinline__ long long phi_off(const DFieldT<T>& f, const Idx& i)
 {
     return (long long)i.b * f.sb + (long long)i.z * f.sz + (long long)i.y * f.sy + i.x;
 }
 
 // A5: div = sum_d (v_d[i + e_d] - v_d[i]) / dx_d over the n_d + 1 faces of the baked field
-template <int DIM>
+template <int DIM, class T>
 __global__ void __launch_bounds__(128)
-k_divergence(DGrid g, DVec v, DField cf, float* __restrict__ div, const float* __restrict__ accm)
+k_divergence(DGridT<T> g, DVecT<T> v, DFieldT<T> cf, T* __restrict__ div, const T* __restrict__ accm)
 {
     Idx i;
     if (!phi_thread_index<DIM>(g, i)) return;
     if (i.x >= g.n[0] || i.y >= g.n[1] || i.z >= g.n[2]) return;
-    float acc = 0.f;
+    T acc = 0;
 #pragma unroll
     for (int c = 0; c < DIM; ++c) {
-        const float lo = phi_fetch<DIM>(v.p[c], g, v.f[c], i.b, i.x, i.y, i.z);
-        const float hi = phi_fetch<DIM>(v.p[c], g, v.f[c], i.b, i.x + (c == 0), i.y + (c == 1), i.z + (c == 2));
-        const float term = phi_div(hi - lo, g.dx[c], g.inv_dx[c]);
+        const T lo = phi_fetch<DIM>(v.p[c], g, v.f[c], i.b, i.x, i.y, i.z);
+        const T hi = phi_fetch<DIM>(v.p[c], g, v.f[c], i.b, i.x + (c == 0), i.y + (c == 1), i.z + (c == 2));
+        const T term = phi_div(hi - lo, g.dx[c], g.inv_dx[c]);
         acc = (c == 0) ? term : acc + term;
     }
     const long long o = phi_off(cf, i);
@@ -101,9 +114,9 @@ k_divergence(DGrid g, DVec v, DField cf, float* __restrict__ div, const float* _
 }
 
 // A6: v_d[face] -= (p[upper cell] - p[lower cell]) / dx_d on the stored faces
-template <int DIM>
+template <int DIM, class T>
 __global__ void __launch_bounds__(128)
-k_grad_sub(DGrid g, DVec vin, DVecOut v, DField pf, const float* __restrict__ p, DField af, const float* __restrict__ accm)
+k_grad_sub(DGridT<T> g, DVecT<T> vin, DVecOutT<T> v, DFieldT<T> pf, const T* __restrict__ p, DFieldT<T> af, const T* __restrict__ accm)
 {
     Idx i;
     if (!phi_thread_index<DIM>(g, i)) return;
@@ -111,13 +124,13 @@ k_grad_sub(DGrid g, DVec vin, DVecOut v, DField pf, const float* __restrict__ p,
 #pragma unroll
     for (int c = 0; c < DIM; ++c) {
         if (!phi_in_range(vin.f[c], DIM, i.x, i.y, i.z)) continue;
-        const float up = phi_fetch<DIM>(p, g, pf, i.b, i.x, i.y, i.z);
-        const float lw = phi_fetch<DIM>(p, g, pf, i.b, i.x - (c == 0), i.y - (c == 1), i.z - (c == 2));
-        float grad = phi_div(up - lw, g.dx[c], g.inv_dx[c]);
+        const T up = phi_fetch<DIM>(p, g, pf, i.b, i.x, i.y, i.z);
+        const T lw = phi_fetch<DIM>(p, g, pf, i.b, i.x - (c == 0), i.y - (c == 1), i.z - (c == 2));
+        T grad = phi_div(up - lw, g.dx[c], g.inv_dx[c]);
         if (accm) {     // hard_bcs = min of the two adjacent cells' accessibility (fluid.py:134)
-            const float au = phi_fetch<DIM>(accm, g, af, i.b, i.x, i.y, i.z);
-            const float al = phi_fetch<DIM>(accm, g, af, i.b, i.x - (c == 0), i.y - (c == 1), i.z - (c == 2));
-            grad *= fminf(au, al);
+            const T au = phi_fetch<DIM>(accm, g, af, i.b, i.x, i.y, i.z);
+            const T al = phi_fetch<DIM>(accm, g, af, i.b, i.x - (c == 0), i.y - (c == 1), i.z - (c == 2));
+            grad *= phi_min(au, al);
         }
         v.p[c][off] = vin.p[c][off] - grad;
     }
@@ -169,25 +182,50 @@ k_axpy(DGrid g, DField cf, float a, const float* __restrict__ x, float* __restri
     y[off] = y[off] + a * x[off];
 }
 
-static dim3 scalar_grid(const DGrid& g)
+template <class T>
+static dim3 scalar_grid(const DGridT<T>& g)
 {
     return dim3((g.fext[0] + 127) / 128, g.fext[1], g.fext[2] * g.batch);
 }
 
+template <class T>
+static int launch_divergence(const DGridT<T>& g, const DVecT<T>& v, const DFieldT<T>& cf, T* div, const T* acc, cudaStream_t s)
+{
+    if (g.dim == 3) k_divergence<3, T><<<scalar_grid(g), 128, 0, s>>>(g, v, cf, div, acc);
+    else            k_divergence<2, T><<<scalar_grid(g), 128, 0, s>>>(g, v, cf, div, acc);
+    return (int)cudaGetLastError();
+}
+
 int phi_launch_divergence(const DGrid& g, const DVec& v, const DField& cf, float* div, const float* acc, cudaStream_t s)
 {
-    if (g.dim == 3) k_divergence<3><<<scalar_grid(g), 128, 0, s>>>(g, v, cf, div, acc);
-    else            k_divergence<2><<<scalar_grid(g), 128, 0, s>>>(g, v, cf, div, acc);
+    return launch_divergence<float>(g, v, cf, div, acc, s);
+}
+
+int phi_launch_divergence(const DGridT<double>& g, const DVecT<double>& v, const DFieldT<double>& cf, double* div, cudaStream_t s)
+{
+    return launch_divergence<double>(g, v, cf, div, nullptr, s);
+}
+
+template <class T>
+static int launch_grad_sub(const DGridT<T>& g, const DVecT<T>& vin, const DVecOutT<T>& v, const DFieldT<T>& pf, const T* p,
+                           const DFieldT<T>* af, const T* acc, cudaStream_t s)
+{
+    const DFieldT<T> a = af ? *af : pf;
+    if (g.dim == 3) k_grad_sub<3, T><<<scalar_grid(g), 128, 0, s>>>(g, vin, v, pf, p, a, acc);
+    else            k_grad_sub<2, T><<<scalar_grid(g), 128, 0, s>>>(g, vin, v, pf, p, a, acc);
     return (int)cudaGetLastError();
 }
 
 int phi_launch_grad_sub(const DGrid& g, const DVec& vin, const DVecOut& v, const DField& pf, const float* p,
                         const DField* af, const float* acc, cudaStream_t s)
 {
-    const DField a = af ? *af : pf;
-    if (g.dim == 3) k_grad_sub<3><<<scalar_grid(g), 128, 0, s>>>(g, vin, v, pf, p, a, acc);
-    else            k_grad_sub<2><<<scalar_grid(g), 128, 0, s>>>(g, vin, v, pf, p, a, acc);
-    return (int)cudaGetLastError();
+    return launch_grad_sub<float>(g, vin, v, pf, p, af, acc, s);
+}
+
+int phi_launch_grad_sub(const DGridT<double>& g, const DVecT<double>& vin, const DVecOutT<double>& v, const DFieldT<double>& pf,
+                        const double* p, cudaStream_t s)
+{
+    return launch_grad_sub<double>(g, vin, v, pf, p, nullptr, nullptr, s);
 }
 
 int phi_launch_buoyancy(const DGrid& g, const DVec& vin, const DVecOut& v, const DField& sf, const float* sarr,

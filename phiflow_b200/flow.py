@@ -8,10 +8,13 @@ Mirrored (same names, argument meaning and error behaviour; reference file:line 
     advect.{semi_lagrangian, mac_cormack, advect}, diffuse.{explicit, implicit}, fluid.{make_incompressible, incompressible_step},
     write / read (field.write / field.read: the reference's .npz field files, see field_io.py).
 Fused notebook steps (one kernel launch for all substeps of a call): reaction_diffusion (Reaction_Diffusion), wave_step (Waves).
+Precision: math.set_global_precision(64) / math.precision(64) make new grids float64 (the Taylor-Green notebook); laplace,
+diffuse.explicit, divergence, spatial_gradient, semi_lagrangian and make_incompressible with Solve('CG') then run the fp64 kernels.
 Fields hold device tensors in the library layout (DESIGN.md section 2); `.numpy()` returns the reference's (x, y[, z]) arrays.
 Anything outside the fast path raises NotImplementedError (where the reference-side façade would fall through to stock
 PhiFlow, INTEGRATION.md section 2).  No CPU fallback.
 """
+import contextlib
 import numbers
 from builtins import range as builtins_range
 from types import SimpleNamespace
@@ -253,14 +256,52 @@ class Diverged(ConvergenceException):
     """_optimize.py: raised when the residual grows (stop_on_l2, _linalg.py:29-36)"""
 
 
+_PRECISION = [32]
+
+
+def set_global_precision(bits: int):
+    """math.set_global_precision (PhiML/phiml/backend/_dtype.py): 32 or 64 bits for the grids created from now on."""
+    _require(bits in (32, 64), f"precision {bits}")
+    _PRECISION[0] = int(bits)
+
+
+def get_precision() -> int:
+    return _PRECISION[0]
+
+
+@contextlib.contextmanager
+def precision(bits: int):
+    """with math.precision(64): ... (PhiML/phiml/backend/_dtype.py)."""
+    old = _PRECISION[0]
+    set_global_precision(bits)
+    try:
+        yield
+    finally:
+        _PRECISION[0] = old
+
+
+def _default_tolerance() -> float:
+    """_optimize.py:130-136: 1e-12 in precision 64, 1e-5 in precision 32, taken when the solve runs."""
+    return 1e-12 if _PRECISION[0] == 64 else 1e-5
+
+
 class Solve:
-    """phiml.math.Solve (_optimize.py:25-41): method, rel_tol, abs_tol, x0, max_iterations, suppress."""
+    """phiml.math.Solve (_optimize.py:25-41): method, rel_tol, abs_tol, x0, max_iterations, suppress.  rel_tol / abs_tol left at None
+    take _default_tolerance() of the precision in force when they are read (_optimize.py:108-111)."""
 
     def __init__(self, method='auto', rel_tol=None, abs_tol=None, x0=None, max_iterations=1000, suppress=(), matrix_offset=0.0):
         self.method, self.x0, self.max_iterations, self.suppress = method or 'auto', x0, int(max_iterations), tuple(suppress)
-        self.rel_tol = 1e-5 if rel_tol is None else float(rel_tol)        # _default_tolerance, fp32 (_optimize.py:130-136)
-        self.abs_tol = 1e-5 if abs_tol is None else float(abs_tol)
+        self._rel_tol = None if rel_tol is None else float(rel_tol)
+        self._abs_tol = None if abs_tol is None else float(abs_tol)
         self.matrix_offset = matrix_offset                                # see DESIGN.md section 3; 0 = plain CG
+
+    @property
+    def rel_tol(self) -> float:
+        return _default_tolerance() if self._rel_tol is None else self._rel_tol
+
+    @property
+    def abs_tol(self) -> float:
+        return _default_tolerance() if self._abs_tol is None else self._abs_tol
 
 
 class SolveInfo:
@@ -313,7 +354,8 @@ def rotate_vector(vector, angle):
 
 
 math = SimpleNamespace(Solve=Solve, SolveTape=SolveTape, NotConverged=NotConverged, Diverged=Diverged,
-                       ConvergenceException=ConvergenceException, extrapolation=extrapolation, sin=_sin, PI=np.pi, rotate_vector=rotate_vector)
+                       ConvergenceException=ConvergenceException, extrapolation=extrapolation, sin=_sin, PI=np.pi, rotate_vector=rotate_vector,
+                       set_global_precision=set_global_precision, get_precision=get_precision, precision=precision)
 
 
 def jit_compile(f=None, **_):
@@ -363,12 +405,19 @@ def set_device(device):
     _DEVICE = str(device)
 
 
-def _domain(res, dx, batch, vspec):
+def _domain(res, dx, batch, vspec, dtype):
     upper = tuple(ops.stored_faces(vspec, a)[1] for a in range(len(res))) if vspec is not None else (False,) * len(res)
-    key = (tuple(res), tuple(dx), batch, upper, _DEVICE)
+    key = (tuple(res), tuple(dx), batch, upper, _DEVICE, dtype)
     if key not in _DOMAINS:
-        _DOMAINS[key] = ops.Domain(res, dx, batch, vbc=vspec, device=_DEVICE)
+        _DOMAINS[key] = ops.Domain(res, dx, batch, vbc=vspec, device=_DEVICE, dtype=dtype)
     return _DOMAINS[key]
+
+
+def _grid_dtype(data):
+    """dtype of a new grid: that of the data it wraps, else the global precision's."""
+    if data is not None:
+        return (data[0] if isinstance(data, (list, tuple)) else data).dtype
+    return torch.float64 if _PRECISION[0] == 64 else torch.float32
 
 
 class _Grid:
@@ -389,6 +438,10 @@ class _Grid:
     def _same_grid(self, other):
         return self.res == other.res and self.lower == other.lower and self.upper == other.upper and self.batch == other.batch
 
+    @property
+    def precision(self) -> int:
+        return 64 if self.dom.dtype == torch.float64 else 32
+
 
 class CenteredGrid(_Grid):
     """CenteredGrid(values, boundary, bounds, x=..., y=...)  (phi/field/_grid.py:21-86).
@@ -397,18 +450,19 @@ class CenteredGrid(_Grid):
     def __init__(self, values=0., boundary=ZERO, bounds=None, batch=1, _data=None, _scale=None, **resolution):
         self._geometry(bounds, resolution, batch)
         self.boundary = _as_ext(boundary)
-        self.dom = _domain(self.res, self.dx, batch, None)
+        self.dom = _domain(self.res, self.dx, batch, None, _grid_dtype(_data))
         self.vector_scale = _scale                       # s * (0, 0.1): a centred vector field that is a scalar times constants
         if _data is not None:
             self.data = _data
         elif isinstance(values, (Box, Sphere, Union)):
-            self.data = self.dom.centered_from_numpy(values.lies_inside(self.points()).astype(np.float32))
+            _require_f32("a geometry as grid values (its mask is sampled at float32 cell centres)", self)
+            self.data = self.dom.centered_from_numpy(values.lies_inside(self.points()).astype(self.dom.np_dtype))
         elif np.isscalar(values):
             self.data = self.dom.alloc_centered()
             if values != 0:
                 self.data += float(values)
         else:
-            self.data = self.dom.centered_from_numpy(np.asarray(values, np.float32))
+            self.data = self.dom.centered_from_numpy(np.asarray(values, self.dom.np_dtype))
 
     def points(self):
         axes = [(np.linspace(0.5 / n, 1 - 0.5 / n, n).astype(np.float32) * np.float32(u - l) + np.float32(l)) for l, u, n in zip(self.lower, self.upper, self.res)]
@@ -443,6 +497,7 @@ class CenteredGrid(_Grid):
     def __add__(self, other):
         if isinstance(other, CenteredGrid):
             assert self._same_grid(other)
+            _same_precision(self, other)
             return self.with_values(self.data + other.data)
         return self.with_values(self.data + float(other))
 
@@ -457,6 +512,7 @@ class CenteredGrid(_Grid):
             g.vector_scale = tuple(float(o) for o in other)
             return g
         if isinstance(other, CenteredGrid):
+            _same_precision(self, other)
             return self.with_values(self.data * other.data)
         return self.with_values(self.data * float(other))
 
@@ -487,20 +543,22 @@ class StaggeredGrid(_Grid):
         self._geometry(bounds, resolution, batch)
         self.boundary = _as_ext(boundary)
         self.vspec = self.boundary.vspec(self.axes)
-        self.dom = _domain(self.res, self.dx, batch, self.vspec)
+        self.dom = _domain(self.res, self.dx, batch, self.vspec, _grid_dtype(_data))
         d = len(self.res)
         if _data is not None:
             self.data = _data
             return
         shapes, _ = self.dom.face_shapes(self.vspec)
+        dt = self.dom.np_dtype
         if isinstance(values, (Box, Sphere)):
-            comps = [values.lies_inside(self.face_points(c)).astype(np.float32) for c in range(d)]
+            _require_f32("a geometry as grid values (its mask is sampled at float32 face centres)", self)
+            comps = [values.lies_inside(self.face_points(c)).astype(dt) for c in range(d)]
         elif np.isscalar(values):
-            comps = [np.full(shapes[c], values, np.float32) for c in range(d)]
+            comps = [np.full(shapes[c], values, dt) for c in range(d)]
         elif isinstance(values, tuple) and all(np.isscalar(v) for v in values):
-            comps = [np.full(shapes[c], values[c], np.float32) for c in range(d)]
+            comps = [np.full(shapes[c], values[c], dt) for c in range(d)]
         else:
-            comps = [np.asarray(v, np.float32) for v in values]
+            comps = [np.asarray(v, dt) for v in values]
         self.data = self.dom.faces_from_numpy(comps, self.vspec)
 
     def face_points(self, c):
@@ -523,13 +581,14 @@ class StaggeredGrid(_Grid):
         if boundary == self.boundary:
             return self
         # different stored faces: go through the reference layout (tests/commit/field/test__grid.py:85-94)
-        new = StaggeredGrid(0, boundary, self.bounds, self.batch, **dict(zip(self.axes, self.res)))
+        with precision(self.precision):
+            new = StaggeredGrid(0, boundary, self.bounds, self.batch, **dict(zip(self.axes, self.res)))
         old = self.numpy()
         comps = []
         for c, a in enumerate(self.axes):
             lo0, hi0 = self.boundary.valid_outer_faces(a)
             lo1, hi1 = boundary.valid_outer_faces(a)
-            full = np.zeros(old[c].shape[:old[c].ndim - len(self.res)] + tuple(n + (1 if i == c else 0) for i, n in enumerate(self.res)), np.float32)
+            full = np.zeros(old[c].shape[:old[c].ndim - len(self.res)] + tuple(n + (1 if i == c else 0) for i, n in enumerate(self.res)), old[c].dtype)
             sl = [slice(None)] * full.ndim
             ax = full.ndim - len(self.res) + c
             sl[ax] = slice(0 if lo0 else 1, self.res[c] + 1 if hi0 else self.res[c])
@@ -552,6 +611,7 @@ class StaggeredGrid(_Grid):
     def _binary(self, other, fn):
         if isinstance(other, StaggeredGrid):
             assert self._same_grid(other) and other.boundary == self.boundary, "staggered operands must share grid and boundary"
+            _same_precision(self, other)
             return self.with_values([fn(a, b) for a, b in zip(self.data, other.data)])
         if isinstance(other, (tuple, list)):
             return self.with_values([fn(a, float(o)) for a, o in zip(self.data, other)])
@@ -577,6 +637,16 @@ class StaggeredGrid(_Grid):
 def _require(cond, what):
     if not cond:
         raise NotImplementedError(f"{what} is outside the phiflow_b200 fast path (use stock PhiFlow)")
+
+
+def _same_precision(*fields):
+    """Fields of one operation share their precision: nothing is converted silently."""
+    bits = {f.precision for f in fields if isinstance(f, _Grid)}
+    _require(len(bits) <= 1, "mixing float32 and float64 fields in one operation")
+
+
+def _require_f32(what, *fields):
+    _require(all(f.precision == 32 for f in fields if isinstance(f, _Grid)), f"{what} in precision 64 (fp32 only)")
 
 
 def divergence(v: StaggeredGrid, order=2) -> CenteredGrid:
@@ -611,7 +681,8 @@ def spatial_gradient(p: CenteredGrid, boundary=None, at='face', order=2) -> Stag
     boundary = _as_ext(boundary)
     _require(at == 'face' and order == 2, "spatial_gradient other than at='face', order 2")
     _require(_pressure_boundary(boundary) == p.boundary, "spatial_gradient with an unrelated field boundary")
-    g = StaggeredGrid(0, boundary, p.bounds, p.batch, **dict(zip(p.axes, p.res)))
+    with precision(p.precision):
+        g = StaggeredGrid(0, boundary, p.bounds, p.batch, **dict(zip(p.axes, p.res)))
     ops.grad_sub(g.dom, g.vspec, g.data, p.data)
     return g * -1.0
 
@@ -620,12 +691,14 @@ def resample(value, to, soft=False, **_):
     """resample(value, to) for the two cases of the notebook step (phi/field/_resample.py:13-63):
     geometry -> CenteredGrid (soft mask, :192-210) and (CenteredGrid * constant vector) -> StaggeredGrid (:272-276)."""
     if isinstance(value, Sphere) and isinstance(to, CenteredGrid):
+        _require_f32("resample(geometry, to=CenteredGrid) (the mask is sampled at float32 cell centres)", to)
         if soft:
             cell_r = float(np.sqrt(sum((h * 0.5) ** 2 for h in to.dx)))
             return to.with_values(to.dom.centered_from_numpy(value.soft_mask(to.points(), cell_r)))
         return to.with_values(to.dom.centered_from_numpy(value.lies_inside(to.points()).astype(np.float32)))
     if isinstance(value, CenteredGrid) and isinstance(to, StaggeredGrid) and value.vector_scale is not None:
         _require(value.res == to.res, "resampling between different resolutions")
+        _require_f32("resample(CenteredGrid * vector, to=StaggeredGrid)", value, to)
         out = StaggeredGrid(0, to.boundary, to.bounds, to.batch, **dict(zip(to.axes, to.res)))
         ops.add_buoyancy(out.dom, out.vspec, value.spec, value.data, value.vector_scale, 1.0, out.data)
         return out
@@ -663,17 +736,20 @@ def read(file: str):
     _require(len(lead) <= 1 and names[:len(lead)] == lead and names[len(lead):len(lead) + len(axes)] == axes, "batch dims after spatial dims")
     default, sides = field_io.extrapolation_from_dict(st['extrapolation'])
     boundary = Extrapolation(default, sides)
-    data = np.asarray(st['data'], np.float32)
+    bits = 64 if np.asarray(st['data']).dtype == np.float64 else 32          # float64 files stay float64
+    data = np.asarray(st['data'], np.float64 if bits == 64 else np.float32)
     batch = data.shape[0] if lead else 1
     bounds = Box(**{a: (st['lower'][a], st['upper'][a]) for a in axes})
     if st['field_type'] == 'CenteredGrid':
         _require(data.ndim == len(lead) + len(axes), "centred grids with channel dims")
         res = dict(zip(axes, data.shape[len(lead):]))
-        return CenteredGrid(data, boundary, bounds, batch, **res)
+        with precision(bits):
+            return CenteredGrid(data, boundary, bounds, batch, **res)
     _require(names[-1] == 'vector' and data.shape[-1] == len(axes), "staggered tensors whose components are not the spatial dims")
     comps = field_io.unstack_staggered_tensor(data, lambda ax: (boundary.side(axes[ax], False), boundary.side(axes[ax], True)), len(axes))
     res = {a: n - 1 for a, n in zip(axes, data.shape[len(lead):len(lead) + len(axes)])}
-    return StaggeredGrid(comps, boundary, bounds, batch, **res)
+    with precision(bits):
+        return StaggeredGrid(comps, boundary, bounds, batch, **res)
 
 
 def where(mask, field_true, field_false):
@@ -687,6 +763,7 @@ def where(mask, field_true, field_false):
     _require(all(f._same_grid(ref) and f.vector_scale is None for f in fields), "field.where of vector fields or fields on different grids")
     plain = lambda x: isinstance(x, numbers.Real) and not isinstance(x, bool)
     _require(all(isinstance(x, CenteredGrid) or plain(x) for x in (field_true, field_false)), "field.where with non-number values")
+    _require_f32("field.where", *fields)
     if isinstance(mask, CenteredGrid):
         m = mask.data != 0
     else:
@@ -727,6 +804,7 @@ class Scene(_scene.Scene):
 def _check_velocity(fld, velocity):
     _require(isinstance(velocity, StaggeredGrid), "advection by a non-staggered velocity")
     _require(fld.res == velocity.res and fld.lower == velocity.lower and fld.upper == velocity.upper, "advection across different grids")
+    _same_precision(fld, velocity)
 
 
 def semi_lagrangian(fld, velocity: StaggeredGrid, dt: float, integrator=None):
@@ -744,6 +822,7 @@ def mac_cormack(fld, velocity: StaggeredGrid, dt: float, correction_strength=1.0
     """advect.mac_cormack (phi/physics/advect.py:182-215); centred fields only on the fast path."""
     _require(integrator is None and isinstance(fld, CenteredGrid), "mac_cormack of staggered fields / other integrators")
     _check_velocity(fld, velocity)
+    _require_f32("advect.mac_cormack", fld, velocity)
     return fld.with_values(ops.mac_cormack_centered(velocity.dom, velocity.vspec, velocity.data, fld.spec, fld.data, float(dt), correction_strength))
 
 
@@ -776,6 +855,7 @@ def implicit(fld, diffusivity: float, dt: float, solve: Solve = None):
     (diffuse.py:129-141, Heat_Flow.ipynb): see _implicit_varying."""
     solve = solve or Solve('CG')
     plain = lambda v: isinstance(v, numbers.Real) and not isinstance(v, bool)
+    _require_f32("diffuse.implicit", fld, diffusivity)
     if isinstance(diffusivity, CenteredGrid) and isinstance(fld, CenteredGrid):
         return _implicit_varying(fld, diffusivity, dt, solve)
     _require(plain(diffusivity) and plain(dt), "implicit diffusion with a Field / vector / per-batch diffusivity or dt")
@@ -842,6 +922,7 @@ def reaction_diffusion(u: CenteredGrid, v: CenteredGrid, du: float, dv: float, f
     _require(isinstance(u, CenteredGrid) and isinstance(v, CenteredGrid), "reaction-diffusion of non-centred fields")
     _require(u.vector_scale is None and v.vector_scale is None, "reaction-diffusion of vector fields")
     _require(u._same_grid(v), "reaction-diffusion of fields on different grids")
+    _require_f32("reaction_diffusion", u, v)
     _require(all(plain(x) for x in (du, dv, f, k, dt)), "reaction-diffusion with Field / per-batch parameters")
     _require(isinstance(substeps, int) and substeps >= 0, f"substeps = {substeps!r}")
     su, sv = u.spec, v.spec
@@ -870,6 +951,7 @@ def wave_step(h_c: CenteredGrid, h_p: CenteredGrid, time, dt: float, k_speed: fl
     _require(isinstance(h_c, CenteredGrid) and isinstance(h_p, CenteredGrid), "the wave step of non-centred fields")
     _require(h_c.vector_scale is None and h_p.vector_scale is None, "the wave step of vector fields")
     _require(h_c._same_grid(h_p) and h_c.boundary == h_p.boundary, "the wave step of fields on different grids or with different boundaries")
+    _require_f32("wave_step", h_c, h_p)
     _require(all(plain(x) for x in (time, dt, k_speed, k_damp)), "the wave step with Field / per-batch parameters")
     _require(isinstance(substeps, int) and substeps >= 0, f"substeps = {substeps!r}")
     _require(all(_fixed_point_side(s) for ax in h_c.spec for s in ax),
@@ -902,8 +984,10 @@ def _cg_params(v: StaggeredGrid, solve: Solve):
     # kernel only: on grids whose lines do not fit it, 'auto' and 'CG-adaptive' raise Unsupported.
     _require(solve.method in ('CG', 'auto', 'CG-adaptive'), f"solver '{solve.method}'")
     adaptive = solve.method in ('CG-adaptive', 'auto')
+    _require(not adaptive or v.precision == 32, f"Solve('{solve.method}') in precision 64 (CG-adaptive runs on the fp32 ring kernel only; "
+                                                f"use Solve('CG'))")
     return ops.cg_params(v.vspec, rtol=solve.rel_tol, atol=solve.abs_tol, max_iter=solve.max_iterations,
-                         matrix_offset=0.0 if adaptive else solve.matrix_offset, method='CG-adaptive' if adaptive else 'CG')
+                         matrix_offset=0.0 if adaptive else solve.matrix_offset, method='CG-adaptive' if adaptive else 'CG', dtype=v.dom.dtype)
 
 
 def _finish_solve(dom, solve: Solve, raw=None):
@@ -978,7 +1062,9 @@ def make_incompressible(velocity: StaggeredGrid, obstacles=(), solve: Solve = No
     _require(active is None and order == 2, "active masks / higher order")
     if solve.x0 is not None:
         _require(isinstance(solve.x0, CenteredGrid) and solve.x0.res == velocity.res and solve.x0.batch == velocity.batch, "x0 on a different grid")
+        _same_precision(velocity, solve.x0)
     if obstacles:
+        _require_f32("make_incompressible with obstacles", velocity)
         accessible, factors = _obstacle_masks_cached(velocity, obstacles)
         res = dict(zip(velocity.axes, velocity.res))
         p_data = solve.x0.data.clone() if solve.x0 is not None else velocity.dom.alloc_centered()
@@ -1010,6 +1096,7 @@ def incompressible_step(v: StaggeredGrid, s: CenteredGrid, p, dt: float, inflow:
     Returns new (v, s, p); inputs are not modified."""
     solve = solve or Solve('CG', 1e-3)
     _check_velocity(s, v)
+    _require_f32("incompressible_step", v, s, p)
     kw = {}
     if obstacles:
         kw['accessible'], kw['factors'] = _obstacle_masks_cached(v, obstacles)
