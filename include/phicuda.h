@@ -12,7 +12,7 @@
  *     cudaMalloc + cudaMemset + device synchronisation / CUDA-IPC open / cudaFree - once per run, never inside a step);
  *   - return 0 on success, a negative PHI_ERR_* or a positive cudaError_t otherwise; the message is kept per thread
  *     and read with phicuda_last_error();
- *   - fp32 (`_f32`) throughout; fp64 (`_f64`, math.set_global_precision(64)) for the stencils, semi-Lagrangian advection and the
+ *   - fp32 (`_f32`) throughout (phicuda_julia_f32 computes in float32 and writes int32 counts); fp64 (`_f64`, math.set_global_precision(64)) for the stencils, semi-Lagrangian advection and the
  *     CG pressure projection (see "fp64" below).  Other precisions are not part of this path (the reference falls through to its
  *     stock backends).
  *
@@ -118,6 +118,7 @@ int         phicuda_device_info(char* name, size_t name_len, int* sm_count, int*
 #define PHI_KERNEL_STENCIL_RING  5   /* k_div_ring / k_gradsub_ring / k_advect_ring: see `stencil` */
 #define PHI_KERNEL_RD_RING       6   /* k_rd_ring       (persistent, TMA ring): phicuda_reaction_diffusion_f32 */
 #define PHI_KERNEL_WAVE_RING     7   /* k_wave_ring     (persistent, TMA ring): phicuda_wave_f32 */
+#define PHI_KERNEL_JULIA         8   /* k_julia         (one thread per batch entry and cell): phicuda_julia_f32 */
 typedef struct PhiLaunchInfo {
     int32_t kernel;        /* PHI_KERNEL_* */
     int32_t generic;       /* 1: variant with per-tile boundary handling, 0: branch-free variant (every tile qualifies) */
@@ -361,6 +362,21 @@ size_t phicuda_wave_scratch_bytes(const PhiGrid* g, int32_t substeps);
 int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, float dd, float k_speed, float k_damp,
                      const PhiWaveDisc* discs, float radius_sq, const float* centers, int32_t substeps, void* scratch,
                      size_t scratch_bytes, void* stream);
+
+/* ---- N10  Julia sets: the Julia_Set notebook's escape counts ---------------------------------------------------------------------
+ * For batch entry b with constant c_b = c[2b] + i c[2b+1] and every cell (i, j) of a 2-D grid, with z_0 = x_i + i y_j:
+ *   counts[b][j][i] = #{ t < iterations : abs(z_t) < 2 },   z_{t+1} = z_t ** 2 + c_b
+ * rounded as PhiML's NumPy backend rounds complex64 on an AVX-512 CPU: z ** 2 = (a*a - b*b, a*b + b*a) without fma (np.power),
+ * then + c per component; abs(z) = big * sqrt(fma(r, r, 1)), r = small / big over |a|, |b|.  Counts are int32 in the centred-array layout of `g`
+ * (element size 4); only the owned cells are written, iterations == 0 writes zeros.  `centers`: n[0] x coordinates, then n[1] y
+ * (host memory, finite), as the caller's grid computes them; `c`: 2 * batch floats (host memory), any values - non-finite constants
+ * count as NumPy's inf / NaN arithmetic does.  Both are copied into `scratch` (phicuda_julia_scratch_bytes) on `stream`, a copy from
+ * pageable memory that waits for the stream's earlier work.  One kernel launch (PHI_KERNEL_JULIA), compute-bound: 4 B/cell written.
+ * 2-D only (3-D returns PHI_ERR_UNSUPPORTED), one GPU.  Every argument check runs before the first CUDA call: a refused call leaves
+ * counts untouched. */
+size_t phicuda_julia_scratch_bytes(const PhiGrid* g);
+int phicuda_julia_f32(const PhiGrid* g, const float* centers, const float* c, int32_t iterations, int32_t* counts, void* scratch,
+                      size_t scratch_bytes, void* stream);
 
 /* ---- N9  fp64: the Taylor-Green step of math.set_global_precision(64) -----------------------------------------------------
  * The same operations as their _f32 counterparts on float64 arrays (same layout, element size 8; x-rows stay padded to multiples of

@@ -43,7 +43,7 @@ class PhiLaunchInfo(C.Structure):
                                          'total_units', 'grid_ctas', 'split')]
 
 
-KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING, KERNEL_RD_RING, KERNEL_WAVE_RING = range(8)
+KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING, KERNEL_RD_RING, KERNEL_WAVE_RING, KERNEL_JULIA = range(9)
 
 
 class PhiWaveDisc(C.Structure):
@@ -132,6 +132,8 @@ PROTOTYPES = {
     'phicuda_wave_scratch_bytes': (C.c_size_t, [_P(PhiGrid), C.c_int32]),
     'phicuda_wave_f32': (C.c_int, [_P(PhiGrid), _P(PhiBC), C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, _P(PhiWaveDisc),
                                    C.c_float, _P(C.c_float), C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'phicuda_julia_scratch_bytes': (C.c_size_t, [_P(PhiGrid)]),
+    'phicuda_julia_f32': (C.c_int, [_P(PhiGrid), _P(C.c_float), _P(C.c_float), C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     'phicuda_laplace_f64': (C.c_int, [_P(PhiGrid), _P(PhiBC), _P(PhiValues64), C.c_void_p, C.c_void_p, C.c_void_p]),
     'phicuda_laplace_axpy_f64': (C.c_int, [_P(PhiGrid), _P(PhiBC), _P(PhiValues64), C.c_void_p, C.c_double, C.c_void_p, C.c_void_p]),
     'phicuda_divergence_f64': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiValues64), F3, C.c_void_p, C.c_void_p]),

@@ -52,9 +52,11 @@ def _dtype_of(dom, *ts) -> torch.dtype:
 
 
 def _f32_only(what: str, dom, *ts):
-    """Entry points without an fp64 kernel refuse float64 arrays and float64 domains instead of reading them as float32."""
-    if dom.dtype == torch.float64 or any(t is not None and t.dtype == torch.float64 for t in ts):
-        raise _lib.Unsupported(_lib.ERR_UNSUPPORTED, f"{what}: float64 arrays are not supported (fp32 only; the fp64 path covers laplace, "
+    """Entry points without an fp64 kernel refuse float64 domains and every array that is not float32 (float64, or the int32 counts of
+    `julia`) instead of reading it as float32."""
+    bad = sorted({str(t.dtype) for t in ts if t is not None and t.dtype != torch.float32} | ({str(dom.dtype)} if dom.dtype != torch.float32 else set()))
+    if bad:
+        raise _lib.Unsupported(_lib.ERR_UNSUPPORTED, f"{what}: {', '.join(bad)} arrays are not supported (fp32 only; the fp64 path covers laplace, "
                                                      f"divergence, grad_sub, semi-Lagrangian advection and the CG projection)")
 
 
@@ -577,6 +579,28 @@ def wave(dom: Domain, spec, h_c, h_p, dd: float, k_speed: float, k_damp: float, 
                                     C.c_float(k_damp), table, C.c_float(radius_sq), coords.ctypes.data_as(C.POINTER(C.c_float)),
                                     C.c_int32(substeps), _ptr(scratch), C.c_size_t(4 * scratch.numel()), _stream()))
     return hc, hp
+
+
+def julia(dom: Domain, centres, c, iterations: int, out=None):
+    """The Julia_Set notebook's escape counts in one launch (include/phicuda.h, N10): for batch entry b and cell (i, j), the number of
+    t < iterations with abs(z_t) < 2, z_0 = centres_x[i] + i centres_y[j], z_{t+1} = z_t ** 2 + c[b], rounded as PhiML's complex64.
+    dom: a 2-D float32 domain with batch len(c) (its centred layout holds the int32 counts); centres: per-axis float32 cell centres (x,
+    then y); c: `batch` complex constants.  Returns `out` (or a new int32 centred array) with every owned cell written."""
+    require_cuda()
+    assert dom.dim == 2 and dom.dtype == torch.float32, "Julia counts are offered on 2-D float32-layout domains"
+    cc = np.ascontiguousarray(np.asarray(c, np.complex64).reshape(-1))
+    assert cc.size == dom.batch, f"{cc.size} constants for a domain of batch {dom.batch}"
+    coords = np.ascontiguousarray(centres, dtype=np.float32).reshape(-1)
+    assert coords.size == sum(dom.res), f"{coords.size} cell centres for resolution {dom.res}"
+    shape = dom._shape(dom.cext)
+    out = torch.zeros(shape, dtype=torch.int32, device=dom.device) if out is None else out
+    assert out.dtype == torch.int32 and tuple(out.shape) == shape and out.is_contiguous(), f"out: {out.dtype} {tuple(out.shape)} is not an int32 centred array of the domain"
+    lib = _lib.load()
+    scratch = _cached_scratch(dom, '_julia_scratch', lib.phicuda_julia_scratch_bytes(C.byref(dom.grid)))
+    pairs = cc.view(np.float32)
+    _lib.check(lib.phicuda_julia_f32(C.byref(dom.grid), coords.ctypes.data_as(C.POINTER(C.c_float)), pairs.ctypes.data_as(C.POINTER(C.c_float)),
+                                     C.c_int32(iterations), _ptr(out), _ptr(scratch), C.c_size_t(4 * scratch.numel()), _stream()))
+    return out
 
 
 def mul_faces(dom: Domain, vbc, v, mask):

@@ -828,6 +828,37 @@ int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, 
     return cuda_fail(e, "wave");
 }
 
+// scratch of the Julia counts: [batch (re, im) pairs of c][n[0] x centres][n[1] y centres]
+size_t phicuda_julia_scratch_bytes(const PhiGrid* g)
+{
+    return g ? (2 * (size_t)g->batch + (size_t)g->n[0] + (size_t)g->n[1]) * sizeof(float) : 0;
+}
+
+int phicuda_julia_f32(const PhiGrid* g, const float* centers, const float* c, int32_t iterations, int32_t* counts, void* scratch,
+                      size_t scratch_bytes, void* stream)
+{
+    // every check runs before the first CUDA call: a refused call leaves counts untouched
+    DGrid dg;
+    CHECK(phi_make_dgrid(g, &dg));
+    if (g->dim != 2) { phi_set_error("julia: 2-D grids only, got %d-D", g->dim); return PHI_ERR_UNSUPPORTED; }
+    if (!centers || !c || !counts || !scratch) { phi_set_error("julia: NULL argument"); return PHI_ERR_INVALID; }
+    if (iterations < 0) { phi_set_error("julia: iterations must be >= 0, got %d", iterations); return PHI_ERR_INVALID; }
+    const int naxis = g->n[0] + g->n[1];
+    for (int i = 0; i < naxis; ++i)
+        if (!std::isfinite(centers[i])) { phi_set_error("julia: cell centre %d is not finite", i); return PHI_ERR_INVALID; }
+    const size_t need = phicuda_julia_scratch_bytes(g);
+    if (scratch_bytes < need) { phi_set_error("julia: scratch %zu < %zu bytes", scratch_bytes, need); return PHI_ERR_INVALID; }
+    if (overlap(scratch, need, counts, centred_elems(g) * sizeof(int32_t))) { phi_set_error("julia: scratch overlaps counts"); return PHI_ERR_INVALID; }
+    std::vector<float> table(need / sizeof(float));
+    memcpy(table.data(), c, 2 * (size_t)g->batch * sizeof(float));
+    memcpy(table.data() + 2 * (size_t)g->batch, centers, (size_t)naxis * sizeof(float));
+    float* dtab = (float*)scratch;
+    cudaError_t ce = cudaMemcpyAsync(dtab, table.data(), need, cudaMemcpyHostToDevice, (cudaStream_t)stream);
+    if (ce != cudaSuccess) return cuda_fail((int)ce, "julia");
+    const float* xc = dtab + 2 * (size_t)g->batch;
+    return cuda_fail(phi_launch_julia(dg, dtab, xc, xc + g->n[0], iterations, counts, (cudaStream_t)stream), "julia");
+}
+
 }  // extern "C"
 
 // ---- N9: fp64 ------------------------------------------------------------------------------------------------------------

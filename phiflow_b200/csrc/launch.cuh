@@ -127,3 +127,6 @@ struct WaveParams { float dd, k_speed, k_damp, r2; };
 // tmp: one centred array, written only for an odd substep count
 int phi_launch_wave(const DGrid& g, const DField& f, float* hc, float* hp, float* tmp, const WaveDisc* discs, const float* coords,
                     const WaveParams& p, int substeps, cudaStream_t s);
+// N10 the Julia_Set notebook's escape counts (julia_kernels.cu), 2-D: c = batch interleaved (re, im) pairs, xc / yc = n[0] / n[1] cell
+// centres, all in device memory; counts: int32 in the centred-array layout, every owned cell written (0 for iterations == 0)
+int phi_launch_julia(const DGrid& g, const float* c, const float* xc, const float* yc, int iterations, int32_t* counts, cudaStream_t s);

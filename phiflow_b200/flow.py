@@ -4,10 +4,12 @@
 
 Mirrored (same names, argument meaning and error behaviour; reference file:line in each docstring):
     Box, Sphere, union, geom.infinite_cylinder, CenteredGrid, StaggeredGrid, extrapolation (ZERO, ONE, PERIODIC, ZERO_GRADIENT, BOUNDARY, combine_sides),
-    Solve, SolveTape, NotConverged, Diverged, math.{sin, PI, rotate_vector}, field.{divergence, laplace, spatial_gradient, where}, resample,
+    Solve, SolveTape, NotConverged, Diverged, math.{sin, exp, linspace, PI, rotate_vector}, PI, field.{divergence, laplace, spatial_gradient, where}, resample,
     advect.{semi_lagrangian, mac_cormack, advect}, diffuse.{explicit, implicit}, fluid.{make_incompressible, incompressible_step},
     write / read (field.write / field.read: the reference's .npz field files, see field_io.py).
 Fused notebook steps (one kernel launch for all substeps of a call): reaction_diffusion (Reaction_Diffusion), wave_step (Waves).
+Julia_Set: julia_set(c, iter_count, bounds, x=..., y=...) returns the escape counts as an int32 CenteredGrid in one kernel launch; an
+int32 grid is a result only, which every operator refuses.
 Precision: math.set_global_precision(64) / math.precision(64) make new grids float64 (the Taylor-Green notebook); laplace,
 diffuse.explicit, divergence, spatial_gradient, semi_lagrangian and make_incompressible with Solve('CG') then run the fp64 kernels.
 Fields hold device tensors in the library layout (DESIGN.md section 2); `.numpy()` returns the reference's (x, y[, z]) arrays.
@@ -29,7 +31,7 @@ from . import scene as _scene
 
 __all__ = ['Scene', 'vec', 'batch', 'iterate', 'jit_compile', 'Box', 'Sphere', 'union', 'geom', 'CenteredGrid', 'StaggeredGrid', 'extrapolation', 'ZERO', 'ONE', 'PERIODIC', 'ZERO_GRADIENT',
            'BOUNDARY', 'combine_sides', 'Solve', 'SolveTape', 'NotConverged', 'Diverged', 'ConvergenceException', 'field',
-           'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read', 'wave_step']
+           'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read', 'wave_step', 'julia_set', 'PI']
 
 AXES = 'xyz'
 
@@ -353,8 +355,28 @@ def rotate_vector(vector, angle):
     return np.array([c * v[0] + (-s) * v[1], s * v[0] + c * v[1]], np.float32)
 
 
+def _linspace(start, stop, dim):
+    """math.linspace(start, stop, batch(time=N)) (PhiML/phiml/math/_ops.py:648): N float32 numbers from start to stop, as a NumPy
+    array along the one dimension (the notebooks' constants); bit for bit PhiML's, whose limits arrive as float32 numbers."""
+    plain = lambda v: isinstance(v, numbers.Real) and not isinstance(v, bool)
+    _require(plain(start) and plain(stop) and isinstance(dim, dict) and len(dim) == 1, "linspace other than between two numbers along one dim")
+    return np.linspace(np.float32(start), np.float32(stop), int(next(iter(dim.values()))), dtype=np.float32)
+
+
+def _exp(x):
+    """math.exp of a plain number or of a float32 / complex64 NumPy array (what math.linspace and arithmetic on it make): float32 or
+    complex64, as PhiML's NumPy backend computes it in precision 32."""
+    if isinstance(x, numbers.Number) and not isinstance(x, bool):
+        x = np.complex64(x) if isinstance(x, complex) else np.float32(x)
+    x = np.asarray(x)
+    _require(x.dtype in (np.float32, np.complex64), f"math.exp of {x.dtype} values")
+    return np.exp(x)
+
+
+PI = np.pi
 math = SimpleNamespace(Solve=Solve, SolveTape=SolveTape, NotConverged=NotConverged, Diverged=Diverged,
-                       ConvergenceException=ConvergenceException, extrapolation=extrapolation, sin=_sin, PI=np.pi, rotate_vector=rotate_vector,
+                       ConvergenceException=ConvergenceException, extrapolation=extrapolation, sin=_sin, exp=_exp, linspace=_linspace, PI=PI,
+                       rotate_vector=rotate_vector,
                        set_global_precision=set_global_precision, get_precision=get_precision, precision=precision)
 
 
@@ -414,9 +436,10 @@ def _domain(res, dx, batch, vspec, dtype):
 
 
 def _grid_dtype(data):
-    """dtype of a new grid: that of the data it wraps, else the global precision's."""
+    """dtype of a new grid's domain: that of the float data it wraps (int32 counts share the float32 layout), else the global
+    precision's."""
     if data is not None:
-        return (data[0] if isinstance(data, (list, tuple)) else data).dtype
+        return torch.float64 if (data[0] if isinstance(data, (list, tuple)) else data).dtype == torch.float64 else torch.float32
     return torch.float64 if _PRECISION[0] == 64 else torch.float32
 
 
@@ -439,8 +462,16 @@ class _Grid:
         return self.res == other.res and self.lower == other.lower and self.upper == other.upper and self.batch == other.batch
 
     @property
-    def precision(self) -> int:
-        return 64 if self.dom.dtype == torch.float64 else 32
+    def dtype(self) -> torch.dtype:
+        data = self.__dict__.get('data')                 # not yet set while a geometry's mask is being sampled: the domain's
+        if data is None:
+            return self.dom.dtype
+        return (data[0] if isinstance(data, (list, tuple)) else data).dtype
+
+    @property
+    def precision(self):
+        """32 or 64 for float32 / float64 values; None for an int32 grid (julia_set's counts), which no operator takes."""
+        return {torch.float32: 32, torch.float64: 64}.get(self.dtype)
 
 
 class CenteredGrid(_Grid):
@@ -495,6 +526,7 @@ class CenteredGrid(_Grid):
         return self.data[idx]
 
     def __add__(self, other):
+        _require_float("arithmetic", self)
         if isinstance(other, CenteredGrid):
             assert self._same_grid(other)
             _same_precision(self, other)
@@ -507,6 +539,7 @@ class CenteredGrid(_Grid):
         return self + (other * -1.0)
 
     def __mul__(self, other):
+        _require_float("arithmetic", self)
         if isinstance(other, (tuple, list)):             # scalar field times a constant vector, e.g. s * (0, 0.1)
             g = self.with_values(self.data)
             g.vector_scale = tuple(float(o) for o in other)
@@ -527,6 +560,7 @@ class CenteredGrid(_Grid):
 
     def __pow__(self, power):
         _require(isinstance(power, numbers.Real) and not isinstance(power, bool), "a power other than a plain number")
+        _require_float("arithmetic", self)
         return self.with_values(self.data ** float(power))
 
     def laplace(self, order=2):
@@ -641,12 +675,20 @@ def _require(cond, what):
 
 def _same_precision(*fields):
     """Fields of one operation share their precision: nothing is converted silently."""
+    _require_float("an operation", *fields)
     bits = {f.precision for f in fields if isinstance(f, _Grid)}
     _require(len(bits) <= 1, "mixing float32 and float64 fields in one operation")
 
 
 def _require_f32(what, *fields):
+    _require_float(what, *fields)
     _require(all(f.precision == 32 for f in fields if isinstance(f, _Grid)), f"{what} in precision 64 (fp32 only)")
+
+
+def _require_float(what, *fields):
+    """Operators take float32 or float64 grids; an int32 grid (julia_set's counts) is refused instead of being read as float32."""
+    bad = sorted({str(f.dtype) for f in fields if isinstance(f, _Grid) and f.precision is None})
+    _require(not bad, f"{what} of {', '.join(bad)} grids")
 
 
 def divergence(v: StaggeredGrid, order=2) -> CenteredGrid:
@@ -664,6 +706,7 @@ def _gradient_boundary(b: Extrapolation) -> Extrapolation:
 def laplace(u: CenteredGrid, order=2) -> CenteredGrid:
     """field.laplace (phi/field/_field_math.py:46-145), ghost cells from u's boundary."""
     _require(isinstance(u, CenteredGrid) and order == 2, "laplace of non-centred / higher-order fields")
+    _require_float("laplace", u)
     out = ops.laplace(u.dom, u.spec, u.data)
     return CenteredGrid(boundary=_gradient_boundary(_gradient_boundary(u.boundary)), bounds=u.bounds, batch=u.batch, _data=out, **dict(zip(u.axes, u.res)))
 
@@ -680,6 +723,7 @@ def spatial_gradient(p: CenteredGrid, boundary=None, at='face', order=2) -> Stag
     make_incompressible uses, fluid.py:158)."""
     boundary = _as_ext(boundary)
     _require(at == 'face' and order == 2, "spatial_gradient other than at='face', order 2")
+    _require_float("spatial_gradient", p)
     _require(_pressure_boundary(boundary) == p.boundary, "spatial_gradient with an unrelated field boundary")
     with precision(p.precision):
         g = StaggeredGrid(0, boundary, p.bounds, p.batch, **dict(zip(p.axes, p.res)))
@@ -836,6 +880,7 @@ def explicit(fld, diffusivity: float, dt: float, substeps: int = 1):
     """diffuse.explicit (phi/physics/diffuse.py:13-60): substeps of  u += (dt/substeps) * diffusivity * laplace(u); for a
     StaggeredGrid every component is diffused with its own boundary (Lid_Driven_Cavity.ipynb, Variable_Boundaries.ipynb)."""
     amount = float(diffusivity) * float(dt) / substeps
+    _require_float("diffuse.explicit", fld)
     if isinstance(fld, StaggeredGrid):
         return fld.with_values(ops.laplace_axpy_faces(fld.dom, fld.vspec, fld.data, amount, substeps))
     _require(isinstance(fld, CenteredGrid), "explicit diffusion of this field type")
@@ -975,6 +1020,25 @@ def wave_step(h_c: CenteredGrid, h_p: CenteredGrid, time, dt: float, k_speed: fl
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# Julia sets  (examples/grids/Julia_Set.ipynb)
+# ----------------------------------------------------------------------------------------------------------------------
+def julia_set(c, iter_count: int, bounds: Box = None, **resolution) -> CenteredGrid:
+    """The Julia_Set notebook's sampled grid in one kernel launch:
+        CenteredGrid(lambda x, y: iterate(julia_map, iter_count, x + y * 1j, 0, c=c)[1], x=..., y=..., bounds=bounds)
+        julia_map(z, counter, c) = z ** 2 + c, counter + (abs(z) < 2)
+    with PhiML's complex64 rounding.  c: one complex constant or a 1-D array of them (the notebook's
+    0.7885 * math.exp(1j * math.linspace(0, 2 * PI, batch(time=100)))), one batch entry each.  Returns an int32 CenteredGrid of batch
+    len(c) whose .numpy() is (batch, x, y) (batch 1: (x, y)); the axes x and y stand for the real and imaginary parts."""
+    cc = np.atleast_1d(np.asarray(c))
+    _require(cc.ndim == 1 and cc.size >= 1 and np.issubdtype(cc.dtype, np.number), "Julia constants other than a 1-D array of numbers")
+    _require(tuple(resolution) == ('x', 'y'), f"a Julia set on axes {tuple(resolution)} (2-D x, y)")
+    _require(isinstance(iter_count, int) and not isinstance(iter_count, bool) and iter_count >= 0, f"iter_count = {iter_count!r}")
+    out = CenteredGrid(bounds=bounds, batch=cc.size, _data=torch.empty(0, dtype=torch.int32), **resolution)
+    out.data = ops.julia(out.dom, np.concatenate(out.axis_centres()), cc.astype(np.complex64), iter_count)
+    return out
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # fluid  (phi/physics/fluid.py)
 # ----------------------------------------------------------------------------------------------------------------------
 def _cg_params(v: StaggeredGrid, solve: Solve):
@@ -1096,7 +1160,7 @@ def incompressible_step(v: StaggeredGrid, s: CenteredGrid, p, dt: float, inflow:
     Returns new (v, s, p); inputs are not modified."""
     solve = solve or Solve('CG', 1e-3)
     _check_velocity(s, v)
-    _require_f32("incompressible_step", v, s, p)
+    _require_f32("incompressible_step", v, s, p, inflow)
     kw = {}
     if obstacles:
         kw['accessible'], kw['factors'] = _obstacle_masks_cached(v, obstacles)
