@@ -119,6 +119,7 @@ int         phicuda_device_info(char* name, size_t name_len, int* sm_count, int*
 #define PHI_KERNEL_RD_RING       6   /* k_rd_ring       (persistent, TMA ring): phicuda_reaction_diffusion_f32 */
 #define PHI_KERNEL_WAVE_RING     7   /* k_wave_ring     (persistent, TMA ring): phicuda_wave_f32 */
 #define PHI_KERNEL_JULIA         8   /* k_julia         (one thread per batch entry and cell): phicuda_julia_f32 */
+#define PHI_KERNEL_POINTS        9   /* k_advect_points (one thread per batch entry and point): phicuda_advect_points_f32 */
 typedef struct PhiLaunchInfo {
     int32_t kernel;        /* PHI_KERNEL_* */
     int32_t generic;       /* 1: variant with per-tile boundary handling, 0: branch-free variant (every tile qualifies) */
@@ -377,6 +378,26 @@ int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, 
 size_t phicuda_julia_scratch_bytes(const PhiGrid* g);
 int phicuda_julia_f32(const PhiGrid* g, const float* centers, const float* c, int32_t iterations, int32_t* counts, void* scratch,
                       size_t scratch_bytes, void* stream);
+
+/* ---- N11  advect.points: points moved through a StaggeredGrid velocity (Euler, RK4) -----------------------------------------------
+ * advect.points(points, velocity, dt, integrator) (phi/physics/advect.py:20-35, 136-153) applied `steps` times, every step in one
+ * launch (PHI_KERNEL_POINTS).  One velocity sample at p: for every component c, idx_a = ((p_a - lower[c][a]) / size[c][a]) * res[c][a]
+ * - 0.5, then math.grid_sample of component c at idx with its own boundary (vbc->comp[c], per-component constants included).
+ *   Euler: p + v0 dt.   RK4: vh = v(p + (dt/2) v0), vh2 = v(p + (dt/2) vh), v1 = v(p + dt vh2), p + dt ((1/6) ((v0 + 2 (vh + vh2)) + v1)).
+ * Every operation is rounded as PhiML's NumPy backend rounds float32 (DESIGN.md row N11): the results equal PhiML's bit for bit.
+ * `map`: the component grids' bounds and resolution [component][axis] in float32, as UniformGrid.stagger computes them
+ * (phi/geom/_grid.py:204-209): size = upper' - lower', res[c][a] = the number of faces of component c stored along axis a.
+ * `points`, `out`: device arrays (batch, npoints, dim), batch = points_batch for `points` and B = max(points_batch, g->batch) for `out`;
+ * points_batch is 1 or g->batch, or g->batch is 1 (the batch broadcasts as in PhiML).  `out` may be `points` when points_batch == B.
+ * `trajectory`: NULL or (steps + 1, B, npoints, dim), entry 0 = the input positions.  Any point is taken, NaN and +-inf included.
+ * One GPU (z-slabs return PHI_ERR_UNSUPPORTED).  npoints == 0 returns 0 without a CUDA call; every argument check runs before the
+ * first CUDA call, and a refused call leaves out and trajectory untouched. */
+#define PHI_INTEGRATOR_EULER 0
+#define PHI_INTEGRATOR_RK4   1
+typedef struct PhiPointMap { float lower[3][3], size[3][3], res[3][3]; } PhiPointMap;   /* [component][axis] */
+int phicuda_advect_points_f32(const PhiGrid* g, const PhiVBC* vbc, const float* const vel[3], const PhiPointMap* map,
+                              const float* points, int64_t npoints, int32_t points_batch, float dt, int32_t integrator,
+                              int32_t steps, float* out, float* trajectory, void* stream);
 
 /* ---- N9  fp64: the Taylor-Green step of math.set_global_precision(64) -----------------------------------------------------
  * The same operations as their _f32 counterparts on float64 arrays (same layout, element size 8; x-rows stay padded to multiples of

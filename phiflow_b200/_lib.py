@@ -43,7 +43,8 @@ class PhiLaunchInfo(C.Structure):
                                          'total_units', 'grid_ctas', 'split')]
 
 
-KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING, KERNEL_RD_RING, KERNEL_WAVE_RING, KERNEL_JULIA = range(9)
+KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING, KERNEL_RD_RING, KERNEL_WAVE_RING, KERNEL_JULIA, KERNEL_POINTS = range(10)
+INTEGRATOR_EULER, INTEGRATOR_RK4 = 0, 1
 
 
 class PhiWaveDisc(C.Structure):
@@ -53,6 +54,10 @@ class PhiWaveDisc(C.Structure):
 class PhiPlumeParams(C.Structure):
     _fields_ = [('dt', C.c_float), ('inflow_rate', C.c_float), ('buoyancy', C.c_float * 3), ('mac_cormack', C.c_int32), ('static_scalar', C.c_int32),
                 ('cg_start_event', C.c_void_p), ('cg_stop_event', C.c_void_p)]
+
+
+class PhiPointMap(C.Structure):
+    _fields_ = [('lower', (C.c_float * 3) * 3), ('size', (C.c_float * 3) * 3), ('res', (C.c_float * 3) * 3)]     # [component][axis]
 
 
 class PhiValues64(C.Structure):
@@ -134,6 +139,8 @@ PROTOTYPES = {
                                    C.c_float, _P(C.c_float), C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
     'phicuda_julia_scratch_bytes': (C.c_size_t, [_P(PhiGrid)]),
     'phicuda_julia_f32': (C.c_int, [_P(PhiGrid), _P(C.c_float), _P(C.c_float), C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'phicuda_advect_points_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), F3, _P(PhiPointMap), C.c_void_p, C.c_int64, C.c_int32, C.c_float,
+                                            C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     'phicuda_laplace_f64': (C.c_int, [_P(PhiGrid), _P(PhiBC), _P(PhiValues64), C.c_void_p, C.c_void_p, C.c_void_p]),
     'phicuda_laplace_axpy_f64': (C.c_int, [_P(PhiGrid), _P(PhiBC), _P(PhiValues64), C.c_void_p, C.c_double, C.c_void_p, C.c_void_p]),
     'phicuda_divergence_f64': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiValues64), F3, C.c_void_p, C.c_void_p]),

@@ -363,6 +363,54 @@ def grid_sample(dom: Domain, bc, grid: torch.Tensor, coords: torch.Tensor, out: 
     return out
 
 
+INTEGRATORS = {'euler': _lib.INTEGRATOR_EULER, 'rk4': _lib.INTEGRATOR_RK4}
+
+
+def point_map(lower, upper, res, vbc) -> _lib.PhiPointMap:
+    """The bounds and resolution of every component grid of a staggered field on Box(lower, upper) at resolution `res`, in float32
+    as UniformGrid.stagger computes them (phi/geom/_grid.py:204-209): unit = size / res along c only, lower' = lower + unit * (-0.5
+    where the lower face is stored, else 0.5), upper' = upper + unit * (0.5 where the upper face is stored, else -0.5), res'_c =
+    n_c + lo + hi - 1; size' = upper' - lower' (Box.size, what Box.global_to_local divides by)."""
+    f32 = np.float32
+    d = len(res)
+    m = _lib.PhiPointMap()
+    for c in range(d):
+        lo_st, hi_st = stored_faces(vbc, c)
+        lo = [f32(v) for v in lower]
+        up = [f32(v) for v in upper]
+        unit = f32(f32(up[c] - lo[c]) / f32(res[c]))
+        lo[c] = f32(lo[c] + f32(unit * f32(-0.5 if lo_st else 0.5)))
+        up[c] = f32(up[c] + f32(unit * f32(0.5 if hi_st else -0.5)))
+        for a in range(d):
+            m.lower[c][a] = lo[a]
+            m.size[c][a] = f32(up[a] - lo[a])
+            m.res[c][a] = res[a] + (int(lo_st) + int(hi_st) - 1 if a == c else 0)
+    return m
+
+
+def advect_points(dom: Domain, vbc, vel, lower, upper, points: torch.Tensor, dt: float, integrator: str = 'euler', steps: int = 1,
+                  out: torch.Tensor = None, trajectory: bool = False):
+    """advect.points (phi/physics/advect.py:136-153) through the staggered velocity `vel` on Box(lower, upper), `steps` times in one
+    launch (include/phicuda.h, N11).  points: float32 CUDA tensor (batch, npoints, dim) of world positions, batch 1 or dom.batch (or
+    dom.batch == 1); integrator: 'euler' or 'rk4'.  Returns out (B, npoints, dim), B = max(batch, dom.batch) - `out` may be `points`
+    when batch == B - and, with trajectory=True, also the positions of every step (steps + 1, B, npoints, dim), entry 0 the input."""
+    require_cuda()
+    _f32_only("advect_points", dom, *vel, points, out)
+    if integrator not in INTEGRATORS:
+        raise _lib.Unsupported(_lib.ERR_UNSUPPORTED, f"advect_points: integrator {integrator!r} (euler and rk4 are supported)")
+    assert points.is_cuda and points.is_contiguous() and points.dim() == 3 and points.shape[-1] == dom.dim, \
+        f"points: {tuple(points.shape)} is not a contiguous CUDA array (batch, npoints, {dom.dim})"
+    B, n = max(points.shape[0], dom.batch), points.shape[1]
+    out = torch.empty((B, n, dom.dim), dtype=torch.float32, device=points.device) if out is None else out
+    assert out.is_contiguous() and tuple(out.shape) == (B, n, dom.dim), f"out: {tuple(out.shape)} is not ({B}, {n}, {dom.dim})"
+    traj = torch.empty((steps + 1, B, n, dom.dim), dtype=torch.float32, device=points.device) if trajectory and steps >= 1 else None
+    _lib.check(_lib.load().phicuda_advect_points_f32(C.byref(dom.grid), C.byref(make_vbc(vbc, dom.dim)), _f3(vel, dom.foff),
+                                                     C.byref(point_map(lower, upper, dom.res, vbc)), _ptr(points), C.c_int64(n),
+                                                     C.c_int32(points.shape[0]), C.c_float(dt), C.c_int32(INTEGRATORS[integrator]),
+                                                     C.c_int32(steps), _ptr(out), _ptr(traj), _stream()))
+    return (out, traj) if trajectory else out
+
+
 def mac_cormack_centered(dom: Domain, vbc, vel, fbc, src, dt: float, correction_strength=1.0, out=None):
     """advect.mac_cormack of a centred field (phi/physics/advect.py:182-215)."""
     require_cuda()

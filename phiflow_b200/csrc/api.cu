@@ -1,4 +1,5 @@
 // C ABI of libphicuda.so (declared in include/phicuda.h): argument validation, descriptor construction, launch order.
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -857,6 +858,57 @@ int phicuda_julia_f32(const PhiGrid* g, const float* centers, const float* c, in
     if (ce != cudaSuccess) return cuda_fail((int)ce, "julia");
     const float* xc = dtab + 2 * (size_t)g->batch;
     return cuda_fail(phi_launch_julia(dg, dtab, xc, xc + g->n[0], iterations, counts, (cudaStream_t)stream), "julia");
+}
+
+int phicuda_advect_points_f32(const PhiGrid* g, const PhiVBC* vbc, const float* const vel[3], const PhiPointMap* map,
+                              const float* points, int64_t npoints, int32_t points_batch, float dt, int32_t integrator,
+                              int32_t steps, float* out, float* trajectory, void* stream)
+{
+    // every check runs before the first CUDA call: a refused call leaves out and trajectory untouched
+    DGrid dg; DVec dv;
+    CHECK(phi_make_dgrid(g, &dg));
+    if (g->halo != 0) { phi_set_error("advect_points: z-slab grids are not supported"); return PHI_ERR_UNSUPPORTED; }
+    CHECK(make_vec(g, vbc, vel, &dv));
+    if (!map || !points || !out) { phi_set_error("advect_points: NULL argument"); return PHI_ERR_INVALID; }
+    if (npoints < 0) { phi_set_error("advect_points: npoints must be >= 0, got %lld", (long long)npoints); return PHI_ERR_INVALID; }
+    if (steps < 1) { phi_set_error("advect_points: steps must be >= 1, got %d", steps); return PHI_ERR_INVALID; }
+    if (integrator != PHI_INTEGRATOR_EULER && integrator != PHI_INTEGRATOR_RK4) { phi_set_error("advect_points: unknown integrator %d", integrator); return PHI_ERR_INVALID; }
+    if (points_batch < 1 || (points_batch != 1 && g->batch != 1 && points_batch != g->batch)) {
+        phi_set_error("advect_points: points batch %d does not broadcast against grid batch %d", points_batch, g->batch); return PHI_ERR_INVALID;
+    }
+    for (int c = 0; c < g->dim; ++c) {
+        const DField& f = dv.f[c];
+        if ((long long)f.sb > INT_MAX) { phi_set_error("advect_points: component %d holds more than 2^31 elements per batch entry", c); return PHI_ERR_UNSUPPORTED; }
+        for (int a = 0; a < g->dim; ++a) {
+            const float lo = map->lower[c][a], sz = map->size[c][a], r = map->res[c][a];
+            if (r != (float)(f.hi[a] - f.lo[a] + 1)) {
+                phi_set_error("advect_points: map res[%d][%d] = %g but component %d stores %d values along axis %d", c, a, r, c, f.hi[a] - f.lo[a] + 1, a);
+                return PHI_ERR_INVALID;
+            }
+            if (!(std::isfinite(sz) && sz > 0.f) || !std::isfinite(lo)) {
+                phi_set_error("advect_points: map lower[%d][%d] = %g, size = %g (finite, size > 0 required)", c, a, lo, sz); return PHI_ERR_INVALID;
+            }
+        }
+    }
+    const long long B = g->batch > points_batch ? g->batch : points_batch;
+    if ((unsigned __int128)npoints * (unsigned)B * (unsigned)(steps + 1) * (unsigned)g->dim * sizeof(float) > (unsigned __int128)INT64_MAX) {
+        phi_set_error("advect_points: %lld points x %lld batch x %d steps exceeds 64-bit offsets", (long long)npoints, B, steps); return PHI_ERR_INVALID;
+    }
+    const size_t in_bytes = (size_t)npoints * points_batch * g->dim * sizeof(float), out_bytes = (size_t)npoints * B * g->dim * sizeof(float);
+    const size_t traj_bytes = out_bytes * ((size_t)steps + 1);
+    if (out != points && overlap(out, out_bytes, points, in_bytes)) { phi_set_error("advect_points: out overlaps points without being points"); return PHI_ERR_INVALID; }
+    if (out == points && points_batch != B) { phi_set_error("advect_points: out may be points only when points are not broadcast (batch %d < %lld)", points_batch, B); return PHI_ERR_INVALID; }
+    if (trajectory && (overlap(trajectory, traj_bytes, points, in_bytes) || overlap(trajectory, traj_bytes, out, out_bytes))) {
+        phi_set_error("advect_points: trajectory overlaps points or out"); return PHI_ERR_INVALID;
+    }
+    const size_t fbytes = face_elems(g) * sizeof(float);
+    for (int c = 0; c < g->dim; ++c)
+        if (overlap(out, out_bytes, vel[c], fbytes) || (trajectory && overlap(trajectory, traj_bytes, vel[c], fbytes))) {
+            phi_set_error("advect_points: out or trajectory overlaps velocity component %d", c); return PHI_ERR_INVALID;
+        }
+    if (npoints == 0) return 0;
+    return cuda_fail(phi_launch_advect_points(dg, dv, *map, points, (long long)npoints, points_batch, dt, integrator, steps, out,
+                                              trajectory, (cudaStream_t)stream), "advect_points");
 }
 
 }  // extern "C"

@@ -130,3 +130,7 @@ int phi_launch_wave(const DGrid& g, const DField& f, float* hc, float* hp, float
 // N10 the Julia_Set notebook's escape counts (julia_kernels.cu), 2-D: c = batch interleaved (re, im) pairs, xc / yc = n[0] / n[1] cell
 // centres, all in device memory; counts: int32 in the centred-array layout, every owned cell written (0 for iterations == 0)
 int phi_launch_julia(const DGrid& g, const float* c, const float* xc, const float* yc, int iterations, int32_t* counts, cudaStream_t s);
+// N11 advect.points (points_kernels.cu): `steps` Euler / RK4 steps of (max(batch, points_batch), npoints) points, out and the optional
+// trajectory (steps + 1 entries) written; points_batch / g.batch of 1 broadcast
+int phi_launch_advect_points(const DGrid& g, const DVec& vel, const PhiPointMap& map, const float* points, long long npoints,
+                             int points_batch, float dt, int integrator, int steps, float* out, float* traj, cudaStream_t s);

@@ -5,9 +5,10 @@
 Mirrored (same names, argument meaning and error behaviour; reference file:line in each docstring):
     Box, Sphere, union, geom.infinite_cylinder, CenteredGrid, StaggeredGrid, extrapolation (ZERO, ONE, PERIODIC, ZERO_GRADIENT, BOUNDARY, combine_sides),
     Solve, SolveTape, NotConverged, Diverged, math.{sin, exp, linspace, PI, rotate_vector}, PI, field.{divergence, laplace, spatial_gradient, where}, resample,
-    advect.{semi_lagrangian, mac_cormack, advect}, diffuse.{explicit, implicit}, fluid.{make_incompressible, incompressible_step},
+    advect.{semi_lagrangian, mac_cormack, advect, points, euler, rk4}, geom.Point, spatial, diffuse.{explicit, implicit}, fluid.{make_incompressible, incompressible_step},
     write / read (field.write / field.read: the reference's .npz field files, see field_io.py).
 Fused notebook steps (one kernel launch for all substeps of a call): reaction_diffusion (Reaction_Diffusion), wave_step (Waves).
+Streamlines: streamlines(x0, v, step_size, iterations) returns every position of an advect.points trajectory from one kernel launch.
 Julia_Set: julia_set(c, iter_count, bounds, x=..., y=...) returns the escape counts as an int32 CenteredGrid in one kernel launch; an
 int32 grid is a result only, which every operator refuses.
 Precision: math.set_global_precision(64) / math.precision(64) make new grids float64 (the Taylor-Green notebook); laplace,
@@ -31,7 +32,7 @@ from . import scene as _scene
 
 __all__ = ['Scene', 'vec', 'batch', 'iterate', 'jit_compile', 'Box', 'Sphere', 'union', 'geom', 'CenteredGrid', 'StaggeredGrid', 'extrapolation', 'ZERO', 'ONE', 'PERIODIC', 'ZERO_GRADIENT',
            'BOUNDARY', 'combine_sides', 'Solve', 'SolveTape', 'NotConverged', 'Diverged', 'ConvergenceException', 'field',
-           'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read', 'wave_step', 'julia_set', 'PI']
+           'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read', 'wave_step', 'julia_set', 'PI', 'spatial', 'streamlines']
 
 AXES = 'xyz'
 
@@ -238,7 +239,15 @@ def union(*geometries):
     return Union(*flat)
 
 
-geom = SimpleNamespace(Box=Box, Sphere=Sphere, union=union, infinite_cylinder=infinite_cylinder)
+class Point:
+    """geom.Point(center) (phi/geom/_geom.py): zero-volume points at `center`, a vec, a float32 NumPy array or a float32 CUDA tensor
+    (..., dim) of world positions - what advect.points moves."""
+
+    def __init__(self, center):
+        self.center = center
+
+
+geom = SimpleNamespace(Box=Box, Sphere=Sphere, union=union, infinite_cylinder=infinite_cylinder, Point=Point)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -390,6 +399,11 @@ def batch(**dims):
     """batch(time=300) as `iterate` uses it: the name and length of the trajectory dimension."""
     assert len(dims) == 1, "one trajectory dimension"
     return dict(dims)
+
+
+def spatial(**dims):
+    """spatial(iter=50) as `iterate` uses it (the Streamlines notebook): the name and length of the trajectory dimension, as `batch`."""
+    return batch(**dims)
 
 
 def iterate(f, iterations, *x0, f_kwargs: dict = None, range=range, substeps: int = 1, **f_kwargs_):
@@ -870,7 +884,98 @@ def mac_cormack(fld, velocity: StaggeredGrid, dt: float, correction_strength=1.0
     return fld.with_values(ops.mac_cormack_centered(velocity.dom, velocity.vspec, velocity.data, fld.spec, fld.data, float(dt), correction_strength))
 
 
-advect = SimpleNamespace(semi_lagrangian=semi_lagrangian, mac_cormack=mac_cormack, advect=semi_lagrangian)
+def euler(data, velocity, dt: float, v0=None):
+    """advect.euler (phi/physics/advect.py:20-24) on points: the positions after one Euler step (what advect.points computes with it)."""
+    _require(v0 is None, "integrators with a given v0")
+    return points(data, velocity, dt, integrator=euler)
+
+
+def rk4(data, velocity, dt: float, v0=None):
+    """advect.rk4 (phi/physics/advect.py:27-35) on points: the positions after one Runge-Kutta-4 step."""
+    _require(v0 is None, "integrators with a given v0")
+    return points(data, velocity, dt, integrator=rk4)
+
+
+def finite_rk4(data, velocity, dt: float, v0=None):
+    """advect.finite_rk4 (phi/physics/advect.py:38-50): not on the fast path."""
+    _require(False, "advect.finite_rk4")
+
+
+_INTEGRATOR_NAMES = {euler: 'euler', rk4: 'rk4'}
+
+
+def _as_points(x, dim):
+    """(kind, float32 tensor (N, dim), shape of x) of a Point centre, vec, float32 NumPy array or float32 CUDA tensor.  A vec comes
+    back as a float32 NumPy vector, the kind `iterate` carries as ONE state variable (a tuple would be several)."""
+    if isinstance(x, torch.Tensor):
+        _require(x.dtype == torch.float32 and x.is_cuda, f"points as a {x.dtype} tensor on {x.device} (float32 CUDA tensors)")
+        kind, t = 'tensor', x
+    elif isinstance(x, tuple) and all(isinstance(v, numbers.Real) and not isinstance(v, bool) for v in x):
+        kind, t = 'vec', torch.tensor(np.array(x, np.float32))
+    else:
+        _require(isinstance(x, np.ndarray) and x.dtype == np.float32, f"points of type {type(x).__name__} "
+                 f"{getattr(x, 'dtype', '')} (a vec, float32 NumPy arrays or float32 CUDA tensors)")
+        kind, t = 'numpy', torch.from_numpy(np.ascontiguousarray(x))
+    _require(t.dim() >= 1 and t.shape[-1] == dim, f"points of shape {tuple(t.shape)} in a {dim}-D velocity")
+    return kind, t, tuple(t.shape)
+
+
+def _from_points(kind, t, shape):
+    if kind == 'tensor':
+        return t.reshape(shape)
+    return t.cpu().numpy().reshape(shape)
+
+
+def _advect_points(x, velocity, dt, integrator, steps, trajectory):
+    """steps of advect.points in one launch; x: the points of any supported kind.  Returns (kind, result tensor, shape of x)."""
+    _require(isinstance(velocity, StaggeredGrid), "advect.points by a non-staggered velocity")
+    _require_f32("advect.points", velocity)
+    _require(integrator in _INTEGRATOR_NAMES, f"advect.points with integrator {getattr(integrator, '__name__', integrator)!r} (euler, rk4)")
+    kind, t, shape = _as_points(x, len(velocity.res))
+    d = len(velocity.res)
+    pts = t.reshape(1, -1, d).to(velocity.dom.device).contiguous()
+    if pts.data_ptr() == t.data_ptr():
+        pts = pts.clone()                                # the kernel writes its own output; the caller's points stay as they are
+    res = ops.advect_points(velocity.dom, velocity.vspec, velocity.data, velocity.lower, velocity.upper, pts, float(dt),
+                            _INTEGRATOR_NAMES[integrator], steps, out=None if trajectory or velocity.batch > 1 else pts,
+                            trajectory=trajectory)
+    return kind, (res[1] if trajectory else res), shape
+
+
+def points(points, velocity: StaggeredGrid, dt: float, integrator=euler):
+    """advect.points (phi/physics/advect.py:136-153): moves the points by `integrator` (advect.euler or advect.rk4) through the float32
+    StaggeredGrid `velocity`, in one kernel launch, bit for bit as PhiML computes it (DESIGN.md row N11).  points: a geom.Point, a
+    vec, a float32 NumPy array or a float32 CUDA tensor (..., dim); the result has the same kind and shape (a Point for a Point; a
+    float32 NumPy vector for a vec).
+    A velocity of batch B > 1 moves the same points in every batch entry; the result then gains a leading axis of length B."""
+    x = points.center if isinstance(points, Point) else points
+    kind, t, shape = _advect_points(x, velocity, dt, integrator, 1, False)
+    out = _from_points(kind, t, (t.shape[0],) + shape if t.shape[0] > 1 else shape)
+    return Point(out) if isinstance(points, Point) else out
+
+
+def streamlines(x0, velocity: StaggeredGrid, step_size: float, iterations: int, integrator=rk4):
+    """The Streamlines notebook's trajectory  iterate(lambda x: advect.points(geom.Point(x), v, step_size, integrator).center,
+    spatial(iter=iterations), x0)  from ONE kernel launch: the positions (iterations + 1, [B,] ..., dim), entry 0 = x0, as a NumPy array
+    (a CUDA tensor for a tensor x0), bit for bit the same as the iterate form."""
+    _require(isinstance(iterations, int) and not isinstance(iterations, bool) and iterations >= 1, f"iterations = {iterations!r}")
+    x = x0.center if isinstance(x0, Point) else x0
+    kind, t, shape = _advect_points(x, velocity, step_size, integrator, iterations, True)
+    shape = (iterations + 1,) + ((t.shape[1],) if t.shape[1] > 1 else ()) + shape
+    return t.reshape(shape) if kind == 'tensor' else t.cpu().numpy().reshape(shape)
+
+
+def _advect(fld, velocity, dt: float, integrator=euler):
+    """advect.advect (phi/physics/advect.py:53-74): points (a Point, vec, array or tensor) go to advect.points, grids to
+    semi_lagrangian (Euler only)."""
+    if isinstance(fld, (Point, np.ndarray, torch.Tensor, tuple)):
+        return points(fld, velocity, dt, integrator)
+    _require(integrator is euler or integrator is None, "grid advection with integrators other than euler")
+    return semi_lagrangian(fld, velocity, dt)
+
+
+advect = SimpleNamespace(semi_lagrangian=semi_lagrangian, mac_cormack=mac_cormack, advect=_advect, points=points, euler=euler, rk4=rk4,
+                         finite_rk4=finite_rk4)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
