@@ -120,6 +120,7 @@ int         phicuda_device_info(char* name, size_t name_len, int* sm_count, int*
 #define PHI_KERNEL_WAVE_RING     7   /* k_wave_ring     (persistent, TMA ring): phicuda_wave_f32 */
 #define PHI_KERNEL_JULIA         8   /* k_julia         (one thread per batch entry and cell): phicuda_julia_f32 */
 #define PHI_KERNEL_POINTS        9   /* k_advect_points (one thread per batch entry and point): phicuda_advect_points_f32 */
+#define PHI_KERNEL_SPH          10   /* k_sph           (persistent, cooperative; grid_ctas set): phicuda_sph_f32 */
 typedef struct PhiLaunchInfo {
     int32_t kernel;        /* PHI_KERNEL_* */
     int32_t generic;       /* 1: variant with per-tile boundary handling, 0: branch-free variant (every tile qualifies) */
@@ -378,6 +379,38 @@ int phicuda_wave_f32(const PhiGrid* g, const PhiBC* bc, float* h_c, float* h_p, 
 size_t phicuda_julia_scratch_bytes(const PhiGrid* g);
 int phicuda_julia_f32(const PhiGrid* g, const float* centers, const float* c, int32_t iterations, int32_t* counts, void* scratch,
                       size_t scratch_bytes, void* stream);
+
+/* ---- N12  SPH: the SPH notebook's dam break (examples/particles/SPH.ipynb, phi/physics/sph.py) ------------------------------------
+ * `substeps` times apply_bounds(sph_step(v)) of the notebook, all in one cooperative launch (PHI_KERNEL_SPH), for n particles in `dim`
+ * = 2 or 3 dimensions with the poly6 kernel.  One substep, per particle i, over the pairs j with sqrt(r2) < support (self included),
+ * delta = x_j - x_i, r2 = sum(delta^2):
+ *   rho_i = (sum_j kernel_norm (support^2 - r2)^3) mass,  p_i = isotropic_exp (rho_i - base_density)
+ *   d = sqrt(max(r2, 1e-5)), gap = smoothing_length - d
+ *   F_i = sum_j pressure_norm ((-delta / d) (p_i + p_j) / (2 rho_j)) gap^2 + viscous_norm ((v_j - v_i) / rho_j) gap
+ *   v' = v + (F_i / rho_i + gravity) dt,  x' = x + dt v';  every component of x' outside [lower, upper] is clipped and its v' scaled
+ *   by damping.
+ * Neighbours are found on PhiML's hash grid: res = max(1, ceil(max(upper - lower, support) / support)) cells per axis of edge
+ * (support res) / res, cell = trunc((x - lower) / edge) clamped into [0, res - 1] (the reference only clamps above; a particle
+ * more than a cell below `lower`, or with a NaN or infinite coordinate, lands in the first or last cell here instead of indexing out
+ * of range).  Sums run over the 3^dim neighbour cells in PhiML's offset order (x outermost), each cell's particles by ascending
+ * index, with one float32 rounding per operation: the result is independent of the launch and equals tests/oracle_sph.py bit for bit.
+ * x, v: device arrays (n, dim); x_out, v_out: (n, dim), rho_out: NULL or (n,), the density of the last substep.  Outputs must not
+ * overlap each other, the inputs or the scratch.  scratch: device memory of phicuda_sph_scratch_bytes (0 for invalid parameters).
+ * n == 0 returns 0 without a CUDA call; every argument check runs before the first CUDA call, and a refused call leaves the outputs
+ * untouched. */
+typedef struct PhiSphParams {
+    float lower[3], upper[3];      /* domain corners (the first `dim` entries) */
+    float support;                 /* s: the neighbour cutoff and minimum hash cell edge */
+    float smoothing_length;        /* h: the gap h - d */
+    float kernel_norm;             /* poly6 normalisation: (315 / 64 / pi) / s^9 in 3-D, (4 / pi) / s^8 in 2-D, rounded by the caller */
+    float mass, pressure_norm, viscous_norm;
+    float isotropic_exp, base_density;
+    float dt, damping;
+    float gravity[3];
+} PhiSphParams;
+size_t phicuda_sph_scratch_bytes(int64_t n, int32_t dim, const PhiSphParams* prm);
+int phicuda_sph_f32(const float* x, const float* v, int64_t n, int32_t dim, const PhiSphParams* prm, int32_t substeps, float* x_out,
+                    float* v_out, float* rho_out, void* scratch, size_t scratch_bytes, void* stream);
 
 /* ---- N11  advect.points: points moved through a StaggeredGrid velocity (Euler, RK4) -----------------------------------------------
  * advect.points(points, velocity, dt, integrator) (phi/physics/advect.py:20-35, 136-153) applied `steps` times, every step in one

@@ -43,7 +43,7 @@ class PhiLaunchInfo(C.Structure):
                                          'total_units', 'grid_ctas', 'split')]
 
 
-KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING, KERNEL_RD_RING, KERNEL_WAVE_RING, KERNEL_JULIA, KERNEL_POINTS = range(10)
+KERNEL_NONE, KERNEL_LAPLACE_RING, KERNEL_LAPLACE_MARCH, KERNEL_CG_RING, KERNEL_CG_MARCH, KERNEL_STENCIL_RING, KERNEL_RD_RING, KERNEL_WAVE_RING, KERNEL_JULIA, KERNEL_POINTS, KERNEL_SPH = range(11)
 INTEGRATOR_EULER, INTEGRATOR_RK4 = 0, 1
 
 
@@ -58,6 +58,13 @@ class PhiPlumeParams(C.Structure):
 
 class PhiPointMap(C.Structure):
     _fields_ = [('lower', (C.c_float * 3) * 3), ('size', (C.c_float * 3) * 3), ('res', (C.c_float * 3) * 3)]     # [component][axis]
+
+
+class PhiSphParams(C.Structure):
+    _fields_ = [('lower', C.c_float * 3), ('upper', C.c_float * 3), ('support', C.c_float), ('smoothing_length', C.c_float),
+                ('kernel_norm', C.c_float), ('mass', C.c_float), ('pressure_norm', C.c_float), ('viscous_norm', C.c_float),
+                ('isotropic_exp', C.c_float), ('base_density', C.c_float), ('dt', C.c_float), ('damping', C.c_float),
+                ('gravity', C.c_float * 3)]
 
 
 class PhiValues64(C.Structure):
@@ -141,6 +148,9 @@ PROTOTYPES = {
     'phicuda_julia_f32': (C.c_int, [_P(PhiGrid), _P(C.c_float), _P(C.c_float), C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     'phicuda_advect_points_f32': (C.c_int, [_P(PhiGrid), _P(PhiVBC), F3, _P(PhiPointMap), C.c_void_p, C.c_int64, C.c_int32, C.c_float,
                                             C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'phicuda_sph_scratch_bytes': (C.c_size_t, [C.c_int64, C.c_int32, _P(PhiSphParams)]),
+    'phicuda_sph_f32': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, _P(PhiSphParams), C.c_int32, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     'phicuda_laplace_f64': (C.c_int, [_P(PhiGrid), _P(PhiBC), _P(PhiValues64), C.c_void_p, C.c_void_p, C.c_void_p]),
     'phicuda_laplace_axpy_f64': (C.c_int, [_P(PhiGrid), _P(PhiBC), _P(PhiValues64), C.c_void_p, C.c_double, C.c_void_p, C.c_void_p]),
     'phicuda_divergence_f64': (C.c_int, [_P(PhiGrid), _P(PhiVBC), _P(PhiValues64), F3, C.c_void_p, C.c_void_p]),

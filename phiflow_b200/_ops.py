@@ -411,6 +411,55 @@ def advect_points(dom: Domain, vbc, vel, lower, upper, points: torch.Tensor, dt:
     return (out, traj) if trajectory else out
 
 
+def sph_params(lower, upper, smoothing_length: float, particle_mass: float, dt: float, gravity, dynamic_visc: float = 0.025,
+               isotropic_exp: float = 20., base_density: float = 1., damping_coef: float = -0.95) -> _lib.PhiSphParams:
+    """The SPH notebook's constants (examples/particles/SPH.ipynb) in float32 as its PhiML tensors round them (include/phicuda.h, N12):
+    Sphere(volume=h ** d) keeps radius_from_volume(volume) and reports volume_from_radius(radius) (phi/geom/_sphere.py:69-90);
+    desired_neighbors = volume_from_radius(h) / volume and support = radius_from_volume(volume desired_neighbors)
+    (phi/physics/sph.py:71-98), which rounds to 0.79999995 rather than h = 0.8 in 3-D; the poly6 normalisation const / s ** (d + 6)
+    (:150-156); P = -(45 m) / (pi h^6), V = (45 visc m) / (pi h^6) with m a float32 number."""
+    f32, d, h = np.float32, len(lower), float(smoothing_length)
+    vol = np.asarray(h ** d, f32)
+    if d == 3:
+        volume = f32(4 / 3 * np.pi) * np.power(np.power(f32(.75 / np.pi) * vol, 1 / 3), 3)
+        s = np.power(f32(.75 / np.pi) * (volume * (f32(4 / 3 * np.pi * h ** 3) / volume)), 1 / 3)
+    else:
+        volume = f32(np.pi) * np.power(np.sqrt(vol / f32(np.pi)), 2)
+        s = np.sqrt((volume * (f32(np.pi * h ** 2) / volume)) / f32(np.pi))
+    m = f32(particle_mass)
+    p = _lib.PhiSphParams()
+    for a in range(d):
+        p.lower[a], p.upper[a], p.gravity[a] = f32(lower[a]), f32(upper[a]), f32(gravity[a])
+    p.support, p.smoothing_length, p.mass = f32(s), f32(h), m
+    p.kernel_norm = f32(f32(315 / 64 / np.pi if d == 3 else 4 / np.pi) / np.power(np.asarray(s, f32), d + 6))
+    p.pressure_norm = f32(-(f32(45.0) * m) / f32(np.pi * h ** 6))
+    p.viscous_norm = f32((f32(45.0 * dynamic_visc) * m) / f32(np.pi * h ** 6))
+    p.isotropic_exp, p.base_density, p.dt, p.damping = f32(isotropic_exp), f32(base_density), f32(dt), f32(damping_coef)
+    return p
+
+
+def sph(x: torch.Tensor, v: torch.Tensor, prm: _lib.PhiSphParams, substeps: int = 1, rho: bool = False):
+    """`substeps` substeps of the SPH notebook's apply_bounds(sph_step(v)) in one launch (include/phicuda.h, N12).  x, v: contiguous
+    float32 CUDA tensors (n, dim), dim 2 or 3; prm: sph_params(...).  Returns new tensors (x, v), and with rho=True also the density
+    of the last substep (n,)."""
+    require_cuda()
+    for name, t in (('x', x), ('v', v)):
+        if t.dtype != torch.float32:
+            raise _lib.Unsupported(_lib.ERR_UNSUPPORTED, f"sph: {name} is {t.dtype} (fp32 only)")
+    for name, t in (('x', x), ('v', v)):
+        assert t.is_cuda and t.is_contiguous() and t.dim() == 2, f"sph: {name}: {tuple(t.shape)} is not a contiguous CUDA array (n, dim)"
+    assert x.shape == v.shape, f"sph: x {tuple(x.shape)} and v {tuple(v.shape)} differ"
+    n, d = x.shape
+    lib = _lib.load()
+    xo, vo = torch.empty_like(x), torch.empty_like(v)
+    ro = torch.empty(n, dtype=torch.float32, device=x.device) if rho else None
+    nbytes = lib.phicuda_sph_scratch_bytes(C.c_int64(n), C.c_int32(d), C.byref(prm))
+    scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=x.device)
+    _lib.check(lib.phicuda_sph_f32(_ptr(x), _ptr(v), C.c_int64(n), C.c_int32(d), C.byref(prm), C.c_int32(substeps), _ptr(xo), _ptr(vo),
+                                   _ptr(ro), _ptr(scratch), C.c_size_t(scratch.numel()), _stream()))
+    return (xo, vo, ro) if rho else (xo, vo)
+
+
 def mac_cormack_centered(dom: Domain, vbc, vel, fbc, src, dt: float, correction_strength=1.0, out=None):
     """advect.mac_cormack of a centred field (phi/physics/advect.py:182-215)."""
     require_cuda()

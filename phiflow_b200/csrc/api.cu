@@ -911,6 +911,80 @@ int phicuda_advect_points_f32(const PhiGrid* g, const PhiVBC* vbc, const float* 
                                               trajectory, (cudaStream_t)stream), "advect_points");
 }
 
+// The kernel's SphParams from the public ones; 0 or the error code of the first check that fails.
+static int sph_params(int64_t n, int32_t dim, const PhiSphParams* prm, SphParams* out)
+{
+    if (!prm) { phi_set_error("sph: NULL parameters"); return PHI_ERR_INVALID; }
+    if (dim != 2 && dim != 3) { phi_set_error("sph: dim must be 2 or 3, got %d", dim); return PHI_ERR_INVALID; }
+    if (n < 0 || n > (1 << 30)) { phi_set_error("sph: n must be in [0, 2^30], got %lld", (long long)n); return PHI_ERR_INVALID; }
+    const float scalars[] = {prm->support, prm->smoothing_length, prm->kernel_norm, prm->mass, prm->pressure_norm, prm->viscous_norm,
+                             prm->isotropic_exp, prm->base_density, prm->dt, prm->damping};
+    for (float f : scalars)
+        if (!std::isfinite(f)) { phi_set_error("sph: every parameter must be finite"); return PHI_ERR_INVALID; }
+    if (!(prm->support > 0.f)) { phi_set_error("sph: support must be > 0, got %g", prm->support); return PHI_ERR_INVALID; }
+    SphParams p = {};
+    p.n = (int)n; p.dim = dim;
+    double cells = 1;
+    for (int a = 0; a < dim; ++a) {
+        const float lo = prm->lower[a], up = prm->upper[a];
+        if (!std::isfinite(lo) || !std::isfinite(up) || !std::isfinite(prm->gravity[a]) || !(lo < up)) {
+            phi_set_error("sph: axis %d: lower %g < upper %g and gravity %g must be finite", a, lo, up, prm->gravity[a]); return PHI_ERR_INVALID;
+        }
+        // build_hash_grid in float32: res = max(1, ceil(max(upper - lower, s) / s)), edge = (s res) / res
+        float size = up - lo;
+        if (!(size >= prm->support)) size = prm->support;
+        const float q = std::ceil(size / prm->support);
+        if (!(q < (float)(1 << 30))) { phi_set_error("sph: axis %d needs %g hash cells", a, q); return PHI_ERR_INVALID; }
+        const int r = q < 1.f ? 1 : (int)q;
+        cells *= r;
+        p.res[a] = r;
+        p.lower[a] = lo; p.upper[a] = up;
+        p.cell[a] = (prm->support * (float)r) / (float)r;
+        p.gravity[a] = prm->gravity[a];
+    }
+    if (cells > (double)(1 << 30)) { phi_set_error("sph: %g hash cells exceed 2^30 (the support is too small for the domain)", cells); return PHI_ERR_INVALID; }
+    p.ncells = (int)cells;
+    p.s = prm->support; p.h = prm->smoothing_length; p.norm = prm->kernel_norm; p.m = prm->mass; p.P = prm->pressure_norm;
+    p.V = prm->viscous_norm; p.iso = prm->isotropic_exp; p.base = prm->base_density; p.dt = prm->dt; p.damping = prm->damping;
+    *out = p;
+    return 0;
+}
+
+size_t phicuda_sph_scratch_bytes(int64_t n, int32_t dim, const PhiSphParams* prm)
+{
+    SphParams p;
+    return sph_params(n, dim, prm, &p) ? 0 : phi_sph_scratch_bytes(p);
+}
+
+int phicuda_sph_f32(const float* x, const float* v, int64_t n, int32_t dim, const PhiSphParams* prm, int32_t substeps, float* x_out,
+                    float* v_out, float* rho_out, void* scratch, size_t scratch_bytes, void* stream)
+{
+    // every check runs before the first CUDA call: a refused call leaves x_out, v_out and rho_out untouched
+    SphParams p;
+    CHECK(sph_params(n, dim, prm, &p));
+    if (substeps < 1) { phi_set_error("sph: substeps must be >= 1, got %d", substeps); return PHI_ERR_INVALID; }
+    if (n == 0) return 0;
+    if (!x || !v || !x_out || !v_out || !scratch) { phi_set_error("sph: NULL argument"); return PHI_ERR_INVALID; }
+    const size_t need = phi_sph_scratch_bytes(p);
+    if (scratch_bytes < need) { phi_set_error("sph: scratch %zu < %zu bytes", scratch_bytes, need); return PHI_ERR_INVALID; }
+    const size_t vec = (size_t)n * dim * sizeof(float), sc = (size_t)n * sizeof(float);
+    const void* outs[] = {x_out, v_out, rho_out, scratch};
+    const size_t out_bytes[] = {vec, vec, sc, need};
+    for (int a = 0; a < 4; ++a) {
+        if (!outs[a]) continue;
+        if (overlap(outs[a], out_bytes[a], x, vec) || overlap(outs[a], out_bytes[a], v, vec)) {
+            phi_set_error("sph: an output or the scratch overlaps x or v"); return PHI_ERR_INVALID;
+        }
+        for (int b = a + 1; b < 4; ++b)
+            if (outs[b] && overlap(outs[a], out_bytes[a], outs[b], out_bytes[b])) {
+                phi_set_error("sph: the outputs and the scratch must not overlap each other"); return PHI_ERR_INVALID;
+            }
+    }
+    int max_ctas = SPH_MAX_CTAS;
+    if (const char* e = getenv("PHICUDA_SPH_CTAS")) { const int c = atoi(e); if (c >= 1 && c < max_ctas) max_ctas = c; }   // launch-geometry tests
+    return cuda_fail(phi_launch_sph(p, x, v, x_out, v_out, rho_out, scratch, substeps, max_ctas, (cudaStream_t)stream), "sph");
+}
+
 }  // extern "C"
 
 // ---- N9: fp64 ------------------------------------------------------------------------------------------------------------

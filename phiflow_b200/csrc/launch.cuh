@@ -134,3 +134,15 @@ int phi_launch_julia(const DGrid& g, const float* c, const float* xc, const floa
 // trajectory (steps + 1 entries) written; points_batch / g.batch of 1 broadcast
 int phi_launch_advect_points(const DGrid& g, const DVec& vel, const PhiPointMap& map, const float* points, long long npoints,
                              int points_batch, float dt, int integrator, int steps, float* out, float* traj, cudaStream_t s);
+// N12 SPH (sph_kernels.cu): `substeps` substeps of the SPH notebook's dam break in one cooperative launch.  The hash grid: res[a]
+// cells of edge cell[a] from lower, ncells = prod(res); every other field as PhiSphParams.  x / v (n, dim) in, xo / vo out (no overlap
+// with the inputs); rho: NULL or the density of the last substep.  max_ctas <= SPH_MAX_CTAS caps the grid.
+#define SPH_MAX_CTAS 4096
+struct SphParams {
+    int n, dim, ncells, res[3];
+    float lower[3], upper[3], cell[3];
+    float s, h, m, P, V, norm, iso, base, dt, damping, gravity[3];
+};
+size_t phi_sph_scratch_bytes(const SphParams& p);
+int phi_launch_sph(const SphParams& p, const float* x, const float* v, float* xo, float* vo, float* rho, void* scratch, int substeps,
+                   int max_ctas, cudaStream_t s);

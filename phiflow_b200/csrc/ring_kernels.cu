@@ -21,6 +21,7 @@
 #include <cstdlib>
 #include <cstring>
 #include "launch.cuh"
+#include "persistent.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -68,7 +69,6 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
 // ---- ring state (per thread, registers) ------------------------------------------------------------------------------
 struct SlotIt {                 // a position in the ring: slot index + parity of its current use
@@ -1911,14 +1911,6 @@ int phi_launch_diffuse_implicit(const CgLaunch& l, int C, const DField* cf, cuda
 }
 
 // ---- persistent steppers (N7, N8): every substep of a call in one cooperative launch ------------------------------------------
-// Between two substeps: the generic-proxy stores of one substep must be visible to the TMA (async proxy) loads of the next one, whose
-// halo lines other CTAs wrote - the sequence k_cg_ring uses between passes.
-__device__ __forceinline__ void step_grid_sync(cg::grid_group& grid)
-{
-    fence_proxy_async();
-    grid.sync();
-    fence_proxy_async();
-}
 
 // d0 = s0 and, with TWO, d1 = s1 on every cell of this CTA's units
 template <int DIM, bool TWO>
@@ -2158,20 +2150,27 @@ int phi_step_ring_max_width(const DGrid& g, int kernel)
     return ring_max_width(g, [&](const DGrid& h) { return phi_step_ring_fits(h, kernel); });
 }
 
-// Sets the dynamic shared memory of fn, sizes the grid from its occupancy (at most one CTA per unit) and launches it cooperatively
-// with args.  -100: not even one CTA fits on an SM.  name: the stepper, in the error message of a failed launch.
-static int launch_step_ring(const void* fn, const RingCfg& cfg, void** args, int kernel, bool generic, const char* name, cudaStream_t s)
+int phi_launch_cooperative(const void* fn, int threads, size_t smem, long long max_ctas, void** args, const char* name, cudaStream_t s,
+                           int* grid)
 {
-    const size_t smem = 128 + (size_t)cfg.R * cfg.stage_floats * 4;
     int per_sm = 0;
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, RING_THREADS, smem);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem);
     if (e != cudaSuccess) return (int)e;
     if (per_sm < 1) return -100;
-    int grid = phi_sm_count() * per_sm;
-    if (grid > cfg.total_units) grid = cfg.total_units;
-    e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(RING_THREADS), args, smem, s);
+    const long long fit = (long long)phi_sm_count() * per_sm;
+    *grid = (int)(fit < max_ctas ? fit : max_ctas);
+    e = cudaLaunchCooperativeKernel(fn, dim3(*grid), dim3(threads), args, smem, s);
     if (e != cudaSuccess) { phi_set_error("%s: cooperative launch failed: %s", name, cudaGetErrorString(e)); return (int)e; }
+    return 0;
+}
+
+// A stepper's cooperative launch: the whole ring in shared memory, at most one CTA per unit.
+static int launch_step_ring(const void* fn, const RingCfg& cfg, void** args, int kernel, bool generic, const char* name, cudaStream_t s)
+{
+    int grid = 0;
+    const int e = phi_launch_cooperative(fn, RING_THREADS, 128 + (size_t)cfg.R * cfg.stage_floats * 4, cfg.total_units, args, name, s, &grid);
+    if (e != 0) return e;
     note_ring_launch(kernel, cfg, generic, false, false, grid);
     return 0;
 }

@@ -9,6 +9,7 @@ Mirrored (same names, argument meaning and error behaviour; reference file:line 
     write / read (field.write / field.read: the reference's .npz field files, see field_io.py).
 Fused notebook steps (one kernel launch for all substeps of a call): reaction_diffusion (Reaction_Diffusion), wave_step (Waves).
 Streamlines: streamlines(x0, v, step_size, iterations) returns every position of an advect.points trajectory from one kernel launch.
+SPH: sph_step(x, v, domain, smoothing_length, particle_mass, dt, gravity, substeps=) runs the SPH notebook's substeps in one kernel launch.
 Julia_Set: julia_set(c, iter_count, bounds, x=..., y=...) returns the escape counts as an int32 CenteredGrid in one kernel launch; an
 int32 grid is a result only, which every operator refuses.
 Precision: math.set_global_precision(64) / math.precision(64) make new grids float64 (the Taylor-Green notebook); laplace,
@@ -32,7 +33,7 @@ from . import scene as _scene
 
 __all__ = ['Scene', 'vec', 'batch', 'iterate', 'jit_compile', 'Box', 'Sphere', 'union', 'geom', 'CenteredGrid', 'StaggeredGrid', 'extrapolation', 'ZERO', 'ONE', 'PERIODIC', 'ZERO_GRADIENT',
            'BOUNDARY', 'combine_sides', 'Solve', 'SolveTape', 'NotConverged', 'Diverged', 'ConvergenceException', 'field',
-           'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read', 'wave_step', 'julia_set', 'PI', 'spatial', 'streamlines']
+           'resample', 'advect', 'diffuse', 'fluid', 'math', 'write', 'read', 'wave_step', 'julia_set', 'PI', 'spatial', 'streamlines', 'sph_step']
 
 AXES = 'xyz'
 
@@ -963,6 +964,29 @@ def streamlines(x0, velocity: StaggeredGrid, step_size: float, iterations: int, 
     kind, t, shape = _advect_points(x, velocity, step_size, integrator, iterations, True)
     shape = (iterations + 1,) + ((t.shape[1],) if t.shape[1] > 1 else ()) + shape
     return t.reshape(shape) if kind == 'tensor' else t.cpu().numpy().reshape(shape)
+
+
+def sph_step(x, v, domain: Box, smoothing_length: float, particle_mass: float, dt: float, gravity, dynamic_visc: float = 0.025,
+             isotropic_exp: float = 20., base_density: float = 1., damping_coef: float = -0.95, substeps: int = 1):
+    """The SPH notebook's substep apply_bounds(sph_step(v)) (examples/particles/SPH.ipynb, phi/physics/sph.py) with the poly6 kernel,
+    `substeps` times in one kernel launch (DESIGN.md row N12).  x, v: particle positions and velocities, float32 NumPy arrays or
+    float32 CUDA tensors of one kind and shape (N, d), d = 2 or 3 = the axes of `domain`; gravity: a vec / d numbers.  The support
+    radius comes from smoothing_length as the notebook's desired_neighbors gives it; particle_mass is the notebook's
+    0.01 * mean(volume).  Returns (x, v) of the same kind.  iterate(lambda x, v: sph_step(x, v, ...), batch(t=480), x, v, substeps=40)
+    runs the notebook's loop one substep per call; sph_step(..., substeps=40) runs a frame in one launch."""
+    kx, tx, sx = _as_points(x, len(domain.names))
+    kv, tv, sv = _as_points(v, len(domain.names))
+    d = len(domain.names)
+    _require(kx == kv and kx in ('numpy', 'tensor'), f"sph_step of {kx} positions and {kv} velocities (both float32 NumPy arrays or both "
+                                                     f"float32 CUDA tensors)")
+    _require(len(sx) == 2 and sx == sv and d in (2, 3), f"sph_step of positions {sx} and velocities {sv} in a {d}-D domain ((N, d), d = 2 or 3)")
+    _require(isinstance(gravity, (tuple, list, np.ndarray)) and len(gravity) == d, f"sph_step with gravity {gravity!r} ({d} numbers)")
+    _require(isinstance(substeps, int) and not isinstance(substeps, bool) and substeps >= 1, f"sph_step with substeps = {substeps!r}")
+    prm = ops.sph_params([domain.lower[k] for k in domain.names], [domain.upper[k] for k in domain.names], smoothing_length,
+                         particle_mass, dt, gravity, dynamic_visc, isotropic_exp, base_density, damping_coef)
+    dev = _DEVICE if kx == 'numpy' else tx.device
+    xo, vo = ops.sph(tx.to(dev).contiguous(), tv.to(dev).contiguous(), prm, substeps)
+    return _from_points(kx, xo, sx), _from_points(kv, vo, sv)
 
 
 def _advect(fld, velocity, dt: float, integrator=euler):
